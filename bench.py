@@ -1,11 +1,12 @@
 #!/usr/bin/env python
-"""bench.py — frames/sec of the PL-SLAM front-end hot path (extract + match + pose-LM) on B200.
+"""bench.py — frames/sec of the PL-SLAM front-end hot path (extract + match + pose-LM) on H100.
 
 One "step" = one batch of synthetic frames per GPU through the whole per-frame hot path (ORB extract, undistort, LSD+LBD
 extract, point matching frame k-1 -> k, line matching, 2 x Optimizer::PoseOptimization on the frame's pose problem).
 BASELINE.json metric: "frames/sec (extract+match+pose-LM) 640x480".  Configurations (BASELINE.json `configs`):
 
-  --config tum    (default, the headline)  640x480, TUM1 camera, ORB 1000, B = 4736 frames per GPU, WEAK scaling
+  --config tum    (default, the headline)  640x480, TUM1 camera, ORB 1000, B = 32 frames per SM (4224 on a 132-SM H100) per GPU,
+                  WEAK scaling
   --config kitti  configs[3]: 1241x376, ORB 2000, no distortion, 256 frames sharded over the ranks (contiguous blocks with a
                   1-frame halo, pl-slam_b200/sharding.py), + one LocalBundleAdjustmentWithLine window (20+40 KFs, 3000 points,
                   400 lines) per rank and step; STRONG scaling
@@ -27,6 +28,7 @@ import json
 import os
 import subprocess
 import sys
+import tempfile
 import threading
 import time
 
@@ -41,7 +43,7 @@ N_PTS, N_LINES = 300, 80             # SURVEY.md §8d config 3
 LINES = (200, 0.0)
 KITTI_K = (718.856, 718.856, 607.1928, 185.2157)      # Examples/Monocular/KITTI00-02.yaml:8-11
 CONFIGS = {
-    "tum": dict(W=640, H=480, orb=(1000, 1.2, 8, 20, 7), camera="tum", scaling="weak", batch=4736, lba=False,
+    "tum": dict(W=640, H=480, orb=(1000, 1.2, 8, 20, 7), camera="tum", scaling="weak", lba=False,
                 workload="640x480 synthetic sequence, TUM1 camera: ORB(1000) + undistort + LSD/LBD(200) extract, frame-to-frame point+line "
                          "matching, the 4 projection searches of steady-state tracking (points: last frame 15/30 px + local map; lines: last frame + local map), "
                          "2x PoseOptimization(300 pts + 80 lines)"),
@@ -56,6 +58,7 @@ CONFIGS = {
 W, H = CONFIGS["tum"]["W"], CONFIGS["tum"]["H"]
 ORB = CONFIGS["tum"]["orb"]
 BASE_FRAMES = 64     # distinct host-generated frames; larger batches add per-replica sensor noise (deterministic)
+FRAMES_PER_SM = 32   # tum batch per GPU = SMs x 32: k_lsd_grow_ordered runs one frame per warp, 32 one-warp CTAs resident per SM
 
 
 def camera_of(cfg):
@@ -90,12 +93,19 @@ def make_inputs(B, seed, w=W, h=H, K=None):
 
 
 # ------------------------------------------------------------------------------------------------ CPU oracle arm
+_NATIVE_DIR = None
+
+
 def use_native_oracle():
     """The CPU legs time the -march=native build of the oracle (BASELINE.md §3: -O3 -march=native), compiled on the box that
-    does the timing; the portable build that travels with the repo stays the checker of the tests."""
-    lib = os.path.join(ROOT, "oracle", "liboracle_native.so")
+    does the timing; the portable build that travels with the repo stays the checker of the tests.  The library goes to a temporary
+    directory: the benchmark writes nothing into the tree, which may be read-only."""
+    global _NATIVE_DIR
+    _NATIVE_DIR = _NATIVE_DIR or tempfile.TemporaryDirectory(prefix="plslam_oracle_native_")
+    lib = os.path.join(_NATIVE_DIR.name, "liboracle_native.so")
     try:
-        subprocess.check_call(["make", "-C", os.path.join(ROOT, "oracle"), "-s", "native"], stdout=subprocess.DEVNULL, stderr=subprocess.DEVNULL)
+        subprocess.check_call(["make", "-C", os.path.join(ROOT, "oracle"), "-s", "native", f"NATIVE_LIB={lib}"],
+                              stdout=subprocess.DEVNULL, stderr=subprocess.DEVNULL)
         os.environ["PLSLAM_ORACLE_LIB"] = lib
         return "-O3 -march=native"
     except Exception:
@@ -266,6 +276,7 @@ class Ctx:
         if not torch.cuda.is_available():
             raise SystemExit("bench.py needs a CUDA device: plslam_b200 has no CPU fallback (use --impl reference for the CPU oracle)")
         torch.cuda.set_device(self.local)
+        self.sms = torch.cuda.get_device_properties(self.local).multi_processor_count
         self.dist = None
         self.comm = None
         if self.world > 1:
@@ -307,7 +318,39 @@ class Ctx:
             self.dist.barrier()
 
 
-def run_config(ctx, name, steps, warmup, batch=None, full=True):
+DUMP_FRAMES = 32     # frames of the batch whose per-feature outputs --dump-outputs writes (seeded choice)
+
+
+def dump_outputs(out_dir, fe, B, gathered=None, lba=None):
+    """Write what the last timed step computed as float32 / float64 .npy files under out_dir.  Per-frame scalars and the pose
+    records cover the whole batch; the per-feature arrays (keypoints, descriptors, keylines, matches) cover DUMP_FRAMES frames
+    drawn with a fixed seed, so the files stay small (a few MB) at any batch size."""
+    os.makedirs(out_dir, exist_ok=True)
+    out = fe.fetch(B)
+    trk = fe.fetch_tracking(B)
+    sel = np.sort(np.random.default_rng(0).choice(B, min(B, DUMP_FRAMES), replace=False))
+    arrays = {"sample_frames": sel.astype(np.float64), "n": out["n"], "nl": out["nl"], "n_pt_matches": out["n_pt_matches"],
+              "n_line_matches": out["n_line_matches"], "poses": out["poses"], "inliers": out["inliers"],
+              "track_n_pt": trk["n_pt"], "track_n_line": trk["n_line"]}
+    for f in ("x", "y", "size", "angle", "response", "octave"):
+        arrays["kps_" + f] = out["kps"][sel][f]
+    for f in out["keylines"].dtype.names:
+        arrays["keylines_" + f] = out["keylines"][sel][f]
+    for k in ("desc", "ldesc", "pt_matches", "line_matches"):
+        arrays[k] = out[k][sel]
+    for k in ("pt_match", "line_match"):
+        arrays["track_" + k] = trk[k][sel]
+    if gathered is not None:
+        arrays["gathered_poses"] = gathered.cpu().numpy()
+    if lba is not None:
+        for k in ("kf_Tcw", "pt_Xw", "ln_Xw", "pe_erase", "le_erase"):
+            arrays["lba_" + k] = lba[k]
+    for k, a in arrays.items():
+        a = np.asarray(a)
+        np.save(os.path.join(out_dir, k + ".npy"), a.astype(np.float64 if a.dtype in (np.float64, np.int64) else np.float32))
+
+
+def run_config(ctx, name, steps, warmup, batch=None, full=True, dump_dir=None):
     """One configuration on this process's GPU; returns the measurements (rank-local python values, timings max over ranks)."""
     import plslam_b200 as pl
     from plslam_b200 import synth, sharding
@@ -316,7 +359,7 @@ def run_config(ctx, name, steps, warmup, batch=None, full=True):
     w, h = cfg["W"], cfg["H"]
     K, D = camera_of(cfg)
     if cfg["scaling"] == "weak":
-        B = batch or cfg["batch"]
+        B = batch or ctx.sms * FRAMES_PER_SM
         halo, count, first, total = 0, B, ctx.rank * B, ctx.world * B
         frames, problems = make_inputs(B, 1 + ctx.rank, w, h, K)      # weak scaling: every rank gets its own B frames
     else:
@@ -339,6 +382,7 @@ def run_config(ctx, name, steps, warmup, batch=None, full=True):
     ba = None
     if cfg["lba"]:
         ba = synth.synth_ba_problem(seed=4 + ctx.rank, K=KITTI_K, w=w, h=h)
+    last = {}
 
     def step():
         fe.run_dev(d_frames.data_ptr(), w, w * h, B, ctx.sptr)
@@ -347,7 +391,7 @@ def run_config(ctx, name, steps, warmup, batch=None, full=True):
             send[:count].copy_(poses[halo:halo + count])
             ctx.allgather(send, gathered, max_count * 16)
         if ba is not None:     # LocalMapping's window of this rank (replicas only, SURVEY.md §8e); runs beside the front-end kernels
-            pl.LocalBundleAdjustmentWithLine(ba)
+            last["lba"] = pl.LocalBundleAdjustmentWithLine(ba)
 
     for _ in range(max(warmup, 3)):
         step()
@@ -367,6 +411,8 @@ def run_config(ctx, name, steps, warmup, batch=None, full=True):
         step()
     ev1.record(ctx.stream)
     torch.cuda.synchronize()
+    if dump_dir and ctx.rank == 0:
+        dump_outputs(dump_dir, fe, B, gathered, last.get("lba"))
     ctx.barrier()
     ms = ctx.max_over_ranks(ev0.elapsed_time(ev1))
     launches = pl.launch_count() - launches0
@@ -459,17 +505,13 @@ def cpu_baseline_single_thread(frames, problems):
     cpu = {"value": 1.0 / med, "unit": "frames/s", "cores": 1, "kind": "port",
            "sample": f"median of {len(per)} frames after 5 warm-up frames, one thread, CPU oracle built {flags} (restatement)",
            "ms_per_frame_median": 1000 * med, "ms_per_frame_mean": 1000 * float(np.mean(per))}
-    try:   # cv2 single-thread cross-check recorded in the build container (the GPU box has no cv2): tools/cv2_crosscheck.py
-        cpu["cv2_check"] = json.load(open(os.path.join(ROOT, "profiles", "r02_cpu_crosscheck.json")))
-    except Exception:
-        pass
     return cpu
 
 
 def run_ours(args):
     ctx = Ctx()
     name = args.config
-    res = run_config(ctx, name, args.steps, args.warmup, args.batch, full=True)
+    res = run_config(ctx, name, args.steps, args.warmup, args.batch, full=True, dump_dir=args.dump_outputs)
     cfg = CONFIGS[name]
     latency, extra, cpu = None, None, None
     if ctx.world == 1 and name == "tum":
@@ -487,7 +529,7 @@ def run_ours(args):
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        peak = float(peaks.get("hbm_gbs", 6650.0))
+        peak = float(peaks.get("hbm_gbs", 3350.0))
         achieved = res["grow_bytes"] / (res["grow_ms"] / 1000.0) / 1e9
         if ctx.world == 1 and name == "tum":      # CPU baseline: the oracle, one thread, bounded sample (rank 0, N=1 only)
             cpu = cpu_baseline_single_thread(res["frames"], res["problems"])
@@ -498,7 +540,7 @@ def run_ours(args):
             "dtype": "u8/i32 front-end, f32 descriptors, f64 LM", "data": "synthetic",
             "config": {"workload": cfg["workload"], "name": name, "batch_per_gpu": B, "frames_per_step_total": res["total"], "halo_frames": res["halo"],
                        "frame": res["frame"], "orb": res["orb"], "lines": list(LINES),
-                       "l2": f"inputs {B * res['frame'][0] * res['frame'][1] / 1e6:.0f} MB per step vs the 126 MB L2; every kernel streams a different frame",
+                       "l2": f"inputs {B * res['frame'][0] * res['frame'][1] / 1e6:.0f} MB per step vs the 50 MB L2; every kernel streams a different frame",
                        "predecessor": "frame 0 of a step is matched against the last frame of the previous step (one sequence)",
                        "exchange": "none at 1 GPU; pl_allgather_poses (NCCL) of the [frames][16] pose records per step at N>1",
                        **({"lba_ms": res["lba_ms"], "lba_window": res["lba_window"]} if "lba_ms" in res else {})},
@@ -506,7 +548,7 @@ def run_ours(args):
             "e2e": res["e2e"],
             "roofline": {"kernel": "k_lsd_grow_ordered", "bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s",
                          "frac": achieved / peak, "traffic": None, "ms_per_launch": res["grow_ms"],
-                         "peak_source": "MEASURED_PEAKS.json (of measured)" if peaks else "fallback 6650 GB/s (of fallback)",
+                         "peak_source": "MEASURED_PEAKS.json (of measured)" if peaks else "H100 SXM data sheet, 3350 GB/s (not measured)",
                          "share_of_step": res["grow_ms"] / (res["ms"] / args.steps)},
             "cpu_baseline": cpu,
         }
@@ -514,15 +556,6 @@ def run_ours(args):
             line["latency"] = latency
         if extra:
             line["extra_configs"] = extra
-        traffic_file = os.path.join(ROOT, "profiles", "traffic_k_lsd_grow.json")
-        if os.path.exists(traffic_file):
-            try:
-                tj = json.load(open(traffic_file))     # one `ncu --set full` capture: DRAM bytes per frame of the launch
-                if tj.get("kernel") == "k_lsd_grow_ordered":
-                    line["roofline"]["traffic"] = float(tj["dram_bytes_per_frame"]) * B
-                    line["roofline"]["traffic_source"] = tj.get("source")
-            except Exception:
-                pass
         emit(line)
     if ctx.world > 1:
         ctx.dist.destroy_process_group()
@@ -552,11 +585,14 @@ def main():
     ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=3)
-    ap.add_argument("--batch", type=int, default=None, help="tum: frames per GPU per step (default 4736 = 148 SMs x 32 resident region-growing "
-                                                            "warps); kitti / euroc: total frames per step over all ranks (default 256 / 512)")
+    ap.add_argument("--batch", type=int, default=None, help="tum: frames per GPU per step (default SMs x 32 resident region-growing "
+                                                            "warps, 4224 on H100); kitti / euroc: total frames per step over all ranks (default 256 / 512)")
     ap.add_argument("--config", default="tum", choices=sorted(CONFIGS), help="BASELINE.json configuration (tum = the headline metric)")
     ap.add_argument("--no-extra", action="store_true", help="default run: skip the short kitti / euroc runs")
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step to DIR/<name>.npy (float32 / float64; a seeded sample of the frames "
+                         "for the per-feature arrays)")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

@@ -1,4 +1,4 @@
-/* plslam_b200 — C ABI of the B200-native PL-SLAM front-end / LM hot path.
+/* plslam_b200 — C ABI of the H100-native PL-SLAM front-end / LM hot path.
  *
  * Every entry point replaces one C++ interface of the reference (HarborC/PL-SLAM); the
  * reference has no FFI of its own (SURVEY.md §8b), so these are what a thin C++ class with the
@@ -8,7 +8,7 @@
  * in HBM) plus a cudaStream_t passed as void* (NULL = the handle's own stream) and are
  * asynchronous; the plain variants take HOST pointers, copy in/out and synchronise.
  * Return value: 0 = ok, <0 = error (pl_last_error() gives the text).  There is NO CPU fallback:
- * without a usable sm_100 device every compute entry point fails with PL_ERR_CUDA.
+ * without a usable sm_90 (H100) device every compute entry point fails with PL_ERR_CUDA.
  */
 #ifndef PLSLAM_B200_H
 #define PLSLAM_B200_H

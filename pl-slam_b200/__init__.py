@@ -1,4 +1,4 @@
-"""plslam_b200 — B200-native PL-SLAM front-end / LM hot path (host-side Python mirror).
+"""plslam_b200 — H100-native PL-SLAM front-end / LM hot path (host-side Python mirror).
 
 The product is the C-ABI library libplslam_b200.so (include/plslam_b200.h).  This package is a thin
 ctypes mirror of the reference's operator classes used by the tests and bench.py; it never imports

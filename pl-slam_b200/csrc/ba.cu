@@ -1,4 +1,4 @@
-// Local bundle adjustment with points and line end-points on sm_100a (fp64).
+// Local bundle adjustment with points and line end-points on sm_90a (fp64).
 //
 // Replaces Optimizer::LocalBundleAdjustmentWithLine (reference src/Optimizer.cc:1645-2100; the points-only twin
 // :1308-1642 is the n_line_edges == 0 case) together with the g2o machinery it drives: BlockSolver_6_3 with the Schur
@@ -122,8 +122,8 @@ __device__ double errors_and_chi2(const BAArgs& A, BAShared& S, bool p_robust, b
 }
 
 // one optimizer.optimize(iterations) call on the level-0 edges.  (Unlike k_pose_opt, this kernel is ONE CTA per problem with the SM
-// to itself: keeping the LM loops rolled and this function out of line shrinks it from 81 k to 21 k SASS instructions but costs
-// 28 % - 54.7 -> 70.0 ms on the 20+40-keyframe window - so the inlined, unrolled form stays.)
+// to itself: keeping the LM loops rolled and this function out of line shrinks it from 81 k to 21 k SASS instructions but makes
+// the 20+40-keyframe window markedly slower, so the inlined, unrolled form stays.)
 __device__ int ba_optimize(const BAArgs& A, BAShared& S, int iterations, bool p_robust, bool l_robust, int tid) {
   const double kDeltaMono = (double)(float)sqrt(5.991), kDeltaLine = (double)(float)sqrt(3.84);
   const int n_lm = A.n_pt + 2 * A.n_ln, n_edges = A.n_pe + 2 * A.n_le;
@@ -493,8 +493,8 @@ extern "C" int pl_local_ba(const PLBAProblem* p, const int* stop_flag_dev, float
   int n_free = 0;
   for (int k = 0; k < n_kf; k++) n_free += !p->kf_fixed[k];
   const size_t n = (size_t)n_free * 6;
-  // Device workspace: ONE cached block per process, sub-allocated by a bump pointer (57 cudaMalloc + cudaFree pairs per call cost 2 ms
-  // in a fresh process and over 100 ms inside a process that holds tens of GB of other allocations: cudaFree synchronises and unmaps).
+  // Device workspace: ONE cached block per process, sub-allocated by a bump pointer (57 cudaMalloc + cudaFree pairs per call are
+  // slow inside a process that holds tens of GB of other allocations: cudaFree synchronises and unmaps).
   // Calls are serialised by the mutex (the reference runs one LocalMapping thread); the block only grows.
   static std::mutex ws_mu;
   static char* ws_base = nullptr; static size_t ws_cap = 0; static int ws_dev = -1;

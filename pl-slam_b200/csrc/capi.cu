@@ -32,11 +32,11 @@ int require_device() {
     int major = 0, minor = 0;
     cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
     cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev);
-    state[slot] = (major == 10) ? 1 : -1;
-    if (state[slot] < 0) set_error("device %d is sm_%d%d; this library is built for sm_100a only", dev, major, minor);
+    state[slot] = (major == 9 && minor == 0) ? 1 : -1;
+    if (state[slot] < 0) set_error("device %d is sm_%d%d; this library is built for sm_90a (H100) only", dev, major, minor);
   }
   if (state[slot] < 0) {
-    if (!g_err[0]) set_error("device %d is not sm_100a; this library is built for sm_100a only", dev);
+    if (!g_err[0]) set_error("device %d is not sm_90a; this library is built for sm_90a (H100) only", dev);
     return PL_ERR_CUDA;
   }
   return PL_OK;

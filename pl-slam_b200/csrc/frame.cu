@@ -1,4 +1,4 @@
-// Frame glue around the hot path (SURVEY.md §8f.1), batched on sm_100a:
+// Frame glue around the hot path (SURVEY.md §8f.1), batched on sm_90a:
 //   initUndistortRectifyMap + remap of every frame     Frame::Frame, src/Frame.cc:220-222  (the map is built ONCE per
 //                                                      camera here; the reference rebuilds it for every frame)
 //   Frame::UndistortKeyPoints                          src/Frame.cc:915-945 (cv::undistortPoints, 5 iterations, fp64)

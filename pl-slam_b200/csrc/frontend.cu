@@ -176,9 +176,8 @@ extern "C" int pl_frontend_create(const PLFrontendConfig* cfg, PLFrontend** out)
   FE_CUDA(cudaEventCreateWithFlags(&h->evStart, cudaEventDisableTiming));
   FE_CUDA(cudaEventCreateWithFlags(&h->evLine, cudaEventDisableTiming));
   FE_CUDA(cudaEventCreateWithFlags(&h->evLm, cudaEventDisableTiming));
-  // The three chains run on separate streams (PLSLAM_FRONTEND_OVERLAP=0: one stream).  Round 1 measured no gain (the region
-  // growing filled the step); with the round-2 step the low-occupancy kernels (matchers, quadtree, pose optimisation) fill the
-  // tails of the others: 338.5 -> 327.7 ms per step at B = 4736.  The enqueue order of the chains makes no difference (327-330 ms).
+  // The three chains run on separate streams (PLSLAM_FRONTEND_OVERLAP=0: one stream): the low-occupancy kernels (matchers,
+  // quadtree, pose optimisation) fill the tails of the others.
   { const char* e = getenv("PLSLAM_FRONTEND_OVERLAP"); h->overlap = !(e && e[0] == '0'); }
   if (const char* e = getenv("PLSLAM_FRONTEND_ORDER")) {
     const std::string o(e);

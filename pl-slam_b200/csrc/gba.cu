@@ -1,4 +1,4 @@
-// Global bundle adjustment with points and line end points on sm_100a (fp64), multi-CTA.
+// Global bundle adjustment with points and line end points on sm_90a (fp64), multi-CTA.
 //
 // Replaces Optimizer::BundleAdjustment(vpKFs, vpMP, vpML, nIterations, pbStopFlag, nLoopKF, bRobust) of the reference
 // (src/Optimizer.cc:275-638; GlobalBundleAdjustemnt :41-58 gathers the whole map and calls it) with the g2o machinery behind

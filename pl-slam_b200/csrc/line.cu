@@ -1,4 +1,4 @@
-// Line-feature extraction (LSD segments + LBD descriptors) for batches of frames on sm_100a.
+// Line-feature extraction (LSD segments + LBD descriptors) for batches of frames on sm_90a.
 //
 // Replaces LINEextractor::operator() (reference src/LineExtractor.cpp:26-93) and what it calls:
 //   LSDDetector::detect           opencv_contrib line_descriptor; spec copy Thirdparty/line_descriptor/src/LSDDetector_custom.cpp:56-215
@@ -323,7 +323,7 @@ __global__ void __launch_bounds__(128) k_lsd_scatter(LineParams P, const int* __
 //                                step     every busy lane advances its task by one micro-step (lane_step)
 // Why it is fast where the previous one-warp-per-region kernel was not: a region is a serial chain (one angle update
 // per added pixel), so 32 lanes on ONE region idle; 32 regions on one warp keep all lanes on useful work, and the
-// number of regions in flight (32 x warps) no longer depends on the batch: B = 1 fills the GPU as well as B = 4736.
+// number of regions in flight (32 x warps) no longer depends on the batch: B = 1 fills the GPU as well as a full batch.
 constexpr int kGrowQ = 256;
 constexpr int kCommitBatches = 4;
 constexpr unsigned kGrowWatchdog = 6u * 1000u * 1000u;
@@ -851,11 +851,11 @@ struct PLLine {
   float2* d_seedcs = nullptr;
   // region growing (lsd_grow_core.cuh): pixel records, status words, list pool, control words, lane buffers, weight table
   lg::Params GP;
-  int grow_warps_target = 148 * 16;   // warps the grow kernel spreads over the GPU when the batch is small (env PLSLAM_LSD_GROW_WARPS)
+  int grow_warps_target = 132 * 16;   // warps the grow kernel spreads over the GPU when the batch is small (env PLSLAM_LSD_GROW_WARPS)
   int grow_wpf_max = 64;              // at most this many warps on one frame (env PLSLAM_LSD_GROW_WPF)
   // batches up to this size use the speculative kernel, larger ones the ordered one (env PLSLAM_LSD_GROW_SPEC_MAXB).  Default 0:
-  // measured on B200 (DESIGN.md §6) the speculative kernel wins on frames made of many small regions (single raw frame 51 vs 95 ms)
-  // and loses on frames whose long, refine-heavy regions form a dependency chain (single undistorted TUM frame: 1.4x slower)
+  // the speculative kernel wins on frames made of many small regions (DESIGN.md §6)
+  // and loses on frames whose long, refine-heavy regions form a dependency chain
   int grow_spec_max_batch = 0;
   size_t lane_warps = 0;              // lane buffers are allocated for this many warps
   int4* d_rec = nullptr; int* d_sq = nullptr;
@@ -930,7 +930,7 @@ extern "C" int pl_line_create(const PLLineConfig* cfg, PLLine** out) {
   LN_TRY(dev_alloc(&h->d_scaled, npx * B)); LN_TRY(dev_alloc(&h->d_seedcs, npx * B)); LN_TRY(dev_alloc(&h->d_rec, npx * B));
   LN_TRY(dev_alloc(&h->d_sq, npx * B));
   {  // speculative region growing: geometry of the run-time structures
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     h->grow_warps_target = sms * 16;
     if (const char* e = getenv("PLSLAM_LSD_GROW_WARPS")) { const int v = atoi(e); if (v > 0) h->grow_warps_target = v; }

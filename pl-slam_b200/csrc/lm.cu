@@ -1,4 +1,4 @@
-// Pose-only Levenberg–Marquardt for batches of frames on sm_100a (fp64).
+// Pose-only Levenberg–Marquardt for batches of frames on sm_90a (fp64).
 //
 // Replaces Optimizer::PoseOptimization / PoseOptimizationWithPoints / PoseOptimizationWithLines
 // (reference src/Optimizer.cc:640-1284) and the g2o machinery they drive: OptimizationAlgorithmLevenberg::solve
@@ -150,8 +150,8 @@ __global__ void __launch_bounds__(LM_THREADS) k_pose_opt(PoseArgs A) {
   };
 
   int nBadPts = 0, nBadLines = 0, total_its = 0;
-  // The loops are NOT unrolled on purpose: unrolled and unswitched on the two robust flags the kernel grew to 147 k SASS
-  // instructions (2.3 MB) and stalled 12 cycles per issue on instruction fetch (profiles/r02_k_pose_opt.md).
+  // The loops are NOT unrolled on purpose: unrolled and unswitched on the two robust flags the kernel grows to ~150 k SASS
+  // instructions (over 2 MB of code) and stalls on instruction fetch.
 #pragma unroll 1
   for (int round = 0; round < 4; round++) {
     // ---- optimizer.optimize(10) on the level-0 edges, starting from the frame's initial pose

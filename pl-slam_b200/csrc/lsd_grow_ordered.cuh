@@ -22,7 +22,7 @@ namespace ord {
 using lg::kDegToRads;
 using lg::kPI;
 // recent queue entries in shared memory; older ones are re-read from the region list in global memory (L1 hits).  The L1 share matters
-// more than the ring: B = 4736, 512 entries 190.5 ms -> 256 entries 184.0 (earlier build); this build 256: 159.3, 128: 160.1, 64: 156.7, 32: 157.0, 16: 157.0
+// more than the ring: a small ring leaves more of the SM's shared memory / L1 split to L1
 #ifndef PL_GROW_RING
 #define PL_GROW_RING 64
 #endif
@@ -152,7 +152,7 @@ __device__ __forceinline__ int region_grow(const Ctx& C, unsigned seed, double p
     if (live == 0u) continue;
     GSTAT(2, 1);
     // lanes that name the same pixel (a free pixel sits in up to four of the 3x3 windows of one step); invalid lanes are unique
-    // (skipping the MATCH when a single entry is expanded - its 8 neighbours are distinct - measured 2.6 % SLOWER: 160.7 -> 164.8 ms)
+    // (skipping the MATCH when a single entry is expanded - its 8 neighbours are distinct - was measured slower)
     const unsigned dups = __match_any_sync(0xffffffffu, pk);
     unsigned acc = 0u;                                 // lanes accepted in this step, in order
     const int cnt0 = cnt;
@@ -200,7 +200,7 @@ __device__ __forceinline__ int region_grow(const Ctx& C, unsigned seed, double p
     }
     __syncwarp();
   }
-  // 63 % of the regions end below need_n and their angle is never read (B = 4736: 160.7 -> 158.9 ms, byte-identical)
+  // most regions end below need_n and their angle is never read
   if (dirty && cnt >= need_n) reg_angle = (double)lg::fast_atan2_deg(sumdy, sumdx) * kDegToRads;
   reg_angle_out = reg_angle;
   return cnt;
@@ -212,7 +212,7 @@ __device__ __noinline__ int region_grow_cold(const Ctx& C, unsigned seed, double
 // region2rect + get_theta: sums in list order (see the header), extents by exact max / min
 __device__ __forceinline__ double pixel_weight(const Ctx& C, int px, int py) {
   // the gradient magnitude sqrt((gx^2 + gy^2) / 4) of the reference from the integer sum of squares, through the table of
-  // exact square roots (an in-kernel fp64 sqrt measured 9 ms slower at B = 4736)
+  // exact square roots (cheaper than an in-kernel fp64 sqrt)
   return __ldg(&C.wtab[__ldg(&C.SQ[C.fb + (unsigned)(py * C.sw + px)])]);
 }
 __device__ __noinline__ void region2rect(const Ctx& C, int n, double reg_angle, double prec, RectD& rec, int lane) {
@@ -412,9 +412,9 @@ __device__ __noinline__ bool refine(const Ctx& C, int& n, double reg_angle, doub
 
 }  // namespace ord
 
-// One warp per frame; grid = frames (32 one-warp CTAs resident per SM: 4736 frames in one wave on 148 SMs).
+// One warp per frame; grid = frames (32 one-warp CTAs resident per SM: 4224 frames in one wave on the 132 SMs of an H100).
 // kPre: examine the neighbourhoods of a whole batch of seeds up front (see below): fewer dependent round trips per frame, but
-// more requests - it pays when the GPU is not full of frames (measured: B = 1 88 -> 81 ms, B = 4736 +7 %).
+// more requests - it pays when the GPU is not full of frames (small batches) and costs when it is.
 template <bool kPre>
 __global__ void __launch_bounds__(32, 32) k_lsd_grow_ordered(LineParams P, int4* __restrict__ REC, const int* __restrict__ SQ, const float2* __restrict__ seedcs,
                                                              const unsigned* __restrict__ order, const int* __restrict__ ndef,
@@ -457,7 +457,7 @@ __global__ void __launch_bounds__(32, 32) k_lsd_grow_ordered(LineParams P, int4*
         single = !any;
         prefetch_l2(&C.S2[C.fb + (unsigned)pidx]);
       }
-#ifndef PL_GROW_NOPF                          // (without these prefetches: 159.0 -> 162.2 ms at B = 4736)
+#ifndef PL_GROW_NOPF                          // (PL_GROW_NOPF builds without these prefetches, for A/B timing)
       if (!kPre && ((todo >> lane) & 1u)) {   // this batch's seeds that will grow: their seed record and 3x3 rows into L2
         prefetch_l2(&C.S2[C.fb + (unsigned)pidx]);
         const int up = max(pidx - P.sw, 1), dn = min(pidx + P.sw, P.npx - 2);

@@ -1,4 +1,4 @@
-// Descriptor matching for batches of frames on sm_100a.
+// Descriptor matching for batches of frames on sm_90a.
 //
 // Replaces (reference file:line)
 //   ORBmatcher::DescriptorDistance / LSDmatcher::DescriptorDistance   ORBmatcher.cc:1764-1780, LSDmatcher.cpp:654-670

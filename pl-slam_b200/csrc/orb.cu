@@ -1,4 +1,4 @@
-// ORB extraction for batches of frames on sm_100a.
+// ORB extraction for batches of frames on sm_90a.
 //
 // Replaces ORB_SLAM2::ORBextractor (reference src/ORBextractor.cc).  Kernel map (DESIGN.md §3):
 //   k_resize_level   ComputePyramid         :1107-1132  (cv::resize INTER_LINEAR, 11-bit fixed point)
@@ -140,7 +140,7 @@ __host__ __device__ __forceinline__ int fast_score_px(const uint8_t* p, int pitc
 }
 
 // Two horizontally adjacent pixels per thread in the two 16-bit halves of a register (s16x2).  The 16 circle differences
-// d[k] = ring[k] - centre are signed 9-bit values: they fit a half exactly, and sm_100a has single-instruction packed 16-bit
+// d[k] = ring[k] - centre are signed 9-bit values: they fit a half exactly, and sm_90a has single-instruction packed 16-bit
 // add and 3-input min / max (VIADD.16x2, VIMNMX3.S16x2 - the DPX family), so
 //   m9[k] = min(d[k .. k+8]) = min3(m3[k], m3[k+3], m3[k+6]),  m3[k] = min3(d[k], d[k+1], d[k+2])      (32 instructions)
 //   M9[k] = max(d[k .. k+8]) likewise                                                                  (32 instructions)

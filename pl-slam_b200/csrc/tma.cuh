@@ -1,9 +1,7 @@
-// Tensor Memory Accelerator helpers (sm_100a): mbarrier + bulk asynchronous copies global -> shared memory.
+// Tensor Memory Accelerator helpers (sm_90a): mbarrier + bulk asynchronous copies global -> shared memory.
 // Image tiles are staged as one bulk copy per tile row (cp.async.bulk, SASS UBLKCP) that all complete one mbarrier.  The
-// tensor-map form (cp.async.bulk.tensor, UTMALDG) would fetch a whole 2-D tile with one instruction, but on this pool's
-// B200 boxes (driver 580.159) it raises "illegal instruction" in every form tried - descriptor in param or global memory,
-// 2-D / 3-D, u8 / u32 elements, with and without a cluster launch attribute - while the 1-D bulk copy with the same
-// mbarrier code works: tools/probe/tma_probe.cu is the reproducer, profiles/r02_tma_probe.md the record.
+// tensor-map form (cp.async.bulk.tensor, UTMALDG) would fetch a whole 2-D tile with one instruction and needs a tensor map per
+// image; tools/probe/tma_probe.cu tries its forms on the GPU at hand.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -1,6 +1,6 @@
 // ORBmatcher / LSDmatcher / Optimizer of the reference (src/ORBmatcher.cc, src/LSDmatcher.cpp, src/Optimizer.cc), SAME
 // signatures, on the plslam_b200 C ABI: every method gathers the members the reference's loop reads into flat arrays,
-// calls one pl_* entry point (one kernel launch on the B200), and writes the members the reference's loop writes.
+// calls one pl_* entry point (one kernel launch on the GPU), and writes the members the reference's loop writes.
 // In the reference tree: compile with -DPLSLAM_IN_REFERENCE_TREE (real Frame.h ... are included through reference_glue.h)
 // IN PLACE of src/ORBmatcher.cc / LSDmatcher.cpp / Optimizer.cc for these methods; here: against reference_mock.h, driven
 // by tests/host/glue_track.cpp through TrackWithMotionModel's call sequence (Tracking.cc:1345-1372) and checked against the

@@ -6,7 +6,7 @@ import numpy as np, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import plslam_b200 as pl
 from plslam_b200 import synth
-B = int(os.environ.get("B", 4736)); W, H = 640, 480
+B = int(os.environ.get("B", 4224)); W, H = 640, 480
 base = synth.synth_sequence(64, W, H, seed=1)
 rng = np.random.Generator(np.random.PCG64(78))
 frames = np.empty((B, H, W), np.uint8)

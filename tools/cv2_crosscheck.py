@@ -1,6 +1,6 @@
 """BASELINE.md §3.2 cross-check of the CPU denominator: the per-frame hot path built from cv2 primitives (single thread,
-cv2.setNumThreads(1)) next to the C++ oracle (one thread), stage by stage, on the bench frames.  cv2 exists only in the BUILD
-container (the GPU box has none), so the result is recorded in profiles/r02_cpu_crosscheck.{json,md} and bench.py quotes it.
+cv2.setNumThreads(1)) next to the C++ oracle (one thread), stage by stage, on the bench frames.  It needs the cv2 Python
+package, which nothing else on the benchmark path does; the result is printed as JSON.
 Stages without a cv2 counterpart (LBD: opencv_contrib is not in the wheel; the pose LM: g2o) are timed on the oracle only."""
 import json, os, sys, time
 import numpy as np
@@ -62,7 +62,5 @@ cv_equiv = st["cv2"][next(iter(st["cv2"]))] + st["cv2"]["remap"] + st["cv2"]["ls
     st["oracle"]["match (SearchForInitialization + SearchDouble)"] + st["oracle"]["2x pose_optimization"]
 out = {"host": f"{os.cpu_count()} cores (build container), one thread, median of {N - 5} frames after 5 warm-up", "cv2_version": cv2.__version__,
        "ms_per_frame": st, "oracle_total_ms": or_sum, "cv2_primitives_plus_oracle_lbd_match_lm_ms": cv_equiv,
-       "oracle_over_cv2": or_sum / cv_equiv,
-       "reading": "see profiles/r02_cpu_crosscheck.md"}
-json.dump(out, open(os.path.join(os.path.dirname(__file__), "..", "profiles", "r02_cpu_crosscheck.json"), "w"), indent=1)
+       "oracle_over_cv2": or_sum / cv_equiv}
 print(json.dumps(out, indent=1))

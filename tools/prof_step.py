@@ -6,7 +6,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import bench
 import plslam_b200 as pl
 from plslam_b200 import synth
-ap = argparse.ArgumentParser(); ap.add_argument("--batch", type=int, default=4736); ap.add_argument("--steps", type=int, default=4)
+ap = argparse.ArgumentParser(); ap.add_argument("--batch", type=int, default=4224); ap.add_argument("--steps", type=int, default=4)
 a = ap.parse_args()
 B = a.batch
 K, D = bench.camera_of(bench.CONFIGS["tum"])

@@ -7,7 +7,7 @@ import bench
 import plslam_b200 as pl
 
 ap = argparse.ArgumentParser()
-ap.add_argument("--batch", type=int, default=4736); ap.add_argument("--steps", type=int, default=4)
+ap.add_argument("--batch", type=int, default=4224); ap.add_argument("--steps", type=int, default=4)
 ap.add_argument("--warmup", type=int, default=2); ap.add_argument("--tag", default="")
 a = ap.parse_args()
 B = a.batch
