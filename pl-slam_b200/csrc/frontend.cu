@@ -91,6 +91,7 @@ struct PLFrontend {
   cudaStream_t sLine = nullptr, sLm = nullptr;      // side streams: LSD/LBD chain and the LM run beside the ORB chain
   cudaEvent_t evStart = nullptr, evLine = nullptr, evLm = nullptr;
   int overlap = 0;
+  int serial_batch = 0;          // batches of at least this many frames run the three chains on one stream (see pl_frontend_create)
   int B = 0, capK = 0, capL = 0;
   // device-resident per-batch state
   uint8_t* d_img = nullptr;
@@ -177,8 +178,17 @@ extern "C" int pl_frontend_create(const PLFrontendConfig* cfg, PLFrontend** out)
   FE_CUDA(cudaEventCreateWithFlags(&h->evLine, cudaEventDisableTiming));
   FE_CUDA(cudaEventCreateWithFlags(&h->evLm, cudaEventDisableTiming));
   // The three chains run on separate streams (PLSLAM_FRONTEND_OVERLAP=0: one stream): the low-occupancy kernels (matchers,
-  // quadtree, pose optimisation) fill the tails of the others.
+  // quadtree, pose optimisation) fill the tails of the others.  Not from 32 frames per SM on: there k_lsd_grow_ordered is one
+  // wave of one-warp CTAs that holds all 32 block slots and the whole register file of every SM, so the other chains are only
+  // placed in its tail, where they slow the grow's last frames by more than they gain (DESIGN.md §7: 402 ms with three streams,
+  // 392 ms with one, at 4224 frames on an H100).
   { const char* e = getenv("PLSLAM_FRONTEND_OVERLAP"); h->overlap = !(e && e[0] == '0'); }
+  {
+    int dev = 0, sms = 132;
+    FE_CUDA(cudaGetDevice(&dev));
+    FE_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    h->serial_batch = 32 * sms;
+  }
   if (const char* e = getenv("PLSLAM_FRONTEND_ORDER")) {
     const std::string o(e);
     if (o.size() == 3 && o.find('L') != std::string::npos && o.find('O') != std::string::npos && o.find('M') != std::string::npos) memcpy(h->order, o.data(), 3);
@@ -311,8 +321,9 @@ extern "C" int pl_frontend_run_dev(PLFrontend* h, const uint8_t* imgs, int strid
   const size_t cp = h->cfg.lm_cap_points, cl = h->cfg.lm_cap_lines;
   // Three independent chains, like the reference's per-frame std::threads (Frame.cc:224-227): the line chain (LSD grow is
   // latency bound and leaves issue slots free), the ORB + point-matching chain, and the two pose optimisations.
-  cudaStream_t sL = h->overlap ? h->sLine : st, sM = h->overlap ? h->sLm : st;
-  if (h->overlap) {
+  const bool overlap = h->overlap && B < h->serial_batch;
+  cudaStream_t sL = overlap ? h->sLine : st, sM = overlap ? h->sLm : st;
+  if (overlap) {
     PL_CUDA(cudaEventRecord(h->evStart, st));
     PL_CUDA(cudaStreamWaitEvent(sL, h->evStart, 0));
     PL_CUDA(cudaStreamWaitEvent(sM, h->evStart, 0));
@@ -406,7 +417,7 @@ extern "C" int pl_frontend_run_dev(PLFrontend* h, const uint8_t* imgs, int strid
     rc = *o == 'L' ? line_chain() : *o == 'O' ? orb_chain() : lm_chain();
     if (rc) return rc;
   }
-  if (h->overlap) {
+  if (overlap) {
     PL_CUDA(cudaEventRecord(h->evLine, sL));
     PL_CUDA(cudaEventRecord(h->evLm, sM));
     PL_CUDA(cudaStreamWaitEvent(st, h->evLine, 0));
