@@ -143,7 +143,9 @@ int pl_lsd_search_double_dev(const uint8_t* d1, const int* n1, const uint8_t* d2
  * per matched point i: pt_obs = mvKeysUn[i].pt, pt_inv_sigma2 = mvInvLevelSigma2[octave], pt_Xw = GetWorldPos();
  * per matched line i: line_func = mvKeyLineFunctions[i] (3 doubles), line_Xw = MapLine::mWorldPos (6 doubles).
  * Outputs: optimised Tcw, mvbOutlier / mvbLineOutlier flags.  Returns the reference's return value
- * (inlier count; 0 and an untouched pose when fewer than 3 correspondences) or an error < 0.               */
+ * (inlier count; 0 and an untouched pose when fewer than 3 correspondences) or an error < 0.
+ * Mode 1 writes only pt_outlier and mode 2 only line_outlier (the other mask is left as the caller passed it, like the
+ * reference's WithPoints / WithLines); the same holds per problem for the [B][cap] masks of pl_pose_optimization_dev. */
 int pl_pose_optimization(int mode, const float* Tcw_in, const float* K, int n_points, const float* pt_obs,
                          const float* pt_inv_sigma2, const float* pt_Xw, int n_lines, const double* line_func,
                          const double* line_Xw, float* Tcw_out, uint8_t* pt_outlier, uint8_t* line_outlier,
@@ -209,7 +211,9 @@ typedef struct PLFrontend PLFrontend;
 int pl_frontend_create(const PLFrontendConfig* cfg, PLFrontend** out);
 void pl_frontend_destroy(PLFrontend* h);
 int pl_frontend_capacities(const PLFrontend* h, int* cap_keypoints, int* cap_lines);
-/* upload the batch's pose problems (host pointers, [B][cap] layouts as in pl_pose_optimization_dev) */
+/* upload the batch's pose problems (host pointers, [B][cap] layouts as in pl_pose_optimization_dev); PL_ERR_ARG if a count is
+ * negative or any n_points[b] > lm_cap_points or n_lines[b] > lm_cap_lines (nothing is uploaded then; the same holds for the
+ * _async form) */
 int pl_frontend_set_pose_problems(PLFrontend* h, int B, const float* Tcw0, const float* K, const int* n_points,
                                   const float* pt_obs, const float* pt_inv_sigma2, const float* pt_Xw, const int* n_lines,
                                   const double* line_func, const double* line_Xw);
@@ -341,7 +345,7 @@ int pl_lsd_search_by_projection_lines(const void* keylines, const double* linefu
  * host-pointer functions above are their B = 1 case.  gate_nmatches / gate_min: frame b runs only if gate_nmatches[b] < gate_min
  * (the "fill(mvpMapPoints, NULL); search again with 2 * th" retry of Tracking.cc:1352-1357); NULL = every frame runs. */
 int pl_orb_search_by_projection_last_dev(const PLKeyPoint* keys_cur, const uint8_t* desc_cur, const int* n_cur, int cap, int B,
-                                         const float* bounds, const float* Tcw /*[B][16]*/, const float* K /*[4]*/,
+                                         const float* bounds, const float* Tcw /*[B][16]*/, const float* K /*[B][4]*/,
                                          const float* scale_factors, int nlevels, const int* n_last, int cap_last,
                                          const uint8_t* last_valid, const float* last_pos, const uint8_t* last_desc,
                                          const int* last_octave, const float* last_angle, float th, int check_orientation,

@@ -495,7 +495,12 @@ def search_double(d1, d2, nnratio=0.7, impl="oracle"):
 
 
 # ---------------------------------------------------------------------------------------------- pose-only LM
-def pose_optimization(mode, Tcw, K, pt_obs, pt_inv_sigma2, pt_Xw, line_func, line_Xw):
+POSE_VARIANTS = {"reference": 0, "jac_5e8": 1, "device_order": 2, "device_order_jac_5e8": 3}
+
+
+def pose_optimization(mode, Tcw, K, pt_obs, pt_inv_sigma2, pt_Xw, line_func, line_Xw, variant="reference"):
+    """variant: "reference", or a rounding variant (oracle_lm.cpp, oracle_pose_optimization_ex): the line Jacobian scaled by 5e8
+    (k_pose_opt's literal) instead of g2o's 1 / (2 * 1e-9), and / or the sums formed in k_pose_opt's order."""
     Tcw = np.ascontiguousarray(Tcw, np.float32); K = np.ascontiguousarray(K, np.float32)
     po = np.ascontiguousarray(pt_obs, np.float32).reshape(-1, 2); pw = np.ascontiguousarray(pt_inv_sigma2, np.float32)
     px = np.ascontiguousarray(pt_Xw, np.float32).reshape(-1, 3)
@@ -503,11 +508,17 @@ def pose_optimization(mode, Tcw, K, pt_obs, pt_inv_sigma2, pt_Xw, line_func, lin
     Tout = np.zeros((4, 4), np.float32)
     pout = np.zeros(max(len(po), 1), np.uint8); lout = np.zeros(max(len(lf), 1), np.uint8)
     its = C.c_int(0)
-    f = lib().oracle_pose_optimization
-    f.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
-                  C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-    n = f(mode, _p(Tcw), _p(K), len(po), _p(po), _p(pw), _p(px), len(lf), _p(lf), _p(lx), _p(Tout), _p(pout), _p(lout),
-          C.byref(its))
+    args = [C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
+            C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    a = (mode, _p(Tcw), _p(K), len(po), _p(po), _p(pw), _p(px), len(lf), _p(lf), _p(lx), _p(Tout), _p(pout), _p(lout), C.byref(its))
+    if variant == "reference":
+        f = lib().oracle_pose_optimization
+        f.argtypes = args
+        n = f(*a)
+    else:
+        f = lib().oracle_pose_optimization_ex
+        f.argtypes = args + [C.c_int]
+        n = f(*a, POSE_VARIANTS[variant])
     return n, Tout, pout[:len(po)].astype(bool), lout[:len(lf)].astype(bool), its.value
 
 
@@ -570,23 +581,29 @@ def line_extract(img, mask=None, nfeatures=200, min_line_length=0.0, order_mode=
 
 
 # ---------------------------------------------------------------------------------------------- local BA
-def local_ba(p, stop_flag=None):
-    """p: dict from synth.synth_ba_problem.  Returns dict(kf_Tcw, pt_Xw, ln_Xw, pe_erase, le_erase, le_erase_kf, its)."""
+LINE_CAMERAS = {"reference": 0, "end_observing_K": 1, "start_K_end": 2}
+
+
+def local_ba(p, stop_flag=None, line_cameras="reference"):
+    """p: dict from synth.synth_ba_problem.  Returns dict(kf_Tcw, pt_Xw, ln_Xw, pe_erase, le_erase, le_erase_kf, its).
+    line_cameras: "reference" (start points with the observing keyframe's K, end points with K_end, Optimizer.cc:1939-1942), or
+    one of the wrong models a test must be able to tell from it: "end_observing_K", "start_K_end".
+    gate_gap: the smallest relative distance of any edge's chi2 from its gate at the two classifications (inf if none ran)."""
     n_kf, n_pt, n_ln, n_pe, n_le = len(p["kf_fixed"]), len(p["pt_Xw"]), len(p["ln_Xw"]), len(p["pe_kf"]), len(p["le_kf"])
     out = dict(kf_Tcw=np.zeros((n_kf, 16), np.float32), pt_Xw=np.zeros((max(n_pt, 1), 3), np.float32),
                ln_Xw=np.zeros((max(n_ln, 1), 6), np.float64), pe_erase=np.zeros(max(n_pe, 1), np.uint8),
                le_erase=np.zeros(max(n_le, 1), np.uint8), le_erase_kf=np.zeros(max(n_le, 1), np.int32))
-    its = C.c_int(0)
+    its = C.c_int(0); gap = C.c_double(0)
     sf = None if stop_flag is None else np.ascontiguousarray(stop_flag, np.int32)
     f = lib().oracle_local_ba
     f.argtypes = [C.c_int] + [C.c_void_p] * 4 + [C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int] + [C.c_void_p] * 4 + \
-                 [C.c_int] + [C.c_void_p] * 3 + [C.c_void_p] * 8
+                 [C.c_int] + [C.c_void_p] * 3 + [C.c_void_p] * 8 + [C.c_int, C.c_void_p]
     a = {k: np.ascontiguousarray(v) for k, v in p.items() if isinstance(v, np.ndarray)}
     f(n_kf, _p(a["kf_Tcw"]), _p(a["kf_fixed"]), _p(a["kf_K"]), _p(a["K_end"]), n_pt, _p(a["pt_Xw"]), n_ln, _p(a["ln_Xw"]), n_pe,
       _p(a["pe_kf"]), _p(a["pe_pt"]), _p(a["pe_obs"]), _p(a["pe_inv_sigma2"]), n_le, _p(a["le_kf"]), _p(a["le_ln"]), _p(a["le_func"]),
       _p(sf), _p(out["kf_Tcw"]), _p(out["pt_Xw"]), _p(out["ln_Xw"]), _p(out["pe_erase"]), _p(out["le_erase"]),
-      _p(out["le_erase_kf"]), C.byref(its))
-    out["its"] = its.value
+      _p(out["le_erase_kf"]), C.byref(its), LINE_CAMERAS[line_cameras], C.byref(gap))
+    out["its"] = its.value; out["gate_gap"] = gap.value
     for k, n in (("pt_Xw", n_pt), ("ln_Xw", n_ln), ("pe_erase", n_pe), ("le_erase", n_le), ("le_erase_kf", n_le)):
         out[k] = out[k][:n]
     return out

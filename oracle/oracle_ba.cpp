@@ -21,6 +21,7 @@
 // :278); every line edge uses the OBSERVING keyframe's intrinsics (:472-475,526-529); edges are inserted points first, then
 // all start-point edges, then all end-point edges (:321-536).
 
+#include <algorithm>
 #include <cmath>
 #include <cstdint>
 #include <cstring>
@@ -78,6 +79,7 @@ struct BA {
   double info_line = 0.5;           // invSigma = 0.5 (Optimizer.cc:1647)
   double delta_p = kDeltaMono, delta_l = kDeltaLine;
   bool end_uses_Kend = true;        // local BA quirk (Optimizer.cc:1939-1942); global BA: the observing keyframe's own K
+  bool start_uses_Kend = false;     // never in the reference: a deliberately wrong camera model for the tests (see oracle_local_ba)
   bool starts_first = false;        // global BA inserts all start-point edges, then all end-point edges
   volatile const int* stop = nullptr;
   int n_lm() const { return n_pt + 2 * n_ln; }
@@ -95,7 +97,8 @@ void point_err(const BA& P, const SE3& T, const double* X, int e, double* out) {
 double line_err(const BA& P, const SE3& T, const double* X, int e, int end) {
   double c[3], k[4], u, v;
   se3_map(T, X, c);
-  if (end == 0 || !P.end_uses_Kend) Kd(P.K, P.le_kf[e], k); else for (int i = 0; i < 4; i++) k[i] = P.Kend[i];
+  const bool use_Kend = end == 0 ? P.start_uses_Kend : P.end_uses_Kend;
+  if (!use_Kend) Kd(P.K, P.le_kf[e], k); else for (int i = 0; i < 4; i++) k[i] = P.Kend[i];
   cam(c, k, u, v);
   const double* l = P.le_f + 3 * e;
   return l[0] * u + l[1] * v + l[2];
@@ -314,11 +317,17 @@ extern "C" int oracle_local_ba(int n_kf, const float* kf_Tcw, const uint8_t* kf_
                                const int* pe_pt, const float* pe_obs, const float* pe_inv_sigma2, int n_le, const int* le_kf,
                                const int* le_ln, const double* le_func, const int* stop_flag, float* kf_Tcw_out,
                                float* pt_Xw_out, double* ln_Xw_out, uint8_t* pe_erase, uint8_t* le_erase, int* le_erase_kf,
-                               int* iterations_out) {
+                               int* iterations_out, int line_cameras, double* gate_gap) {
+  // line_cameras: 0 = the reference (start points: observing keyframe's K, end points: K_end).  The tests' "wrong camera"
+  // models, which an implementation must be told apart from: 1 = end points with the observing K, 2 = start points with K_end.
+  // gate_gap (may be NULL): the smallest relative distance |chi2 - gate| / gate of any edge from its chi2 gate (5.991 points,
+  // 3.84 line end points) at the two classifications; an implementation that sums in another order can only agree on the
+  // masks if this is well above rounding level.
   BA P;
   P.n_kf = n_kf; P.n_pt = n_pt; P.n_ln = n_ln; P.n_pe = n_pe; P.n_le = n_le;
   P.T.resize(n_kf); P.fixed.assign(kf_fixed, kf_fixed + n_kf); P.K = kf_K;
   for (int i = 0; i < 4; i++) P.Kend[i] = (double)K_end[i];
+  P.end_uses_Kend = line_cameras != 1; P.start_uses_Kend = line_cameras == 2;
   for (int k = 0; k < n_kf; k++) P.T[k] = se3_from_cv(kf_Tcw + 16 * k);
   P.X.resize((size_t)3 * (n_pt + 2 * n_ln));
   for (int i = 0; i < 3 * n_pt; i++) P.X[i] = (double)pt_Xw[i];
@@ -328,6 +337,8 @@ extern "C" int oracle_local_ba(int n_kf, const float* kf_Tcw, const uint8_t* kf_
   P.p_lvl.assign(n_pe + 1, 0); P.l_lvl.assign(n_le + 1, 0);
   P.stop = stop_flag;
   int its = 0;
+  double gap = std::numeric_limits<double>::infinity();
+  auto near = [&](double c2, double gate) { gap = std::min(gap, std::fabs(c2 - gate) / gate); };
   if (!(stop_flag && *stop_flag)) {
     its += optimize(P, 5);
     bool more = !(stop_flag && *stop_flag);
@@ -336,11 +347,13 @@ extern "C" int oracle_local_ba(int n_kf, const float* kf_Tcw, const uint8_t* kf_
         double w = (double)pe_inv_sigma2[e], c2 = P.perr[2 * e] * (w * P.perr[2 * e]) + P.perr[2 * e + 1] * (w * P.perr[2 * e + 1]);
         double c[3]; se3_map(P.T[pe_kf[e]], lm_point(P, pe_pt[e]), c);
         if (c2 > 5.991 || !(c[2] > 0.0)) P.p_lvl[e] = 1;
+        near(c2, 5.991);
       }
       P.p_robust = false;
       for (int e = 0; e < n_le; e++) {
         double c1 = P.lerr[2 * e] * (P.info_line * P.lerr[2 * e]), c2 = P.lerr[2 * e + 1] * (P.info_line * P.lerr[2 * e + 1]);
         if (c1 > 3.84 || c2 > 3.84) P.l_lvl[e] = 1;
+        near(c1, 3.84); near(c2, 3.84);
       }
       P.l_robust = false;
       its += optimize(P, 10);
@@ -349,10 +362,12 @@ extern "C" int oracle_local_ba(int n_kf, const float* kf_Tcw, const uint8_t* kf_
       double w = (double)pe_inv_sigma2[e], c2 = P.perr[2 * e] * (w * P.perr[2 * e]) + P.perr[2 * e + 1] * (w * P.perr[2 * e + 1]);
       double c[3]; se3_map(P.T[pe_kf[e]], lm_point(P, pe_pt[e]), c);
       pe_erase[e] = (c2 > 5.991 || !(c[2] > 0.0)) ? 1 : 0;
+      near(c2, 5.991);
     }
     for (int e = 0; e < n_le; e++) {
       double c1 = P.lerr[2 * e] * (P.info_line * P.lerr[2 * e]);   // e1 and e2 both read the START-point edge (:2030-2031)
       le_erase[e] = (c1 > 3.84) ? 1 : 0;
+      near(c1, 3.84);
       le_erase_kf[e] = le_kf[e / 2];                                // vpLineEdgeKF[i] with the double push (:1924,1948)
     }
   } else {
@@ -366,6 +381,7 @@ extern "C" int oracle_local_ba(int n_kf, const float* kf_Tcw, const uint8_t* kf_
   for (int i = 0; i < 3 * n_pt; i++) pt_Xw_out[i] = (float)P.X[i];
   for (int i = 0; i < 6 * n_ln; i++) ln_Xw_out[i] = (double)(float)P.X[3 * n_pt + i];   // via Converter::toCvMat (float) -> Vector6d
   if (iterations_out) *iterations_out = its;
+  if (gate_gap) *gate_gap = gap;
   return 0;
 }
 

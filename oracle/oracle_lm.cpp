@@ -62,6 +62,11 @@ struct Problem {
   std::vector<double> le;        // line endpoint errors [nl][2] (start, end), component 0 only
   std::vector<uint8_t> p_active, l_active;   // level 0
   bool p_robust, l_robust;
+  // Rounding variants, for tests that need results which do not hang on the last bits of a sum (oracle_pose_optimization_ex):
+  // the line Jacobians' central-difference scale (g2o's 1 / (2 * 1e-9), or the literal 5e8 that k_pose_opt uses, one ulp
+  // higher), and the order the chi2 and H / b sums are formed in (sequential, or k_pose_opt's: see device_sum).
+  double jac_scale = 1.0 / (2 * 1e-9);
+  bool device_order = false;
 };
 const double kDeltaMono = (double)(float)std::sqrt(5.991);   // const float deltaMono = sqrt(5.991)
 const double kDeltaLine = (double)(float)std::sqrt(3.84);
@@ -70,6 +75,18 @@ inline void huber(double e, double delta, double rho[3]) {
   double dsqr = delta * delta;
   if (e <= dsqr) { rho[0] = e; rho[1] = 1.; rho[2] = 0.; }
   else { double s = std::sqrt(e); rho[0] = 2 * s * delta - dsqr; rho[1] = delta / s; rho[2] = -0.5 * rho[1] / e; }
+}
+// k_pose_opt's summation order: edge i goes to thread i % 128, which adds its edges in index order (points before lines);
+// v[t * n + k] holds thread t's partial k.  The CTA then reduces with butterflies inside each warp (xor 16, 8, 4, 2, 1) and adds
+// the four warp totals in warp order.
+constexpr int kDevThreads = 128;
+void device_sum(std::vector<double>& v, int n, double* out) {
+  std::vector<double> nv(v.size());
+  for (int o = 16; o > 0; o >>= 1) {
+    for (int t = 0; t < kDevThreads; t++) for (int k = 0; k < n; k++) nv[t * n + k] = v[t * n + k] + v[(t ^ o) * n + k];
+    v.swap(nv);
+  }
+  for (int k = 0; k < n; k++) { double s = 0; for (int w = 0; w < kDevThreads / 32; w++) s += v[32 * w * n + k]; out[k] = s; }
 }
 inline void point_error(const Problem& P, const SE3& T, int i, double e[2]) {
   double X[3] = {(double)P.pt_X[3 * i], (double)P.pt_X[3 * i + 1], (double)P.pt_X[3 * i + 2]}, c[3];
@@ -91,6 +108,21 @@ void compute_active_errors(Problem& P, const SE3& T) {
 }
 double active_robust_chi2(const Problem& P) {
   double chi = 0, rho[3];
+  if (P.device_order) {
+    std::vector<double> v(kDevThreads, 0.0);
+    for (int i = 0; i < P.np; i++) if (P.p_active[i]) {
+      double w = (double)P.pt_w[i];
+      double c2 = P.pe[2 * i] * (w * P.pe[2 * i]) + P.pe[2 * i + 1] * (w * P.pe[2 * i + 1]);
+      if (P.p_robust) { huber(c2, kDeltaMono, rho); v[i % kDevThreads] += rho[0]; } else v[i % kDevThreads] += c2;
+    }
+    for (int i = 0; i < P.nl; i++) if (P.l_active[i])
+      for (int e = 0; e < 2; e++) {
+        double c2 = P.le[2 * i + e] * P.le[2 * i + e];
+        if (P.l_robust) { huber(c2, kDeltaLine, rho); v[i % kDevThreads] += rho[0]; } else v[i % kDevThreads] += c2;
+      }
+    device_sum(v, 1, &chi);
+    return chi;
+  }
   for (int i = 0; i < P.np; i++) if (P.p_active[i]) {
     double w = (double)P.pt_w[i];
     double c2 = P.pe[2 * i] * (w * P.pe[2 * i]) + P.pe[2 * i + 1] * (w * P.pe[2 * i + 1]);
@@ -107,6 +139,7 @@ void build_system(const Problem& P, const SE3& T, double H[6][6], double b[6]) {
   memset(H, 0, sizeof(double) * 36);
   memset(b, 0, sizeof(double) * 6);
   double rho[3];
+  std::vector<double> v(P.device_order ? kDevThreads * 27 : 0, 0.0);   // device order: per thread 21 unique H entries + 6 of b
   for (int i = 0; i < P.np; i++) if (P.p_active[i]) {
     double X[3] = {(double)P.pt_X[3 * i], (double)P.pt_X[3 * i + 1], (double)P.pt_X[3 * i + 2]}, c[3];
     se3_map(T, X, c);
@@ -120,14 +153,22 @@ void build_system(const Problem& P, const SE3& T, double H[6][6], double b[6]) {
     const double* e = &P.pe[2 * i];
     double r1 = 1.0;
     if (P.p_robust) { huber(e[0] * (w * e[0]) + e[1] * (w * e[1]), kDeltaMono, rho); r1 = rho[1]; }
+    if (P.device_order) {
+      double* acc = &v[(size_t)(i % kDevThreads) * 27];
+      int k = 0;
+      for (int a = 0; a < 6; a++)
+        for (int c2 = a; c2 < 6; c2++) acc[k++] += J[0][a] * (r1 * w) * J[0][c2] + J[1][a] * (r1 * w) * J[1][c2];
+      for (int a = 0; a < 6; a++) acc[21 + a] -= r1 * (J[0][a] * (w * e[0]) + J[1][a] * (w * e[1]));
+      continue;
+    }
     for (int a = 0; a < 6; a++) {
       b[a] -= r1 * (J[0][a] * (w * e[0]) + J[1][a] * (w * e[1]));
       for (int c2 = 0; c2 < 6; c2++) H[a][c2] += J[0][a] * (r1 * w) * J[0][c2] + J[1][a] * (r1 * w) * J[1][c2];
     }
   }
   if (P.nl > 0) {
-    // numeric Jacobian: central differences, delta = 1e-9, through oplus (exp(d)*T)
-    const double delta = 1e-9, scalar = 1.0 / (2 * delta);
+    // numeric Jacobian: central differences, delta = 1e-9, through oplus (exp(d)*T); scale 1 / (2 delta) unless a variant asks
+    const double delta = 1e-9, scalar = P.jac_scale;
     SE3 Tp[6], Tm[6];
     for (int d = 0; d < 6; d++) {
       double add[6] = {0, 0, 0, 0, 0, 0};
@@ -140,11 +181,26 @@ void build_system(const Problem& P, const SE3& T, double H[6][6], double b[6]) {
         for (int d = 0; d < 6; d++) J[d] = scalar * (line_error(P, Tp[d], i, e) - line_error(P, Tm[d], i, e));
         double err = P.le[2 * i + e], r1 = 1.0;
         if (P.l_robust) { huber(err * err, kDeltaLine, rho); r1 = rho[1]; }
+        if (P.device_order) {
+          double* acc = &v[(size_t)(i % kDevThreads) * 27];
+          int k = 0;
+          for (int a = 0; a < 6; a++)
+            for (int c2 = a; c2 < 6; c2++) acc[k++] += J[a] * r1 * J[c2];
+          for (int a = 0; a < 6; a++) acc[21 + a] -= r1 * (J[a] * err);
+          continue;
+        }
         for (int a = 0; a < 6; a++) {
           b[a] -= r1 * (J[a] * err);
           for (int c2 = 0; c2 < 6; c2++) H[a][c2] += J[a] * r1 * J[c2];
         }
       }
+  }
+  if (P.device_order) {      // the kernel keeps the upper triangle and mirrors it
+    double s[27];
+    device_sum(v, 27, s);
+    int k = 0;
+    for (int a = 0; a < 6; a++) for (int c2 = a; c2 < 6; c2++) { H[a][c2] = s[k]; H[c2][a] = s[k]; k++; }
+    for (int a = 0; a < 6; a++) b[a] = s[21 + a];
   }
 }
 
@@ -202,10 +258,12 @@ void optimize(Problem& P, SE3& T, SE3& Terr, int iterations, int* its_done) {
 }
 }  // namespace
 
-extern "C" int oracle_pose_optimization(int mode, const float* Tcw_in, const float* K, int np, const float* pt_obs,
-                                        const float* pt_inv_sigma2, const float* pt_Xw, int nl, const double* line_func,
-                                        const double* line_Xw, float* Tcw_out, uint8_t* pt_outlier,
-                                        uint8_t* line_outlier, int* iterations_out) {
+// variant (0 = the reference): bit 0 = line Jacobian scale 5e8 instead of 1 / (2 * 1e-9), bit 1 = k_pose_opt's summation order.
+// A problem whose result is the same under every variant does not sit on a rounding-level LM decision (DESIGN.md §5).
+extern "C" int oracle_pose_optimization_ex(int mode, const float* Tcw_in, const float* K, int np, const float* pt_obs,
+                                           const float* pt_inv_sigma2, const float* pt_Xw, int nl, const double* line_func,
+                                           const double* line_Xw, float* Tcw_out, uint8_t* pt_outlier,
+                                           uint8_t* line_outlier, int* iterations_out, int variant) {
   if (mode == 1) nl = 0;
   if (mode == 2) np = 0;
   Problem P;
@@ -214,6 +272,8 @@ extern "C" int oracle_pose_optimization(int mode, const float* Tcw_in, const flo
   P.pe.assign(2 * (size_t)np + 2, 0.0); P.le.assign(2 * (size_t)nl + 2, 0.0);
   P.p_active.assign(np + 1, 1); P.l_active.assign(nl + 1, 1);
   P.p_robust = true; P.l_robust = true;
+  if (variant & 1) P.jac_scale = 5e8;
+  P.device_order = (variant & 2) != 0;
   for (int i = 0; i < np; i++) pt_outlier[i] = 0;
   for (int i = 0; i < nl; i++) line_outlier[i] = 0;
   memcpy(Tcw_out, Tcw_in, 16 * sizeof(float));
@@ -248,4 +308,12 @@ extern "C" int oracle_pose_optimization(int mode, const float* Tcw_in, const flo
   (void)Terr;
   se3_to_cv(T, Tcw_out);
   return mode == 2 ? nl - nLineBad : np - nBad;
+}
+
+extern "C" int oracle_pose_optimization(int mode, const float* Tcw_in, const float* K, int np, const float* pt_obs,
+                                        const float* pt_inv_sigma2, const float* pt_Xw, int nl, const double* line_func,
+                                        const double* line_Xw, float* Tcw_out, uint8_t* pt_outlier,
+                                        uint8_t* line_outlier, int* iterations_out) {
+  return oracle_pose_optimization_ex(mode, Tcw_in, K, np, pt_obs, pt_inv_sigma2, pt_Xw, nl, line_func, line_Xw, Tcw_out, pt_outlier,
+                                     line_outlier, iterations_out, 0);
 }

@@ -42,7 +42,7 @@ __global__ void k_track_points(const PLKeyPoint* __restrict__ ku_prev, const PLK
   if (!v) return;
   const PLKeyPoint k = ku_prev[o];
   const float* T = Tcw0 + 16 * b;
-  const float fx = K[0], fy = K[1], cx = K[2], cy = K[3];
+  const float fx = K[4 * b], fy = K[4 * b + 1], cx = K[4 * b + 2], cy = K[4 * b + 3];
   const float z = __fadd_rn(1.5f, __fmul_rn(0.25f, (float)(i & 15)));
   const float xc = __fmul_rn(__fdiv_rn(__fsub_rn(k.x, cx), fx), z), yc = __fmul_rn(__fdiv_rn(__fsub_rn(k.y, cy), fy), z);
   const float dx = __fsub_rn(xc, T[3]), dy = __fsub_rn(yc, T[7]), dz = __fsub_rn(z, T[11]);
@@ -226,11 +226,23 @@ extern "C" int pl_frontend_capacities(const PLFrontend* h, int* cap_keypoints, i
   return PL_OK;
 }
 
+// A problem over the configured capacities would lose its surplus correspondences without a word (the kernel clamps): refused.
+static int check_pose_problem_sizes(const PLFrontend* h, int B, const int* n_points, const int* n_lines) {
+  for (int b = 0; b < B; b++)
+    if (n_points[b] < 0 || n_points[b] > h->cfg.lm_cap_points || n_lines[b] < 0 || n_lines[b] > h->cfg.lm_cap_lines) {
+      set_error("pose problem %d has %d points and %d lines; the capacities are %d and %d", b, n_points[b], n_lines[b],
+                h->cfg.lm_cap_points, h->cfg.lm_cap_lines);
+      return PL_ERR_ARG;
+    }
+  return PL_OK;
+}
+
 // LM problems of the batch (device-resident until replaced).  Host pointers; [B][cap] layouts.
 extern "C" int pl_frontend_set_pose_problems(PLFrontend* h, int B, const float* Tcw0, const float* K, const int* n_points,
                                              const float* pt_obs, const float* pt_inv_sigma2, const float* pt_Xw,
                                              const int* n_lines, const double* line_func, const double* line_Xw) {
   PL_ARG(h && B >= 1 && B <= h->B && Tcw0 && K && n_points && pt_obs && pt_inv_sigma2 && pt_Xw && n_lines && line_func && line_Xw);
+  if (int rc = check_pose_problem_sizes(h, B, n_points, n_lines)) return rc;
   const size_t cp = h->cfg.lm_cap_points, cl = h->cfg.lm_cap_lines, b = B;
   cudaStream_t st = h->stream;
   PL_CUDA(cudaMemcpyAsync(h->d_T0, Tcw0, 64 * b, cudaMemcpyHostToDevice, st));
@@ -249,6 +261,7 @@ extern "C" long long pl_frontend_set_pose_problems_async(PLFrontend* h, int B, c
                                                          const float* pt_obs, const float* pt_inv_sigma2, const float* pt_Xw,
                                                          const int* n_lines, const double* line_func, const double* line_Xw, void* stream_) {
   PL_ARG(h && B >= 1 && B <= h->B && Tcw0 && K && n_points && pt_obs && pt_inv_sigma2 && pt_Xw && n_lines && line_func && line_Xw);
+  if (int rc = check_pose_problem_sizes(h, B, n_points, n_lines)) return rc;
   const size_t cp = h->cfg.lm_cap_points, cl = h->cfg.lm_cap_lines, b = B;
   cudaStream_t st = stream_ ? (cudaStream_t)stream_ : h->stream;
   PL_CUDA(cudaMemcpyAsync(h->d_T0, Tcw0, 64 * b, cudaMemcpyHostToDevice, st));

@@ -367,8 +367,10 @@ extern "C" int pl_pose_optimization(int mode, const float* Tcw_in, const float* 
     if (ret == PL_OK) {
       int inl = 0, its = 0;
       cudaError_t e = cudaMemcpy(Tcw_out, dTo, 64, cudaMemcpyDeviceToHost);
-      if (e == cudaSuccess && n_points && pt_outlier) e = cudaMemcpy(pt_outlier, dpo, n_points, cudaMemcpyDeviceToHost);
-      if (e == cudaSuccess && n_lines && line_outlier) e = cudaMemcpy(line_outlier, dlo, n_lines, cudaMemcpyDeviceToHost);
+      // the kernel writes only the masks of the edges the mode optimises (mode 1: points, mode 2: lines); the other one is the
+      // caller's and stays untouched, as the reference leaves mvbLineOutlier / mvbOutlier alone in those modes
+      if (e == cudaSuccess && mode != 2 && n_points && pt_outlier) e = cudaMemcpy(pt_outlier, dpo, n_points, cudaMemcpyDeviceToHost);
+      if (e == cudaSuccess && mode != 1 && n_lines && line_outlier) e = cudaMemcpy(line_outlier, dlo, n_lines, cudaMemcpyDeviceToHost);
       if (e == cudaSuccess) e = cudaMemcpy(&inl, dinl, 4, cudaMemcpyDeviceToHost);
       if (e == cudaSuccess) e = cudaMemcpy(&its, dits, 4, cudaMemcpyDeviceToHost);
       if (e != cudaSuccess) { set_error("pose optimisation: %s", cudaGetErrorString(e)); ret = PL_ERR_CUDA; }

@@ -306,7 +306,7 @@ struct SkipAssigned {
 
 struct ProjLastArgs {
   const PLKeyPoint* keys; const uint8_t* desc; const int* n; int cap;   // current frame [B][cap]
-  const float* bounds; const float* Tcw; const float* K; const float* scaleFactors; int nlevels;
+  const float* bounds; const float* Tcw; const float* K; const float* scaleFactors; int nlevels;   // Tcw [B][16], K [B][4]
   const int* n_last; int cap_last; const uint8_t* last_valid; const float* last_pos; const uint8_t* last_desc;
   const int* last_octave; const float* last_angle;
   float th; int checkOri; const uint8_t* preassigned; int* match; int* nmatches;
@@ -340,7 +340,8 @@ __global__ void __launch_bounds__(32) k_search_proj_last(ProjLastArgs A) {
   __syncwarp();
   int nmatches = 0;
   SkipAssigned skip{match};
-  const float fx = A.K[0], fy = A.K[1], cx = A.K[2], cy = A.K[3];
+  const float* Kb = A.K + 4 * b;      // frame b's camera ([B][4]; the host-pointer entries are B = 1)
+  const float fx = Kb[0], fy = Kb[1], cx = Kb[2], cy = Kb[3];
   for (int i = 0; i < NL; i++) {
     if (!A.last_valid[lb + i]) continue;
     const float* X = A.last_pos + (lb + i) * 3;

@@ -136,13 +136,19 @@ def synth_pose_problem(seed=3, n_points=300, n_lines=80, outlier_frac=0.10, K=TU
 
 # ---------------------------------------------------------------------------------------------- local BA window
 def synth_ba_problem(seed=4, n_free=20, n_fixed=40, n_pt=3000, n_ln=400, obs_pt=5, obs_ln=4, K=TUM1_K, w=640, h=480,
-                     noise_px=1.0, outlier_frac=0.03, pert_t=0.01, pert_deg=0.3, pert_X=0.02):
+                     noise_px=1.0, outlier_frac=0.03, pert_t=0.01, pert_deg=0.3, pert_X=0.02, Ks=None, K_end=None):
     """KITTI/TUM-shaped local-BA window (SURVEY.md §8d config 4): cameras on a smooth path in front of a scene,
     points with ~obs_pt and lines with ~obs_ln observations, noisy observations, a few gross outliers, perturbed
-    initial estimates.  Keyframe 0 is fixed (mnId == 0) together with the `n_fixed` covisible-but-not-local ones."""
+    initial estimates.  Keyframe 0 is fixed (mnId == 0) together with the `n_fixed` covisible-but-not-local ones.
+
+    Ks ([n_kf][4], optional): one camera per keyframe; keyframe k's observations are made with Ks[k] (as float32, the
+    precision the optimisers read).  K_end (optional): the current keyframe's camera the local BA projects line end
+    points with.  Both default to K; neither draws from the random stream, so the default output does not change."""
     rng = np.random.Generator(np.random.PCG64(seed))
-    fx, fy, cx, cy = K
     n_kf = n_free + n_fixed
+    if Ks is not None:
+        Ks = np.asarray(Ks, np.float32).reshape(n_kf, 4)
+    cams = [K] * n_kf if Ks is None else [tuple(float(v) for v in Ks[k]) for k in range(n_kf)]
     Ts = []
     for k in range(n_kf):
         s = k / max(n_kf - 1, 1)
@@ -155,8 +161,9 @@ def synth_ba_problem(seed=4, n_free=20, n_fixed=40, n_pt=3000, n_ln=400, obs_pt=
     Ts = Ts[order]
     fixed = np.zeros(n_kf, np.uint8); fixed[n_free:] = 1; fixed[0] = 1
 
-    def project(T, X):
-        Xc = X @ T[:3, :3].T + T[:3, 3]
+    def project(k, X):
+        fx, fy, cx, cy = cams[k]
+        Xc = X @ Ts[k, :3, :3].T + Ts[k, :3, 3]
         return np.stack([Xc[:, 0] / Xc[:, 2] * fx + cx, Xc[:, 1] / Xc[:, 2] * fy + cy], 1), Xc[:, 2]
 
     Xw = np.stack([rng.uniform(-4, 4, n_pt), rng.uniform(-2, 2, n_pt), rng.uniform(3, 9, n_pt)], 1)
@@ -165,7 +172,7 @@ def synth_ba_problem(seed=4, n_free=20, n_fixed=40, n_pt=3000, n_ln=400, obs_pt=
         cand = rng.permutation(n_kf)
         got = 0
         for k in cand:
-            uv, z = project(Ts[k], Xw[i:i + 1])
+            uv, z = project(k, Xw[i:i + 1])
             if z[0] > 0.5 and 0 < uv[0, 0] < w and 0 < uv[0, 1] < h:
                 octv = rng.integers(0, 8)
                 o = uv[0] + rng.normal(0, noise_px, 2) * 1.2 ** octv
@@ -182,7 +189,7 @@ def synth_ba_problem(seed=4, n_free=20, n_fixed=40, n_pt=3000, n_ln=400, obs_pt=
     for i in range(n_ln):
         got = 0
         for k in rng.permutation(n_kf):
-            ua, za = project(Ts[k], A[i:i + 1]); ub, zb = project(Ts[k], Bp[i:i + 1])
+            ua, za = project(k, A[i:i + 1]); ub, zb = project(k, Bp[i:i + 1])
             if za[0] > 0.5 and zb[0] > 0.5 and 0 < ua[0, 0] < w and 0 < ua[0, 1] < h and 0 < ub[0, 0] < w and 0 < ub[0, 1] < h:
                 pa = ua[0] + rng.normal(0, noise_px, 2); pb = ub[0] + rng.normal(0, noise_px, 2)
                 if rng.random() < outlier_frac:
@@ -198,7 +205,8 @@ def synth_ba_problem(seed=4, n_free=20, n_fixed=40, n_pt=3000, n_ln=400, obs_pt=
             dR = _rot(*np.deg2rad(rng.uniform(-pert_deg, pert_deg, 3)))
             T0[k, :3, :3] = dR @ Ts[k, :3, :3]; T0[k, :3, 3] = dR @ Ts[k, :3, 3] + rng.uniform(-pert_t, pert_t, 3)
     return dict(kf_Tcw=T0.astype(np.float32).reshape(n_kf, 16), kf_Tcw_true=Ts, kf_fixed=fixed,
-                kf_K=np.tile(np.array(K, np.float32), (n_kf, 1)), K_end=np.array(K, np.float32),
+                kf_K=np.tile(np.array(K, np.float32), (n_kf, 1)) if Ks is None else Ks.copy(),
+                K_end=np.array(K if K_end is None else K_end, np.float32),
                 pt_Xw=(Xw + rng.normal(0, pert_X, Xw.shape)).astype(np.float32), pt_Xw_true=Xw,
                 ln_Xw=np.ascontiguousarray(Lw + rng.normal(0, pert_X, Lw.shape)), ln_Xw_true=Lw,
                 pe_kf=np.array(pe_kf, np.int32), pe_pt=np.array(pe_pt, np.int32), pe_obs=np.array(pe_obs, np.float32).reshape(-1, 2),
