@@ -467,6 +467,97 @@ int pl_lsd_fuse_search(const void* keylines, int nl, const uint8_t* kf_point_des
                        const double* pos, const double* normal, const float* min_dist, const float* max_dist, const uint8_t* ml_desc,
                        float th, int* best_idx, int* best_dist, int* stop_at);
 
+/* ------------------------------------------------------------------ tracking a batch of frames against a fixed map
+ * Tracking::TrackLocalMapWithLines (src/Tracking.cc:1491-1562) with SearchLocalPoints (:1751-1801) and SearchLocalLines
+ * (:1803-1855), in localisation mode (mbOnlyTracking), for B frames at once; every intermediate stays on the device.
+ *
+ * The map (pl_map_create, uploaded once): per map point pos = MapPoint::GetWorldPos, normal = GetNormal, the RAW
+ * mfMinDistance / mfMaxDistance (see pl_frame_is_in_frustum_points), desc = GetDescriptor; per map line pos = mWorldPos
+ * (start, end), normal = GetNormal, the raw distances and desc = GetDescriptor.  Host pointers; the handle owns device copies. */
+typedef struct PLMapDesc {
+  int n_points;
+  const float* pt_pos /*[n][3]*/; const float* pt_normal /*[n][3]*/; const float* pt_min_dist; const float* pt_max_dist;
+  const uint8_t* pt_desc /*[n][32]*/;
+  int n_lines;
+  const double* ln_pos /*[n][6]*/; const double* ln_normal /*[n][3]*/; const float* ln_min_dist; const float* ln_max_dist;
+  const uint8_t* ln_desc /*[n][32]*/;
+} PLMapDesc;
+typedef struct PLMap PLMap;
+int pl_map_create(const PLMapDesc* desc, PLMap** out);
+void pl_map_destroy(PLMap* m);
+/* Sticky flag of the track calls since the last check: PL_ERR_ARG if a local-list entry or a pre-assigned match named an index
+ * outside the map (such an entry is treated as absent), else PL_OK; clears the flag.  Synchronises the device.  The host entry
+ * point checks it itself; callers of the _dev entry points call it after synchronising their stream. */
+int pl_map_check_indices(PLMap* m);
+
+/* The frames ([B][cap] device arrays in the front end's layouts; host arrays with B = 1 for pl_track_local_map):
+ *   keys_un = mvKeysUn, desc = mDescriptors, n = N; keylines = mvKeylinesUn (68 B records), line_func = mvKeyLineFunctions,
+ *   line_desc = mLdesc, nl = NL; bounds = {mnMinX, mnMinY, mnMaxX, mnMaxY}, one for the batch (the search grid's bounds);
+ *   scale_factors / inv_level_sigma2 = mvScaleFactors / mvInvLevelSigma2 ([nlevels]), log_scale_factor = mfLogScaleFactor;
+ *   Tcw0 [B][16] = the pose guess (mTcw, row-major), K [B][4] = {fx, fy, cx, cy} of each frame;
+ *   point_map_in [B][cap_points] / line_map_in [B][cap_lines] = the matches the frame already holds (mvpMapPoints / mvpMapLines
+ *   from TrackWithMotionModel, TrackReferenceKeyFrame or Relocalization) as map indices, -1 for none; NULL = no match held. */
+typedef struct PLTrackFrames {
+  int B;
+  const PLKeyPoint* keys_un; const uint8_t* desc; const int* n; int cap_points;
+  const void* keylines; const double* line_func; const uint8_t* line_desc; const int* nl; int cap_lines;
+  const float* bounds; const float* scale_factors; const float* inv_level_sigma2; int nlevels; float log_scale_factor;
+  const float* Tcw0; const float* K;
+  const int* point_map_in; const int* line_map_in;
+} PLTrackFrames;
+/* The local maps (mvpLocalMapPoints / mvpLocalMapLines, built by the caller's UpdateLocalMap): frame b's list is
+ * pt_index[pt_offset[b] .. pt_offset[b] + pt_count[b]) of map-point indices, in the reference's order; frames may share or
+ * overlap their ranges.  Offsets, counts and frames_since_reloc are HOST arrays [B] (read during the call); the index arrays
+ * (n_pt_index / n_ln_index entries) are on the device (host for pl_track_local_map).  PL_ERR_ARG before anything is enqueued: a
+ * count over cap_local_points / cap_local_lines or negative, a negative offset, or a range past the end of its index array.  frames_since_reloc[b] = mCurrentFrame.mnId - mnLastRelocFrameId: th = 5 below 2, else 1
+ * (:1793-1798, :1850-1853); max_frames = mMaxFrames: frame b needs 50 inliers while frames_since_reloc[b] < max_frames, else 30
+ * (:1555-1561). */
+typedef struct PLTrackLocal {
+  const int* pt_offset; const int* pt_count; const int* pt_index; int n_pt_index; int cap_local_points;
+  const int* ln_offset; const int* ln_count; const int* ln_index; int n_ln_index; int cap_local_lines;
+  const int* frames_since_reloc; int max_frames;
+} PLTrackLocal;
+/* Results (device arrays, host for pl_track_local_map).  Required: Tcw [B][16] = the optimised pose; point_map [B][cap_points] /
+ * line_map [B][cap_lines] = mvpMapPoints / mvpMapLines after the searches (map index or -1); point_outlier / line_outlier =
+ * mvbOutlier / mvbLineOutlier (0 for features without a match); inliers [B][2] = {mnMatchesInliers, mnLineMatchesInliers};
+ * ok [B] = the return value.
+ * Optional (NULL = kept in the scratch): the isInFrustum outputs per local-list entry, [B][cap_local_*] (pt_proj [.][2],
+ * ln_proj [.][4]; in_view = 0 for entries the frame already holds, :1776-1777), the raw search results pt_match [B][cap_points] /
+ * ln_match [B][cap_lines] (local-list position, -1 none, -2 held before the search), and the PoseOptimization problem exactly as
+ * pl_pose_optimization_dev reads it ([B][cap_points] / [B][cap_lines] layouts, counts [B]). */
+typedef struct PLTrackOut {
+  float* Tcw; int* point_map; uint8_t* point_outlier; int* line_map; uint8_t* line_outlier; int* inliers; int* ok;
+  uint8_t* pt_in_view; float* pt_proj; int* pt_level; float* pt_view_cos;
+  uint8_t* ln_in_view; float* ln_proj; int* ln_level; float* ln_view_cos;
+  int* pt_match; int* ln_match;
+  int* prob_n_points; float* prob_pt_obs; float* prob_pt_inv_sigma2; float* prob_pt_Xw;
+  int* prob_n_lines; double* prob_line_func; double* prob_line_Xw;
+} PLTrackOut;
+/* Per frame b, in the reference's order: Ow of Frame::UpdatePoseMatrices (Frame.cc:552-558); the local-map entries the frame
+ * already holds are skipped (mnLastFrameSeen == mnId, :1754-1779), the others go through isInFrustum(., 0.5); then
+ * ORBmatcher(0.8).SearchByProjection(F, mvpLocalMapPoints, th) (ORBmatcher.cc:56-152) and LSDmatcher().SearchByProjection(F,
+ * mvpLocalMapLines, th) (LSDmatcher.cpp:221-338, nnratio 0.7), with the features that hold a match pre-assigned; the
+ * PoseOptimization problem in feature order, points then lines (Optimizer.cc:640-841: mvKeysUn[i].pt, mvInvLevelSigma2[octave],
+ * GetWorldPos; mvKeyLineFunctions[i], mWorldPos), solved by pl_pose_optimization_dev mode 0; then the inlier counts and the
+ * return value (:1504-1561, mbOnlyTracking branch).  A frame with fewer than 3 correspondences keeps its pose.
+ * The caller applies the map statistics the reference updates on the way: IncreaseVisible for every held match and every local
+ * entry with pt_in_view / ln_in_view set, IncreaseFound for every match that is not an outlier.
+ * Scratch: pl_track_local_map_scratch_bytes(B, caps) bytes of device memory (16-byte aligned).  Asynchronous on `stream`
+ * (NULL = the map's stream); the host arrays of PLTrackLocal are read before the call returns. */
+size_t pl_track_local_map_scratch_bytes(int B, int cap_points, int cap_lines, int cap_local_points, int cap_local_lines);
+int pl_track_local_map_dev(PLMap* map, const PLTrackFrames* frames, const PLTrackLocal* local, const PLTrackOut* out, void* scratch,
+                           void* stream);
+/* The same for ONE frame on host pointers (frames->B must be 1; caps = the counts, or larger); synchronous.  Returns ok (0 / 1)
+ * or an error. */
+int pl_track_local_map(PLMap* map, const PLTrackFrames* frames, const PLTrackLocal* local, const PLTrackOut* out);
+/* The step on the features of the front end's LAST step (pl_frontend_run / run_dev / submit): frames 0 .. B-1 of that step
+ * (PL_ERR_ARG if B exceeds that step's batch or no step has run), with the
+ * handle's bounds and ORB tables; Tcw0 / K / point_map_in / line_map_in are device arrays ([B][capK] / [B][capL] layouts of
+ * pl_frontend_capacities).  Asynchronous on `stream` (NULL = the handle's stream). */
+int pl_frontend_track_local_map_dev(PLFrontend* h, PLMap* map, int B, const float* Tcw0, const float* K, const int* point_map_in,
+                                    const int* line_map_in, const PLTrackLocal* local, const PLTrackOut* out, void* scratch,
+                                    void* stream);
+
 /* ------------------------------------------------------------------ multi-GPU exchange (SURVEY.md §8e)
  * Frames shard across the GPUs of one box with no data-path collective; the ONE exchange is an all-gather of the per-frame
  * pose records (64 B per frame) over NCCL / NVLink so that the rank running the sequential Tracking logic (Tracking.cc:329)

@@ -879,3 +879,198 @@ def _lsd_fuse_search(self, keylines, kf_point_desc, bounds, Tcw, Ow, K, scale_li
 
 
 LSDmatcher.FuseSearch = _lsd_fuse_search
+
+
+# ---------------------------------------------------------------------------------------------- tracking against a fixed map
+class PLMapDesc(C.Structure):
+    _fields_ = [("n_points", C.c_int), ("pt_pos", vp), ("pt_normal", vp), ("pt_min_dist", vp), ("pt_max_dist", vp), ("pt_desc", vp),
+                ("n_lines", C.c_int), ("ln_pos", vp), ("ln_normal", vp), ("ln_min_dist", vp), ("ln_max_dist", vp), ("ln_desc", vp)]
+
+
+class PLTrackFrames(C.Structure):
+    _fields_ = [("B", C.c_int), ("keys_un", vp), ("desc", vp), ("n", vp), ("cap_points", C.c_int), ("keylines", vp), ("line_func", vp),
+                ("line_desc", vp), ("nl", vp), ("cap_lines", C.c_int), ("bounds", vp), ("scale_factors", vp), ("inv_level_sigma2", vp),
+                ("nlevels", C.c_int), ("log_scale_factor", C.c_float), ("Tcw0", vp), ("K", vp), ("point_map_in", vp), ("line_map_in", vp)]
+
+
+class PLTrackLocal(C.Structure):
+    _fields_ = [("pt_offset", vp), ("pt_count", vp), ("pt_index", vp), ("n_pt_index", C.c_int), ("cap_local_points", C.c_int),
+                ("ln_offset", vp), ("ln_count", vp), ("ln_index", vp), ("n_ln_index", C.c_int), ("cap_local_lines", C.c_int),
+                ("frames_since_reloc", vp), ("max_frames", C.c_int)]
+
+
+_TRACK_OUT = ["Tcw", "point_map", "point_outlier", "line_map", "line_outlier", "inliers", "ok", "pt_in_view", "pt_proj", "pt_level",
+              "pt_view_cos", "ln_in_view", "ln_proj", "ln_level", "ln_view_cos", "pt_match", "ln_match", "prob_n_points", "prob_pt_obs",
+              "prob_pt_inv_sigma2", "prob_pt_Xw", "prob_n_lines", "prob_line_func", "prob_line_Xw"]
+_TAPS = _TRACK_OUT[7:]
+
+
+class PLTrackOut(C.Structure):
+    _fields_ = [(k, vp) for k in _TRACK_OUT]
+
+
+def _track_lib():
+    L = lib()
+    if not getattr(L, "_track_types", False):
+        L.pl_map_create.argtypes = [C.POINTER(PLMapDesc), C.POINTER(vp)]
+        L.pl_map_destroy.argtypes = [vp]
+        L.pl_map_check_indices.argtypes = [vp]
+        L.pl_track_local_map_scratch_bytes.argtypes = [C.c_int] * 5
+        L.pl_track_local_map_scratch_bytes.restype = C.c_size_t
+        L.pl_track_local_map_dev.argtypes = [vp, C.POINTER(PLTrackFrames), C.POINTER(PLTrackLocal), C.POINTER(PLTrackOut), vp, vp]
+        L.pl_track_local_map.argtypes = [vp, C.POINTER(PLTrackFrames), C.POINTER(PLTrackLocal), C.POINTER(PLTrackOut)]
+        L.pl_frontend_track_local_map_dev.argtypes = [vp, vp, C.c_int, vp, vp, vp, vp, C.POINTER(PLTrackLocal), C.POINTER(PLTrackOut), vp, vp]
+        L._track_types = True
+    return L
+
+
+class Map:
+    """A fixed map on the device (pl_map_create): map points (GetWorldPos, GetNormal, raw mfMinDistance / mfMaxDistance,
+    GetDescriptor) and map lines (mWorldPos, GetNormal, raw distances, GetDescriptor), indexed 0..n-1."""
+
+    def __init__(self, pt_pos, pt_normal, pt_min_dist, pt_max_dist, pt_desc, ln_pos, ln_normal, ln_min_dist, ln_max_dist, ln_desc):
+        self._a = [_f32(pt_pos).reshape(-1, 3), _f32(pt_normal).reshape(-1, 3), _f32(pt_min_dist), _f32(pt_max_dist),
+                   np.ascontiguousarray(pt_desc, np.uint8).reshape(-1, 32), np.ascontiguousarray(ln_pos, np.float64).reshape(-1, 6),
+                   np.ascontiguousarray(ln_normal, np.float64).reshape(-1, 3), _f32(ln_min_dist), _f32(ln_max_dist),
+                   np.ascontiguousarray(ln_desc, np.uint8).reshape(-1, 32)]
+        a = self._a
+        self.n_points, self.n_lines = len(a[0]), len(a[5])
+        d = PLMapDesc(self.n_points, *[_p(x) for x in a[:5]], self.n_lines, *[_p(x) for x in a[5:]])
+        self._h = vp()
+        check(_track_lib().pl_map_create(C.byref(d), C.byref(self._h)))
+
+    def __del__(self):
+        if getattr(self, "_h", None) and self._h.value:
+            lib().pl_map_destroy(self._h)
+            self._h = vp()
+
+    def check_indices(self):
+        """PL_ERR_ARG (raised) if a call since the last check met an index outside the map."""
+        check(_track_lib().pl_map_check_indices(self._h))
+
+
+def _local_struct(local, B, keep, to_dev):
+    """local: dict(pt_index, pt_offset [B], pt_count [B], ln_index, ln_offset, ln_count, frames_since_reloc [B], max_frames,
+    cap_local_points / cap_local_lines (default: the largest count))."""
+    host = {k: np.ascontiguousarray(local[k], np.int32) for k in ("pt_offset", "pt_count", "ln_offset", "ln_count", "frames_since_reloc")}
+    for k, v in host.items():
+        assert v.shape == (B,), k
+    keep.append(host)
+    cLP = int(local.get("cap_local_points", max(int(host["pt_count"].max(initial=0)), 1)))
+    cLL = int(local.get("cap_local_lines", max(int(host["ln_count"].max(initial=0)), 1)))
+    arrs = [np.ascontiguousarray(local[k], np.int32).ravel() for k in ("pt_index", "ln_index")]
+    idx = [to_dev(a) for a in arrs]
+    keep.append(idx)
+    s = PLTrackLocal(_p(host["pt_offset"]), _p(host["pt_count"]), idx[0][1], len(arrs[0]), cLP, _p(host["ln_offset"]), _p(host["ln_count"]),
+                     idx[1][1], len(arrs[1]), cLL, _p(host["frames_since_reloc"]), int(local["max_frames"]))
+    return s, cLP, cLL
+
+
+def _out_shapes(B, cap, capL, cLP, cLL):
+    return dict(Tcw=((B, 4, 4), np.float32), point_map=((B, cap), np.int32), point_outlier=((B, cap), np.uint8),
+                line_map=((B, capL), np.int32), line_outlier=((B, capL), np.uint8), inliers=((B, 2), np.int32), ok=((B,), np.int32),
+                pt_in_view=((B, cLP), np.uint8), pt_proj=((B, cLP, 2), np.float32), pt_level=((B, cLP), np.int32),
+                pt_view_cos=((B, cLP), np.float32), ln_in_view=((B, cLL), np.uint8), ln_proj=((B, cLL, 4), np.float32),
+                ln_level=((B, cLL), np.int32), ln_view_cos=((B, cLL), np.float32), pt_match=((B, cap), np.int32),
+                ln_match=((B, capL), np.int32), prob_n_points=((B,), np.int32), prob_pt_obs=((B, cap, 2), np.float32),
+                prob_pt_inv_sigma2=((B, cap), np.float32), prob_pt_Xw=((B, cap, 3), np.float32), prob_n_lines=((B,), np.int32),
+                prob_line_func=((B, capL, 3), np.float64), prob_line_Xw=((B, capL, 6), np.float64))
+
+
+def _torch_dev():
+    import torch
+    keep = []
+
+    def to_dev(a):
+        a = np.ascontiguousarray(a)
+        t = torch.from_numpy(a.view(np.uint8).reshape(-1).copy() if a.size else np.zeros(16, np.uint8)).cuda()
+        keep.append(t)
+        return t, vp(t.data_ptr())
+    return torch, keep, to_dev
+
+
+def _run_dev(call, B, cap, capL, cLP, cLL, taps, keep, torch):
+    shapes = _out_shapes(B, cap, capL, cLP, cLL)
+    names = _TRACK_OUT if taps else _TRACK_OUT[:7]
+    dev = {}
+    for k in names:
+        shp, dt = shapes[k]
+        dev[k] = torch.zeros(max(int(np.prod(shp)) * np.dtype(dt).itemsize, 16), dtype=torch.uint8, device="cuda")
+    o = PLTrackOut(*[vp(dev[k].data_ptr()) if k in dev else None for k in _TRACK_OUT])
+    scratch = torch.empty(int(_track_lib().pl_track_local_map_scratch_bytes(B, cap, capL, cLP, cLL)), dtype=torch.uint8, device="cuda")
+    torch.cuda.synchronize()
+    check(call(o, vp(scratch.data_ptr())))
+    torch.cuda.synchronize()
+    out = {}
+    for k in names:
+        shp, dt = shapes[k]
+        nb = int(np.prod(shp)) * np.dtype(dt).itemsize
+        out[k] = dev[k][:nb].cpu().numpy().view(dt).reshape(shp)
+    return out
+
+
+def track_local_map(map, frames, local, taps=False, host=False):
+    """Tracking::TrackLocalMapWithLines (localisation mode) for B frames against `map` (pl_track_local_map_dev).
+
+    frames: dict(keys_un [B][cap] KP_DTYPE, desc [B][cap][32], n [B], keylines [B][capL] KEYLINE_DTYPE, line_func [B][capL][3],
+    line_desc [B][capL][32], nl [B], bounds [4], scale_factors, inv_level_sigma2, log_scale_factor, Tcw0 [B][4][4], K [B][4],
+    point_map_in / line_map_in ([B][cap] map index or -1; optional)).  local: see _local_struct.
+    Returns dict(Tcw, point_map, point_outlier, line_map, line_outlier, inliers [B][2], ok [B]) plus, with taps=True, the
+    intermediates of PLTrackOut.  host=True (B = 1 only) calls the host-pointer entry pl_track_local_map instead."""
+    L = _track_lib()
+    B, cap = frames["keys_un"].shape[:2]
+    capL = frames["keylines"].shape[1]
+    nlev = len(frames["scale_factors"])
+    arr = dict(keys_un=np.ascontiguousarray(frames["keys_un"], KP_DTYPE), desc=np.ascontiguousarray(frames["desc"], np.uint8),
+               n=np.ascontiguousarray(frames["n"], np.int32), keylines=np.ascontiguousarray(frames["keylines"], KEYLINE_DTYPE),
+               line_func=np.ascontiguousarray(frames["line_func"], np.float64), line_desc=np.ascontiguousarray(frames["line_desc"], np.uint8),
+               nl=np.ascontiguousarray(frames["nl"], np.int32), bounds=_f32(frames["bounds"]), scale_factors=_f32(frames["scale_factors"]),
+               inv_level_sigma2=_f32(frames["inv_level_sigma2"]), Tcw0=_f32(frames["Tcw0"]).reshape(B, 16), K=_f32(frames["K"]).reshape(B, 4))
+    for k in ("point_map_in", "line_map_in"):
+        if frames.get(k) is not None:
+            arr[k] = np.ascontiguousarray(frames[k], np.int32)
+    if host:
+        assert B == 1
+        keep = []
+        s, cLP, cLL = _local_struct(local, 1, keep, lambda a: (a, _p(a)))
+        F = PLTrackFrames(1, _p(arr["keys_un"]), _p(arr["desc"]), _p(arr["n"]), cap, _p(arr["keylines"]), _p(arr["line_func"]),
+                          _p(arr["line_desc"]), _p(arr["nl"]), capL, _p(arr["bounds"]), _p(arr["scale_factors"]), _p(arr["inv_level_sigma2"]),
+                          nlev, float(frames["log_scale_factor"]), _p(arr["Tcw0"]), _p(arr["K"]), _p(arr.get("point_map_in")),
+                          _p(arr.get("line_map_in")))
+        n, nl = int(arr["n"][0]), int(arr["nl"][0])
+        lp, ll = int(s.cap_local_points), int(s.cap_local_lines)
+        shapes = _out_shapes(1, cap, capL, lp, ll)
+        out = {k: np.zeros(shp, dt) for k, (shp, dt) in shapes.items()}
+        names = _TRACK_OUT if taps else _TRACK_OUT[:7]
+        o = PLTrackOut(*[_p(out[k]) if (k in names and k != "ok") else None for k in _TRACK_OUT])
+        out["ok"][0] = check(L.pl_track_local_map(map._h, C.byref(F), C.byref(s), C.byref(o)))
+        return {k: out[k] for k in names}
+    torch, keep, to_dev = _torch_dev()
+    d = {k: to_dev(v)[1] for k, v in arr.items()}
+    s, cLP, cLL = _local_struct(local, B, keep, to_dev)
+    F = PLTrackFrames(B, d["keys_un"], d["desc"], d["n"], cap, d["keylines"], d["line_func"], d["line_desc"], d["nl"], capL, d["bounds"],
+                      d["scale_factors"], d["inv_level_sigma2"], nlev, float(frames["log_scale_factor"]), d["Tcw0"], d["K"],
+                      d.get("point_map_in"), d.get("line_map_in"))
+    out = _run_dev(lambda o, scr: L.pl_track_local_map_dev(map._h, C.byref(F), C.byref(s), C.byref(o), scr, None),
+                   B, cap, capL, cLP, cLL, taps, keep, torch)
+    map.check_indices()
+    return out
+
+
+def _frontend_track_local_map(self, map, Tcw0, K, local, point_map_in=None, line_map_in=None, taps=False):
+    """Tracking::TrackLocalMapWithLines on the features of the last run() / run_dev() (pl_frontend_track_local_map_dev): frames
+    0..B-1 of that step, B = len(Tcw0).  point_map_in / line_map_in are [B][capK] / [B][capL] (map index or -1) or None."""
+    L = _track_lib()
+    B = len(Tcw0)
+    torch, keep, to_dev = _torch_dev()
+    T0 = to_dev(_f32(Tcw0).reshape(B, 16))[1]; Kd = to_dev(_f32(K).reshape(B, 4))[1]
+    pm = None if point_map_in is None else to_dev(np.ascontiguousarray(point_map_in, np.int32).reshape(B, self.capK))[1]
+    lm = None if line_map_in is None else to_dev(np.ascontiguousarray(line_map_in, np.int32).reshape(B, self.capL))[1]
+    s, cLP, cLL = _local_struct(local, B, keep, to_dev)
+    out = _run_dev(lambda o, scr: L.pl_frontend_track_local_map_dev(self._h, map._h, B, T0, Kd, pm, lm, C.byref(s), C.byref(o), scr, None),
+                   B, self.capK, self.capL, cLP, cLL, taps, keep, torch)
+    map.check_indices()
+    return out
+
+
+Frontend.track_local_map = _frontend_track_local_map

@@ -131,12 +131,15 @@ struct PLFrontend {
   int slot = 0;
   long long submitted = 0, completed = 0;
   int wrap = 0;       // 1: frame 0 is matched against the LAST frame of the same batch (closed loop); 0: against the last frame of the previous step
+  float* d_orb_tab = nullptr;
+  int last_B = 0;                       // frames of the last step (0: none yet) and where its mvKeysUn are
+  const PLKeyPoint* last_ku = nullptr;   // mvScaleFactors, mvInvLevelSigma2 for pl_frontend_track_local_map_dev (made on first use)
 };
 
 extern "C" void pl_frontend_destroy(PLFrontend* h) {
   if (!h) return;
   pl_orb_destroy(h->orb); pl_line_destroy(h->line); pl_undistort_destroy(h->und);
-  cudaFree(h->d_und); cudaFree(h->d_kpsu_prev);
+  cudaFree(h->d_und); cudaFree(h->d_kpsu_prev); cudaFree(h->d_orb_tab);
   cudaFree(h->d_in[0]); cudaFree(h->d_in[1]); cudaFree(h->d_stage);
   if (h->sUp) cudaStreamDestroy(h->sUp);
   if (h->sDown) cudaStreamDestroy(h->sDown);
@@ -436,6 +439,7 @@ extern "C" int pl_frontend_run_dev(PLFrontend* h, const uint8_t* imgs, int strid
     PL_CUDA(cudaStreamWaitEvent(st, h->evLine, 0));
     PL_CUDA(cudaStreamWaitEvent(st, h->evLm, 0));
   }
+  h->last_B = B; h->last_ku = h->und ? h->d_kpsu_prev + cK : h->d_kps;
   return PL_OK;
 }
 
@@ -667,4 +671,29 @@ extern "C" int pl_frontend_dump(PLFrontend* h, int B, const char* path) {
   fclose(f);
   if (!ok) { set_error("short write to %s", path); return PL_ERR_ARG; }
   return PL_OK;
+}
+
+// Tracking::TrackLocalMapWithLines on the frames of the last step (track.cu): mvKeysUn, descriptors, keylines, line functions and line
+// descriptors stay where the step left them; mvScaleFactors / mvInvLevelSigma2 / mfLogScaleFactor are the handle's ORB tables.
+extern "C" int pl_frontend_track_local_map_dev(PLFrontend* h, PLMap* map, int B, const float* Tcw0, const float* K, const int* point_map_in,
+                                               const int* line_map_in, const PLTrackLocal* local, const PLTrackOut* out, void* scratch,
+                                               void* stream) {
+  // only the frames the last step produced: later slots hold an older step's features, or none
+  PL_ARG(h && B >= 1 && B <= h->last_B);
+  const int nlev = h->cfg.orb_nlevels;
+  if (!h->d_orb_tab) {
+    std::vector<float> tab(2 * (size_t)nlev);
+    int rc = pl_orb_tables(h->orb, tab.data(), nullptr, nullptr, tab.data() + nlev, nullptr, nullptr, nullptr);
+    if (rc) return rc;
+    if ((rc = dev_alloc(&h->d_orb_tab, tab.size()))) return rc;
+    PL_CUDA(cudaMemcpy(h->d_orb_tab, tab.data(), tab.size() * sizeof(float), cudaMemcpyHostToDevice));
+  }
+  PLTrackFrames F;
+  F.B = B;
+  F.keys_un = h->last_ku; F.desc = h->d_desc; F.n = h->d_n; F.cap_points = h->capK;
+  F.keylines = h->d_kl; F.line_func = h->d_lf; F.line_desc = h->d_ldesc; F.nl = h->d_nl; F.cap_lines = h->capL;
+  F.bounds = h->d_bounds; F.scale_factors = h->d_orb_tab; F.inv_level_sigma2 = h->d_orb_tab + nlev; F.nlevels = nlev;
+  F.log_scale_factor = logf(h->cfg.orb_scale_factor);   // Frame: mfLogScaleFactor = log(mfScaleFactor) on a float
+  F.Tcw0 = Tcw0; F.K = K; F.point_map_in = point_map_in; F.line_map_in = line_map_in;
+  return pl_track_local_map_dev(map, &F, local, out, scratch, stream ? stream : (void*)h->stream);
 }

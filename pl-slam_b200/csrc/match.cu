@@ -17,6 +17,7 @@
 // Frames of a batch are independent -> one warp (CTA) per frame, grid = B.
 
 #include "common.cuh"
+#include "search.cuh"
 #include "libm_glibc.cuh"
 #include <vector>
 
@@ -395,6 +396,8 @@ struct ProjPointsArgs {
   const float* bounds; const float* scaleFactors;
   const int* n_mp; int cap_mp; const uint8_t* in_view; const float* proj; const int* level; const float* view_cos;
   const uint8_t* mp_desc; float th; float nnratio; const uint8_t* preassigned; int* match; int* nmatches;
+  const float* th_frame;   // [B] per-frame th (NULL: th)
+  const int* desc_row;     // [B][cap_mp] row of mp_desc for each entry (NULL: the entry's own [B][cap_mp] row)
 };
 
 __global__ void __launch_bounds__(32) k_search_proj_points(ProjPointsArgs A) {
@@ -413,14 +416,16 @@ __global__ void __launch_bounds__(32) k_search_proj_points(ProjPointsArgs A) {
   __syncwarp();
   int nmatches = 0;
   SkipAssigned skip{match};
-  const bool bFactor = A.th != 1.0f;
+  const float th = A.th_frame ? A.th_frame[b] : A.th;
+  const bool bFactor = th != 1.0f;
   for (int i = 0; i < NM; i++) {
     if (!A.in_view[mb + i]) continue;
     const int lvl = A.level[mb + i];
     float r = ((double)A.view_cos[mb + i] > 0.998) ? 2.5f : 4.0f;  // float vs the double literal 0.998
-    if (bFactor) r = __fmul_rn(r, A.th);
+    if (bFactor) r = __fmul_rn(r, th);
+    const long long drow = A.desc_row ? (long long)A.desc_row[mb + i] : mb + i;
     Top2 t = window_top2(k, d, sg.start, sg.items, g, A.proj[(mb + i) * 2], A.proj[(mb + i) * 2 + 1],
-                         __fmul_rn(r, A.scaleFactors[lvl]), lvl - 1, lvl, A.mp_desc + (mb + i) * 32, skip, lane, packed);
+                         __fmul_rn(r, A.scaleFactors[lvl]), lvl - 1, lvl, A.mp_desc + drow * 32, skip, lane, packed);
     if (t.best == KEY_NONE) continue;
     const int bestDist = key_dist(t.best), bestIdx = key_idx(t.best);
     if (bestDist <= 100) {
@@ -661,6 +666,8 @@ struct LineSearchArgs {
   float th, nnratio; int variant;
   const uint8_t* preassigned; int* match; int* nmatches;
   int* g_start; unsigned short* g_items; unsigned short* g_path; unsigned short* g_plen; int* g_first;   // scratch per frame
+  const float* th_frame;   // [B] per-frame th (NULL: th)
+  const int* q_desc_row;   // [B][cap_q] row of q_desc for each query (NULL: the query's own [B][cap_q] row)
 };
 
 __global__ void __launch_bounds__(32) k_line_search(LineSearchArgs A) {
@@ -682,13 +689,15 @@ __global__ void __launch_bounds__(32) k_line_search(LineSearchArgs A) {
   __syncwarp();
   int nmatches = 0;
   const long long qb = (long long)b * A.cap_q;
-  const bool bFactor = A.th != 1.0f;
+  const float th = A.th_frame ? A.th_frame[b] : A.th;
+  const bool bFactor = th != 1.0f;
   for (int q = 0; q < NQ; q++) {
     if (!A.q_valid[qb + q]) continue;
     const float* p = A.q_proj + (qb + q) * 4;
     float r, TH;
-    if (A.variant == 0) { r = A.th; TH = 0.96f; }
-    else { r = ((double)A.q_view_cos[qb + q] > 0.998) ? 5.0f : 8.0f; if (bFactor) r = __fmul_rn(r, A.th); TH = 0.998f; }
+    if (A.variant == 0) { r = th; TH = 0.96f; }
+    else { r = ((double)A.q_view_cos[qb + q] > 0.998) ? 5.0f : 8.0f; if (bFactor) r = __fmul_rn(r, th); TH = 0.998f; }
+    const uint8_t* qd = A.q_desc + (A.q_desc_row ? (long long)A.q_desc_row[qb + q] : qb + q) * 32;
     line_candidates(kl, lf, L, g, p[0], p[1], p[2], p[3], r, TH, first, N, lane);
     // candidates in first-occurrence order; top-2 by (distance, order)
     unsigned long long k1 = KEY_NONE, k2 = KEY_NONE;
@@ -696,7 +705,7 @@ __global__ void __launch_bounds__(32) k_line_search(LineSearchArgs A) {
       const int ord = first[id];
       if (ord == 0x7fffffff) continue;
       if (match[id] != -1) continue;
-      const int dist = hamming256(A.q_desc + (qb + q) * 32, d + 32 * id);
+      const int dist = hamming256(qd, d + 32 * id);
       if (A.variant == 0) {
         const float a = A.q_length[qb + q], c = kl[id].lineLength;
         const float mx = fmaxf(a, c), mn = fminf(a, c);
@@ -1168,7 +1177,7 @@ extern "C" int pl_orb_search_by_projection_points(const PLKeyPoint* keys, const 
   int rc = require_device(); if (rc) return rc;
   Stage s;
   const int cap = std::max(n, 1), capm = std::max(n_mp, 1);
-  ProjPointsArgs A;
+  ProjPointsArgs A{};
   A.keys = s.up(keys, n); A.desc = s.up(desc, (size_t)n * 32); A.n = s.up(&n, 1); A.cap = cap;
   A.bounds = s.up(bounds, 4); A.scaleFactors = s.up(scale_factors, nlevels);
   A.n_mp = s.up(&n_mp, 1); A.cap_mp = capm; A.in_view = s.up(in_view, n_mp); A.proj = s.up(proj, (size_t)n_mp * 2);
@@ -1208,14 +1217,15 @@ extern "C" int pl_orb_search_by_projection_last_dev(const PLKeyPoint* keys_cur, 
   PL_LAUNCH_CHECK();
   return PL_OK;
 }
-extern "C" int pl_orb_search_by_projection_points_dev(const PLKeyPoint* keys, const uint8_t* desc, const int* n, int cap, int B,
-                                                      const float* bounds, const float* scale_factors, const int* n_mp, int cap_mp,
-                                                      const uint8_t* in_view, const float* proj, const int* level, const float* view_cos,
-                                                      const uint8_t* mp_desc, float th, float nnratio, const uint8_t* preassigned,
-                                                      int* match, int* nmatches, void* stream) {
+int pl::search_by_projection_points_launch(const PLKeyPoint* keys, const uint8_t* desc, const int* n, int cap, int B,
+                                           const float* bounds, const float* scale_factors, const int* n_mp, int cap_mp,
+                                           const uint8_t* in_view, const float* proj, const int* level, const float* view_cos,
+                                           const uint8_t* mp_desc, float th, const float* th_frame, const int* desc_row, float nnratio,
+                                           const uint8_t* preassigned, int* match, int* nmatches, void* stream) {
   PL_ARG(keys && desc && n && bounds && scale_factors && n_mp && in_view && proj && level && view_cos && mp_desc && match && nmatches &&
          B >= 1 && cap >= 1 && cap <= 6144 && cap_mp >= 1);
-  ProjPointsArgs A;
+  ProjPointsArgs A{};
+  A.th_frame = th_frame; A.desc_row = desc_row;
   A.keys = keys; A.desc = desc; A.n = n; A.cap = cap; A.bounds = bounds; A.scaleFactors = scale_factors; A.n_mp = n_mp; A.cap_mp = cap_mp;
   A.in_view = in_view; A.proj = proj; A.level = level; A.view_cos = view_cos; A.mp_desc = mp_desc; A.th = th; A.nnratio = nnratio;
   A.preassigned = preassigned; A.match = match; A.nmatches = nmatches;
@@ -1224,6 +1234,14 @@ extern "C" int pl_orb_search_by_projection_points_dev(const PLKeyPoint* keys, co
   k_search_proj_points<<<B, 32, sm, (cudaStream_t)stream>>>(A);
   PL_LAUNCH_CHECK();
   return PL_OK;
+}
+extern "C" int pl_orb_search_by_projection_points_dev(const PLKeyPoint* keys, const uint8_t* desc, const int* n, int cap, int B,
+                                                      const float* bounds, const float* scale_factors, const int* n_mp, int cap_mp,
+                                                      const uint8_t* in_view, const float* proj, const int* level, const float* view_cos,
+                                                      const uint8_t* mp_desc, float th, float nnratio, const uint8_t* preassigned,
+                                                      int* match, int* nmatches, void* stream) {
+  return search_by_projection_points_launch(keys, desc, n, cap, B, bounds, scale_factors, n_mp, cap_mp, in_view, proj, level, view_cos,
+                                            mp_desc, th, nullptr, nullptr, nnratio, preassigned, match, nmatches, stream);
 }
 
 extern "C" int pl_match_bf_knn2(const uint8_t* d1, int n1, const uint8_t* d2, int n2, int* idx, int* dist) {
@@ -1338,7 +1356,7 @@ static int line_search_host(int variant, const void* kls, const double* lfunc, c
   int rc = require_device(); if (rc) return rc;
   Stage s;
   const int cap = std::max(n, 1), capq = std::max(n_q, 1);
-  LineSearchArgs A;
+  LineSearchArgs A{};
   A.kl = (const KeyLine68*)s.up((const uint8_t*)kls, (size_t)n * 68); A.lfunc = s.up(lfunc, (size_t)n * 3); A.desc = s.up(desc, (size_t)n * 32);
   A.n = s.up(&n, 1); A.cap = cap; A.bounds = s.up(bounds, 4);
   A.n_q = s.up(&n_q, 1); A.cap_q = capq; A.q_valid = s.up(q_valid, n_q); A.q_proj = s.up(q_proj, (size_t)n_q * 4);
@@ -1378,14 +1396,15 @@ extern "C" size_t pl_lsd_search_scratch_bytes(int cap, int B) {
   return per * (size_t)B + 256;
 }
 /* variant 0 = SearchByProjection(CurrentFrame, LastFrame, th) (q_length = last lineLength), 1 = (F, vpMapLines, th) (q_view_cos) */
-extern "C" int pl_lsd_search_by_projection_dev(int variant, const void* keylines, const double* linefunc, const uint8_t* desc, const int* n,
-                                               int cap, int B, const float* bounds, const int* n_q, int cap_q, const uint8_t* q_valid,
-                                               const float* q_proj, const uint8_t* q_desc, const float* q_length_or_view_cos, float th,
-                                               float nnratio, const uint8_t* preassigned, int* match, int* nmatches, void* scratch,
-                                               void* stream) {
+int pl::lsd_search_by_projection_launch(int variant, const void* keylines, const double* linefunc, const uint8_t* desc, const int* n,
+                                       int cap, int B, const float* bounds, const int* n_q, int cap_q, const uint8_t* q_valid,
+                                       const float* q_proj, const uint8_t* q_desc, const float* q_length_or_view_cos, float th,
+                                       const float* th_frame, const int* q_desc_row, float nnratio, const uint8_t* preassigned, int* match,
+                                       int* nmatches, void* scratch, void* stream) {
   PL_ARG(keylines && linefunc && desc && n && bounds && n_q && q_valid && q_proj && q_desc && q_length_or_view_cos && match && nmatches &&
          scratch && B >= 1 && cap >= 1 && cap < 60000 && cap_q >= 1 && (variant == 0 || variant == 1));
-  LineSearchArgs A;
+  LineSearchArgs A{};
+  A.th_frame = th_frame; A.q_desc_row = q_desc_row;
   A.kl = (const KeyLine68*)keylines; A.lfunc = linefunc; A.desc = desc; A.n = n; A.cap = cap; A.bounds = bounds;
   A.n_q = n_q; A.cap_q = cap_q; A.q_valid = q_valid; A.q_proj = q_proj; A.q_desc = q_desc;
   A.q_length = variant == 0 ? q_length_or_view_cos : nullptr; A.q_view_cos = variant == 1 ? q_length_or_view_cos : nullptr;
@@ -1398,6 +1417,14 @@ extern "C" int pl_lsd_search_by_projection_dev(int variant, const void* keylines
   k_line_search<<<B, 32, 0, (cudaStream_t)stream>>>(A);
   PL_LAUNCH_CHECK();
   return PL_OK;
+}
+extern "C" int pl_lsd_search_by_projection_dev(int variant, const void* keylines, const double* linefunc, const uint8_t* desc, const int* n,
+                                               int cap, int B, const float* bounds, const int* n_q, int cap_q, const uint8_t* q_valid,
+                                               const float* q_proj, const uint8_t* q_desc, const float* q_length_or_view_cos, float th,
+                                               float nnratio, const uint8_t* preassigned, int* match, int* nmatches, void* scratch,
+                                               void* stream) {
+  return lsd_search_by_projection_launch(variant, keylines, linefunc, desc, n, cap, B, bounds, n_q, cap_q, q_valid, q_proj, q_desc,
+                                         q_length_or_view_cos, th, nullptr, nullptr, nnratio, preassigned, match, nmatches, scratch, stream);
 }
 
 // ------------------------------------------------------------------------------------------------ §8f.2 wrappers

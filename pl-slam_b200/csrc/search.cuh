@@ -1,0 +1,20 @@
+// Launchers of the batched projection searches (match.cu) with two inputs the public entry points leave NULL:
+//   th_frame  [B]       th of each frame (NULL: the scalar th for every frame)
+//   desc_row  [B][cap]  row of the descriptor array that entry (b, i) compares with (NULL: row b * cap + i)
+// pl_track_local_map_dev (track.cu) uses them to search every frame with its own th against the map's descriptors, read
+// through the frame's local-map list instead of a [B][cap_local] gather.
+#pragma once
+#include "common.cuh"
+
+namespace pl {
+int search_by_projection_points_launch(const PLKeyPoint* keys, const uint8_t* desc, const int* n, int cap, int B,
+                                       const float* bounds, const float* scale_factors, const int* n_mp, int cap_mp,
+                                       const uint8_t* in_view, const float* proj, const int* level, const float* view_cos,
+                                       const uint8_t* mp_desc, float th, const float* th_frame, const int* desc_row, float nnratio,
+                                       const uint8_t* preassigned, int* match, int* nmatches, void* stream);
+int lsd_search_by_projection_launch(int variant, const void* keylines, const double* linefunc, const uint8_t* desc, const int* n,
+                                    int cap, int B, const float* bounds, const int* n_q, int cap_q, const uint8_t* q_valid,
+                                    const float* q_proj, const uint8_t* q_desc, const float* q_length_or_view_cos, float th,
+                                    const float* th_frame, const int* q_desc_row, float nnratio, const uint8_t* preassigned, int* match,
+                                    int* nmatches, void* scratch, void* stream);
+}  // namespace pl

@@ -1,0 +1,493 @@
+// Tracking::TrackLocalMapWithLines (src/Tracking.cc:1491-1562) for a batch of frames against a map that stays on the device:
+//   k_track_held             the map indices each frame already holds, sorted (SearchLocalPoints / Lines step 1, :1754-1766)
+//   k_track_frustum_points   Frame::isInFrustum(pMP, 0.5) per (frame, local-list entry) unless the frame holds the point (:1769-1786)
+//   k_track_frustum_lines    Frame::isInFrustum(pML, 0.5) likewise (:1825-1842)
+//   k_search_proj_points     ORBmatcher(0.8).SearchByProjection(F, mvpLocalMapPoints, th)   (match.cu, per-frame th)
+//   k_line_search            LSDmatcher().SearchByProjection(F, mvpLocalMapLines, th)       (match.cu, variant 1)
+//   k_track_build            the PoseOptimization problem in feature order (Optimizer.cc:640-841)
+//   k_pose_opt               Optimizer::PoseOptimization (lm.cu, mode 0, unchanged)
+//   k_track_writeback        masks per feature, mnMatchesInliers / mnLineMatchesInliers and the return value (:1504-1561)
+// The searches read the map's descriptors through the per-entry map index (desc_row) rather than a [B][cap_local][32] gather.
+#include "common.cuh"
+#include "frustum.cuh"
+#include "search.cuh"
+#include <limits.h>
+#include <vector>
+
+struct PLMap {
+  int n_points = 0, n_lines = 0;
+  float *pt_pos = nullptr, *pt_normal = nullptr, *pt_min = nullptr, *pt_max = nullptr;
+  uint8_t* pt_desc = nullptr;
+  double *ln_pos = nullptr, *ln_normal = nullptr;
+  float *ln_min = nullptr, *ln_max = nullptr;
+  uint8_t* ln_desc = nullptr;
+  int* flag = nullptr;            // sticky: an index outside the map was met
+  cudaStream_t stream = nullptr;
+};
+
+namespace pl {
+constexpr int kTrackThreads = 256;
+
+// Sorted map indices of the matches frame b holds (INT_MAX padded) and the pre-assigned flags the searches take.
+__global__ void __launch_bounds__(kTrackThreads) k_track_held(const int* __restrict__ map_in, const int* __restrict__ n, int cap, int n_map,
+                                                              int pow2, int* __restrict__ held, int* __restrict__ n_held,
+                                                              uint8_t* __restrict__ pre, int* __restrict__ flag) {
+  extern __shared__ int s[];
+  __shared__ int cnt;
+  const int b = blockIdx.x, tid = threadIdx.x;
+  const int N = min(n[b], cap);
+  const long long o = (long long)b * cap;
+  if (tid == 0) cnt = 0;
+  __syncthreads();
+  for (int i = tid; i < pow2; i += kTrackThreads) {
+    int v = INT_MAX;
+    if (map_in && i < N) {
+      const int m = map_in[o + i];
+      if (m >= n_map) atomicOr(flag, 1);
+      else if (m >= 0) { v = m; atomicAdd(&cnt, 1); }
+    }
+    s[i] = v;
+    if (i < cap) pre[o + i] = v != INT_MAX;
+  }
+  __syncthreads();
+  for (int k = 2; k <= pow2; k <<= 1)
+    for (int j = k >> 1; j > 0; j >>= 1) {
+      for (int i = tid; i < pow2; i += kTrackThreads) {
+        const int p = i ^ j;
+        if (p > i) {
+          const int a = s[i], c = s[p];
+          if ((a > c) == ((i & k) == 0)) { s[i] = c; s[p] = a; }
+        }
+      }
+      __syncthreads();
+    }
+  for (int i = tid; i < cap; i += kTrackThreads) held[o + i] = s[i];
+  if (tid == 0) n_held[b] = cnt;
+}
+
+__device__ __forceinline__ bool held_by(const int* held, int nh, int m) {
+  int lo = 0, hi = nh;
+  while (lo < hi) { const int mid = (lo + hi) >> 1; if (held[mid] < m) lo = mid + 1; else hi = mid; }
+  return lo < nh && held[lo] == m;
+}
+
+struct TrackFrustumArgs {
+  const float* Tcw0; const float* K; const float* bounds; float logScaleFactor; int nlevels;
+  const int* off; const int* cnt; const int* index; int n_map; int cap_local;
+  const int* held; const int* n_held; int cap;            // held matches, [B][cap] rows
+  uint8_t* in_view; float* proj; int* level; float* view_cos; int* row; int* flag;
+};
+__device__ __forceinline__ int frustum_entry(const TrackFrustumArgs& A, int b, int i, FrustumArgs& F) {
+  const int m = A.index[A.off[b] + i];
+  if (m < 0 || m >= A.n_map) { atomicOr(A.flag, 1); return -1; }
+  A.row[(long long)b * A.cap_local + i] = m;
+  if (held_by(A.held + (long long)b * A.cap, A.n_held[b], m)) return -1;   // mnLastFrameSeen == mnId: mbTrackInView stays false
+  for (int k = 0; k < 16; k++) F.T[k] = A.Tcw0[16 * b + k];
+  camera_center(F.T, F.Ow);
+  for (int k = 0; k < 4; k++) { F.K[k] = A.K[4 * b + k]; F.bounds[k] = A.bounds[k]; }
+  F.logScaleFactor = A.logScaleFactor; F.viewingCosLimit = 0.5f; F.nScaleLevels = A.nlevels; F.n = 0;
+  return m;
+}
+__global__ void __launch_bounds__(128) k_track_frustum_points(TrackFrustumArgs A, const float* __restrict__ pos, const float* __restrict__ normal,
+                                                              const float* __restrict__ minD, const float* __restrict__ maxD) {
+  const int b = blockIdx.y, i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= A.cap_local) return;
+  const long long o = (long long)b * A.cap_local + i;
+  A.in_view[o] = 0; A.proj[2 * o] = A.proj[2 * o + 1] = 0; A.level[o] = 0; A.view_cos[o] = 0; A.row[o] = 0;
+  if (i >= A.cnt[b]) return;
+  FrustumArgs F;
+  const int m = frustum_entry(A, b, i, F);
+  if (m < 0) return;
+  float u, v, vc; int l;
+  if (!frustum_point(F, pos + 3 * (long long)m, normal + 3 * (long long)m, minD[m], maxD[m], u, v, l, vc)) return;
+  A.in_view[o] = 1; A.proj[2 * o] = u; A.proj[2 * o + 1] = v; A.level[o] = l; A.view_cos[o] = vc;
+}
+__global__ void __launch_bounds__(128) k_track_frustum_lines(TrackFrustumArgs A, const double* __restrict__ pos, const double* __restrict__ normal,
+                                                             const float* __restrict__ minD, const float* __restrict__ maxD) {
+  const int b = blockIdx.y, i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= A.cap_local) return;
+  const long long o = (long long)b * A.cap_local + i;
+  A.in_view[o] = 0; for (int k = 0; k < 4; k++) A.proj[4 * o + k] = 0; A.level[o] = 0; A.view_cos[o] = 0; A.row[o] = 0;
+  if (i >= A.cnt[b]) return;
+  FrustumArgs F;
+  const int m = frustum_entry(A, b, i, F);
+  if (m < 0) return;
+  float pr[4], vc; int l;
+  if (!frustum_line(F, pos + 6 * (long long)m, normal + 3 * (long long)m, minD[m], maxD[m], pr, l, vc)) return;
+  A.in_view[o] = 1; for (int k = 0; k < 4; k++) A.proj[4 * o + k] = pr[k];
+  A.level[o] = l; A.view_cos[o] = vc;
+}
+
+// Exclusive block scan of one flag per thread; returns the flag's slot, adds the block's total to *base (all threads).
+__device__ __forceinline__ int block_slot(bool f, int* warp_tot, int& base) {
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const unsigned bal = __ballot_sync(0xffffffffu, f);
+  if (lane == 0) warp_tot[w] = __popc(bal);
+  __syncthreads();
+  int before = base, total = 0;
+  for (int k = 0; k < kTrackThreads / 32; k++) { if (k < w) before += warp_tot[k]; total += warp_tot[k]; }
+  __syncthreads();
+  base += total;
+  return before + __popc(bal & ((1u << lane) - 1u));
+}
+
+struct TrackBuildArgs {
+  const PLKeyPoint* keys; const int* n; int cap; const float* inv_sigma2;
+  const double* lfunc; const int* nl; int capL;
+  const int* pmap_in; const int* lmap_in;               // may be NULL
+  const int* pmatch; const int* lmatch;                 // search results (-2 held, -1, local position)
+  const int* prow; int cap_lp; const int* lrow; int cap_ll;
+  const float* map_pt; const double* map_ln;
+  int* point_map; int* line_map; int* pslot; int* lslot;
+  int* np; float* obs; float* w; float* X; int* nlp; double* lf; double* lX;
+};
+// mvpMapPoints / mvpMapLines after the searches, and the problem in feature order: points then lines
+__global__ void __launch_bounds__(kTrackThreads) k_track_build(TrackBuildArgs A) {
+  __shared__ int warp_tot[kTrackThreads / 32];
+  const int b = blockIdx.x;
+  {
+    const int N = min(A.n[b], A.cap);
+    const long long o = (long long)b * A.cap;
+    int base = 0;
+    for (int c = 0; c < A.cap; c += kTrackThreads) {
+      const int i = c + threadIdx.x;
+      int fm = -1;
+      if (i < N) {
+        const int mm = A.pmatch[o + i];
+        fm = mm == -2 ? A.pmap_in[o + i] : mm >= 0 ? A.prow[(long long)b * A.cap_lp + mm] : -1;
+      }
+      const int slot = block_slot(fm >= 0, warp_tot, base);
+      if (i < A.cap) { A.point_map[o + i] = fm; A.pslot[o + i] = fm >= 0 ? slot : -1; }
+      if (fm >= 0) {
+        const PLKeyPoint k = A.keys[o + i];
+        const long long s = o + slot;
+        A.obs[2 * s] = k.x; A.obs[2 * s + 1] = k.y; A.w[s] = A.inv_sigma2[k.octave];
+        for (int d = 0; d < 3; d++) A.X[3 * s + d] = A.map_pt[3 * (long long)fm + d];
+      }
+    }
+    if (threadIdx.x == 0) A.np[b] = base;
+  }
+  {
+    const int N = min(A.nl[b], A.capL);
+    const long long o = (long long)b * A.capL;
+    int base = 0;
+    for (int c = 0; c < A.capL; c += kTrackThreads) {
+      const int i = c + threadIdx.x;
+      int fm = -1;
+      if (i < N) {
+        const int mm = A.lmatch[o + i];
+        fm = mm == -2 ? A.lmap_in[o + i] : mm >= 0 ? A.lrow[(long long)b * A.cap_ll + mm] : -1;
+      }
+      const int slot = block_slot(fm >= 0, warp_tot, base);
+      if (i < A.capL) { A.line_map[o + i] = fm; A.lslot[o + i] = fm >= 0 ? slot : -1; }
+      if (fm >= 0) {
+        const long long s = o + slot;
+        for (int d = 0; d < 3; d++) A.lf[3 * s + d] = A.lfunc[3 * (o + i) + d];
+        for (int d = 0; d < 6; d++) A.lX[6 * s + d] = A.map_ln[6 * (long long)fm + d];
+      }
+    }
+    if (threadIdx.x == 0) A.nlp[b] = base;
+  }
+}
+
+// mvbOutlier / mvbLineOutlier per feature, the inlier counts (mbOnlyTracking: every non-outlier match) and the return value
+__global__ void __launch_bounds__(kTrackThreads) k_track_writeback(const int* __restrict__ pslot, const uint8_t* __restrict__ pout, int cap,
+                                                                   const int* __restrict__ lslot, const uint8_t* __restrict__ lout, int capL,
+                                                                   const int* __restrict__ min_inliers, uint8_t* __restrict__ point_outlier,
+                                                                   uint8_t* __restrict__ line_outlier, int* __restrict__ inliers,
+                                                                   int* __restrict__ ok) {
+  __shared__ int cnt[2];
+  const int b = blockIdx.x;
+  if (threadIdx.x < 2) cnt[threadIdx.x] = 0;
+  __syncthreads();
+  int np = 0, nl = 0;
+  for (int i = threadIdx.x; i < cap; i += kTrackThreads) {
+    const long long o = (long long)b * cap + i;
+    const int s = pslot[o];
+    const uint8_t f = s >= 0 ? pout[(long long)b * cap + s] : 0;
+    point_outlier[o] = f;
+    np += s >= 0 && !f;
+  }
+  for (int i = threadIdx.x; i < capL; i += kTrackThreads) {
+    const long long o = (long long)b * capL + i;
+    const int s = lslot[o];
+    const uint8_t f = s >= 0 ? lout[(long long)b * capL + s] : 0;
+    line_outlier[o] = f;
+    nl += s >= 0 && !f;
+  }
+  np = warp_sum(np); nl = warp_sum(nl);
+  if ((threadIdx.x & 31) == 0) { atomicAdd(&cnt[0], np); atomicAdd(&cnt[1], nl); }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    inliers[2 * b] = cnt[0]; inliers[2 * b + 1] = cnt[1];
+    ok[b] = cnt[0] >= min_inliers[b];   // < 50 shortly after a relocalisation, < 30 otherwise: false (:1555-1561)
+  }
+}
+
+// ---- scratch layout (one carve for the size query and the call)
+struct TrackScratch {
+  int *tab;                 // [5][B]: pt_off, pt_cnt, ln_off, ln_cnt, min_inliers
+  float* th;                // [B]
+  int *pheld, *nph, *lheld, *nlh;
+  uint8_t *ppre, *lpre;
+  uint8_t* piv; float* pproj; int* plev; float* pvc; int* prow;
+  uint8_t* liv; float* lproj; int* llev; float* lvc; int* lrow;
+  int *pmatch, *pnm, *lmatch, *lnm; void* lsd;
+  int *np, *nl; float *obs, *w, *X; double *lf, *lX;
+  int *pslot, *lslot; uint8_t *pout, *lout; int *inl, *its; double* lm;
+};
+static size_t carve(void* base, int B, int cap, int capL, int cLP, int cLL, TrackScratch* t) {
+  size_t off = 0;
+  auto take = [&](size_t bytes) { void* p = base ? (char*)base + off : nullptr; off += (bytes + 15) / 16 * 16; return p; };
+  const size_t b = B, k = cap, l = capL, lp = cLP, ll = cLL;
+  TrackScratch s;
+  s.tab = (int*)take(5 * b * 4); s.th = (float*)take(b * 4);
+  s.pheld = (int*)take(b * k * 4); s.nph = (int*)take(b * 4); s.lheld = (int*)take(b * l * 4); s.nlh = (int*)take(b * 4);
+  s.ppre = (uint8_t*)take(b * k); s.lpre = (uint8_t*)take(b * l);
+  s.piv = (uint8_t*)take(b * lp); s.pproj = (float*)take(b * lp * 8); s.plev = (int*)take(b * lp * 4); s.pvc = (float*)take(b * lp * 4);
+  s.prow = (int*)take(b * lp * 4);
+  s.liv = (uint8_t*)take(b * ll); s.lproj = (float*)take(b * ll * 16); s.llev = (int*)take(b * ll * 4); s.lvc = (float*)take(b * ll * 4);
+  s.lrow = (int*)take(b * ll * 4);
+  s.pmatch = (int*)take(b * k * 4); s.pnm = (int*)take(b * 4); s.lmatch = (int*)take(b * l * 4); s.lnm = (int*)take(b * 4);
+  s.lsd = take(pl_lsd_search_scratch_bytes(capL, B));
+  s.np = (int*)take(b * 4); s.nl = (int*)take(b * 4);
+  s.obs = (float*)take(b * k * 8); s.w = (float*)take(b * k * 4); s.X = (float*)take(b * k * 12);
+  s.lf = (double*)take(b * l * 24); s.lX = (double*)take(b * l * 48);
+  s.pslot = (int*)take(b * k * 4); s.lslot = (int*)take(b * l * 4); s.pout = (uint8_t*)take(b * k); s.lout = (uint8_t*)take(b * l);
+  s.inl = (int*)take(b * 4); s.its = (int*)take(b * 4);
+  s.lm = (double*)take(pl_pose_optimization_scratch_doubles(B, cap, capL) * 8);
+  if (t) *t = s;
+  return off;
+}
+static int pow2_at_least(int n) { int p = 1; while (p < n) p <<= 1; return p; }
+}  // namespace pl
+using namespace pl;
+
+extern "C" void pl_map_destroy(PLMap* m) {
+  if (!m) return;
+  for (void* p : {(void*)m->pt_pos, (void*)m->pt_normal, (void*)m->pt_min, (void*)m->pt_max, (void*)m->pt_desc, (void*)m->ln_pos,
+                  (void*)m->ln_normal, (void*)m->ln_min, (void*)m->ln_max, (void*)m->ln_desc, (void*)m->flag})
+    cudaFree(p);
+  if (m->stream) cudaStreamDestroy(m->stream);
+  delete m;
+}
+extern "C" int pl_map_create(const PLMapDesc* d, PLMap** out) {
+  PL_ARG(d && out && d->n_points >= 0 && d->n_lines >= 0);
+  PL_ARG(d->n_points == 0 || (d->pt_pos && d->pt_normal && d->pt_min_dist && d->pt_max_dist && d->pt_desc));
+  PL_ARG(d->n_lines == 0 || (d->ln_pos && d->ln_normal && d->ln_min_dist && d->ln_max_dist && d->ln_desc));
+  int rc = require_device(); if (rc) return rc;
+  PLMap* m = new PLMap;
+  m->n_points = d->n_points; m->n_lines = d->n_lines;
+  const size_t np = std::max(d->n_points, 1), nl = std::max(d->n_lines, 1);
+  cudaError_t e = cudaSuccess;
+  auto up = [&](auto** dst, const void* src, size_t n_alloc, size_t bytes) {
+    if (e == cudaSuccess) e = cudaMalloc((void**)dst, n_alloc);
+    if (e == cudaSuccess && bytes) e = cudaMemcpy(*dst, src, bytes, cudaMemcpyHostToDevice);
+  };
+  const size_t P = d->n_points, L = d->n_lines;
+  up(&m->pt_pos, d->pt_pos, np * 12, P * 12); up(&m->pt_normal, d->pt_normal, np * 12, P * 12);
+  up(&m->pt_min, d->pt_min_dist, np * 4, P * 4); up(&m->pt_max, d->pt_max_dist, np * 4, P * 4); up(&m->pt_desc, d->pt_desc, np * 32, P * 32);
+  up(&m->ln_pos, d->ln_pos, nl * 48, L * 48); up(&m->ln_normal, d->ln_normal, nl * 24, L * 24);
+  up(&m->ln_min, d->ln_min_dist, nl * 4, L * 4); up(&m->ln_max, d->ln_max_dist, nl * 4, L * 4); up(&m->ln_desc, d->ln_desc, nl * 32, L * 32);
+  up(&m->flag, nullptr, 4, 0);
+  if (e == cudaSuccess) e = cudaMemset(m->flag, 0, 4);
+  if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking);
+  if (e != cudaSuccess) { set_error("pl_map_create: %s", cudaGetErrorString(e)); pl_map_destroy(m); return PL_ERR_CUDA; }
+  *out = m;
+  return PL_OK;
+}
+extern "C" int pl_map_check_indices(PLMap* m) {
+  PL_ARG(m);
+  int f = 0;
+  PL_CUDA(cudaDeviceSynchronize());
+  PL_CUDA(cudaMemcpy(&f, m->flag, 4, cudaMemcpyDeviceToHost));
+  if (!f) return PL_OK;
+  PL_CUDA(cudaMemset(m->flag, 0, 4));
+  set_error("track_local_map: a local-map entry or a held match named an index outside the map");
+  return PL_ERR_ARG;
+}
+
+extern "C" size_t pl_track_local_map_scratch_bytes(int B, int cap_points, int cap_lines, int cap_local_points, int cap_local_lines) {
+  if (B < 1 || cap_points < 1 || cap_lines < 1) return 0;
+  return carve(nullptr, B, cap_points, cap_lines, std::max(cap_local_points, 1), std::max(cap_local_lines, 1), nullptr);
+}
+
+extern "C" int pl_track_local_map_dev(PLMap* map, const PLTrackFrames* F, const PLTrackLocal* L, const PLTrackOut* O, void* scratch,
+                                      void* stream_) {
+  PL_ARG(map && F && L && O && scratch);
+  const int B = F->B, cap = F->cap_points, capL = F->cap_lines;
+  // cap_points: the point search's limit; cap_lines: k_track_held sorts a frame's held lines in shared memory (4 B per
+  // next_pow2(cap_lines) entries), which fits an SM's 227 KB up to 32768
+  PL_ARG(B >= 1 && cap >= 1 && cap <= 6144 && capL >= 1 && capL <= 32768 && F->nlevels >= 1);
+  PL_ARG(F->keys_un && F->desc && F->n && F->keylines && F->line_func && F->line_desc && F->nl && F->bounds && F->scale_factors &&
+         F->inv_level_sigma2 && F->Tcw0 && F->K);
+  PL_ARG(L->pt_offset && L->pt_count && L->ln_offset && L->ln_count && L->frames_since_reloc && L->cap_local_points >= 0 &&
+         L->cap_local_lines >= 0 && L->n_pt_index >= 0 && L->n_ln_index >= 0);
+  PL_ARG(O->Tcw && O->point_map && O->point_outlier && O->line_map && O->line_outlier && O->inliers && O->ok);
+  const int cLP = std::max(L->cap_local_points, 1), cLL = std::max(L->cap_local_lines, 1);
+  // host-side checks before anything is enqueued
+  std::vector<int> tab((size_t)5 * B);
+  std::vector<float> th(B);
+  bool any_pt = false, any_ln = false;
+  for (int b = 0; b < B; b++) {
+    if (L->pt_count[b] < 0 || L->pt_count[b] > L->cap_local_points || L->ln_count[b] < 0 || L->ln_count[b] > L->cap_local_lines) {
+      set_error("frame %d has %d local points and %d local lines; the capacities are %d and %d", b, L->pt_count[b], L->ln_count[b],
+                L->cap_local_points, L->cap_local_lines);
+      return PL_ERR_ARG;
+    }
+    if (L->pt_offset[b] < 0 || (long long)L->pt_offset[b] + L->pt_count[b] > L->n_pt_index || L->ln_offset[b] < 0 ||
+        (long long)L->ln_offset[b] + L->ln_count[b] > L->n_ln_index) {
+      set_error("frame %d's local lists [%d, +%d) / [%d, +%d) leave the index arrays of %d points / %d lines", b, L->pt_offset[b],
+                L->pt_count[b], L->ln_offset[b], L->ln_count[b], L->n_pt_index, L->n_ln_index);
+      return PL_ERR_ARG;
+    }
+    any_pt |= L->pt_count[b] > 0; any_ln |= L->ln_count[b] > 0;
+    tab[b] = L->pt_offset[b]; tab[B + b] = L->pt_count[b]; tab[2 * B + b] = L->ln_offset[b]; tab[3 * B + b] = L->ln_count[b];
+    tab[4 * B + b] = L->frames_since_reloc[b] < L->max_frames ? 50 : 30;
+    th[b] = L->frames_since_reloc[b] < 2 ? 5.0f : 1.0f;   // if(mCurrentFrame.mnId < mnLastRelocFrameId + 2) th = 5
+  }
+  PL_ARG(!any_pt || L->pt_index);
+  PL_ARG(!any_ln || L->ln_index);
+  cudaStream_t st = stream_ ? (cudaStream_t)stream_ : map->stream;
+  TrackScratch s;
+  carve(scratch, B, cap, capL, cLP, cLL, &s);
+  // pageable sources: the copies are staged before cudaMemcpyAsync returns, so the vectors may go
+  PL_CUDA(cudaMemcpyAsync(s.tab, tab.data(), tab.size() * 4, cudaMemcpyHostToDevice, st));
+  PL_CUDA(cudaMemcpyAsync(s.th, th.data(), th.size() * 4, cudaMemcpyHostToDevice, st));
+  const int* d_poff = s.tab; const int* d_pcnt = s.tab + B; const int* d_loff = s.tab + 2 * B; const int* d_lcnt = s.tab + 3 * B;
+  const int* d_min_inl = s.tab + 4 * B;
+  // outputs the caller asked for are the working arrays themselves
+  uint8_t* piv = O->pt_in_view ? O->pt_in_view : s.piv; float* pproj = O->pt_proj ? O->pt_proj : s.pproj;
+  int* plev = O->pt_level ? O->pt_level : s.plev; float* pvc = O->pt_view_cos ? O->pt_view_cos : s.pvc;
+  uint8_t* liv = O->ln_in_view ? O->ln_in_view : s.liv; float* lproj = O->ln_proj ? O->ln_proj : s.lproj;
+  int* llev = O->ln_level ? O->ln_level : s.llev; float* lvc = O->ln_view_cos ? O->ln_view_cos : s.lvc;
+  int* pmatch = O->pt_match ? O->pt_match : s.pmatch; int* lmatch = O->ln_match ? O->ln_match : s.lmatch;
+  int* np = O->prob_n_points ? O->prob_n_points : s.np; int* nl = O->prob_n_lines ? O->prob_n_lines : s.nl;
+  float* obs = O->prob_pt_obs ? O->prob_pt_obs : s.obs; float* w = O->prob_pt_inv_sigma2 ? O->prob_pt_inv_sigma2 : s.w;
+  float* X = O->prob_pt_Xw ? O->prob_pt_Xw : s.X;
+  double* lf = O->prob_line_func ? O->prob_line_func : s.lf; double* lX = O->prob_line_Xw ? O->prob_line_Xw : s.lX;
+
+  // 1. matches already held
+  const int p2 = pow2_at_least(cap), l2 = pow2_at_least(capL);
+  PL_CUDA(cudaFuncSetAttribute(k_track_held, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(std::max(p2, l2) * 4)));
+  k_track_held<<<B, kTrackThreads, p2 * 4, st>>>(F->point_map_in, F->n, cap, map->n_points, p2, s.pheld, s.nph, s.ppre, map->flag);
+  PL_LAUNCH_CHECK();
+  k_track_held<<<B, kTrackThreads, l2 * 4, st>>>(F->line_map_in, F->nl, capL, map->n_lines, l2, s.lheld, s.nlh, s.lpre, map->flag);
+  PL_LAUNCH_CHECK();
+  // 2. isInFrustum(., 0.5) per (frame, local entry)
+  TrackFrustumArgs A;
+  A.Tcw0 = F->Tcw0; A.K = F->K; A.bounds = F->bounds; A.logScaleFactor = F->log_scale_factor; A.nlevels = F->nlevels; A.flag = map->flag;
+  A.off = d_poff; A.cnt = d_pcnt; A.index = L->pt_index; A.n_map = map->n_points; A.cap_local = cLP; A.held = s.pheld; A.n_held = s.nph;
+  A.cap = cap; A.in_view = piv; A.proj = pproj; A.level = plev; A.view_cos = pvc; A.row = s.prow;
+  k_track_frustum_points<<<dim3((cLP + 127) / 128, B), 128, 0, st>>>(A, map->pt_pos, map->pt_normal, map->pt_min, map->pt_max);
+  PL_LAUNCH_CHECK();
+  A.off = d_loff; A.cnt = d_lcnt; A.index = L->ln_index; A.n_map = map->n_lines; A.cap_local = cLL; A.held = s.lheld; A.n_held = s.nlh;
+  A.cap = capL; A.in_view = liv; A.proj = lproj; A.level = llev; A.view_cos = lvc; A.row = s.lrow;
+  k_track_frustum_lines<<<dim3((cLL + 127) / 128, B), 128, 0, st>>>(A, map->ln_pos, map->ln_normal, map->ln_min, map->ln_max);
+  PL_LAUNCH_CHECK();
+  // 3. the two projection searches, every frame with its own th, descriptors read through the entry's map index
+  int rc;
+  if ((rc = search_by_projection_points_launch(F->keys_un, F->desc, F->n, cap, B, F->bounds, F->scale_factors, d_pcnt, cLP, piv, pproj, plev,
+                                               pvc, map->pt_desc, 1.0f, s.th, s.prow, 0.8f, s.ppre, pmatch, s.pnm, st))) return rc;
+  if ((rc = lsd_search_by_projection_launch(1, F->keylines, F->line_func, F->line_desc, F->nl, capL, B, F->bounds, d_lcnt, cLL, liv, lproj,
+                                            map->ln_desc, lvc, 1.0f, s.th, s.lrow, 0.7f, s.lpre, lmatch, s.lnm, s.lsd, st))) return rc;
+  // 4. the pose problem in feature order, then PoseOptimization
+  TrackBuildArgs Bd;
+  Bd.keys = F->keys_un; Bd.n = F->n; Bd.cap = cap; Bd.inv_sigma2 = F->inv_level_sigma2; Bd.lfunc = F->line_func; Bd.nl = F->nl; Bd.capL = capL;
+  Bd.pmap_in = F->point_map_in; Bd.lmap_in = F->line_map_in; Bd.pmatch = pmatch; Bd.lmatch = lmatch;
+  Bd.prow = s.prow; Bd.cap_lp = cLP; Bd.lrow = s.lrow; Bd.cap_ll = cLL; Bd.map_pt = map->pt_pos; Bd.map_ln = map->ln_pos;
+  Bd.point_map = O->point_map; Bd.line_map = O->line_map; Bd.pslot = s.pslot; Bd.lslot = s.lslot;
+  Bd.np = np; Bd.obs = obs; Bd.w = w; Bd.X = X; Bd.nlp = nl; Bd.lf = lf; Bd.lX = lX;
+  k_track_build<<<B, kTrackThreads, 0, st>>>(Bd);
+  PL_LAUNCH_CHECK();
+  if ((rc = pl_pose_optimization_dev(0, B, F->Tcw0, F->K, np, cap, obs, w, X, nl, capL, lf, lX, O->Tcw, s.pout, s.lout, s.inl, s.its, s.lm,
+                                     st))) return rc;
+  // 5. write back per feature
+  k_track_writeback<<<B, kTrackThreads, 0, st>>>(s.pslot, s.pout, cap, s.lslot, s.lout, capL, d_min_inl, O->point_outlier, O->line_outlier,
+                                                  O->inliers, O->ok);
+  PL_LAUNCH_CHECK();
+  return PL_OK;
+}
+
+// B = 1 on host pointers: stage, run, copy back, check the index flag.  The device arrays are sized by the counts.
+extern "C" int pl_track_local_map(PLMap* map, const PLTrackFrames* F, const PLTrackLocal* L, const PLTrackOut* O) {
+  PL_ARG(map && F && L && O && F->B == 1 && F->n && F->nl && L->pt_count && L->ln_count && L->pt_offset && L->ln_offset);
+  PL_ARG(O->Tcw && O->point_map && O->point_outlier && O->line_map && O->line_outlier && O->inliers);
+  const int n = *F->n, nl = *F->nl;
+  PL_ARG(n >= 0 && nl >= 0 && n <= F->cap_points && nl <= F->cap_lines && F->nlevels >= 1);
+  PL_ARG(L->pt_count[0] >= 0 && L->ln_count[0] >= 0 && L->pt_offset[0] >= 0 && L->ln_offset[0] >= 0);
+  PL_ARG(L->pt_count[0] <= L->cap_local_points && L->ln_count[0] <= L->cap_local_lines);
+  PL_ARG((long long)L->pt_offset[0] + L->pt_count[0] <= L->n_pt_index && (long long)L->ln_offset[0] + L->ln_count[0] <= L->n_ln_index);
+  int rc = require_device(); if (rc) return rc;
+  const int cap = std::max(n, 1), capL = std::max(nl, 1);
+  const size_t lp = (size_t)L->pt_count[0], ll = (size_t)L->ln_count[0];
+  const int cLP = std::max((int)lp, 1), cLL = std::max((int)ll, 1);
+  std::vector<void*> fr;
+  cudaError_t e = cudaSuccess;
+  auto dal = [&](size_t bytes) -> void* {
+    void* p = nullptr;
+    if (e == cudaSuccess) e = cudaMalloc(&p, std::max<size_t>(bytes, 16));
+    if (e == cudaSuccess) { fr.push_back(p); e = cudaMemset(p, 0, std::max<size_t>(bytes, 16)); }
+    return e == cudaSuccess ? p : nullptr;
+  };
+  auto dup = [&](const void* h, size_t bytes) -> void* {
+    void* p = dal(bytes);
+    if (p && h && bytes) e = cudaMemcpy(p, h, bytes, cudaMemcpyHostToDevice);
+    return e == cudaSuccess ? p : nullptr;
+  };
+  PLTrackFrames D = *F;
+  D.cap_points = cap; D.cap_lines = capL;
+  D.keys_un = (const PLKeyPoint*)dup(F->keys_un, (size_t)n * sizeof(PLKeyPoint)); D.desc = (const uint8_t*)dup(F->desc, (size_t)n * 32);
+  D.n = (const int*)dup(&n, 4);
+  D.keylines = dup(F->keylines, (size_t)nl * 68); D.line_func = (const double*)dup(F->line_func, (size_t)nl * 24);
+  D.line_desc = (const uint8_t*)dup(F->line_desc, (size_t)nl * 32); D.nl = (const int*)dup(&nl, 4);
+  D.bounds = (const float*)dup(F->bounds, 16); D.scale_factors = (const float*)dup(F->scale_factors, (size_t)F->nlevels * 4);
+  D.inv_level_sigma2 = (const float*)dup(F->inv_level_sigma2, (size_t)F->nlevels * 4);
+  D.Tcw0 = (const float*)dup(F->Tcw0, 64); D.K = (const float*)dup(F->K, 16);
+  D.point_map_in = F->point_map_in ? (const int*)dup(F->point_map_in, (size_t)n * 4) : nullptr;
+  D.line_map_in = F->line_map_in ? (const int*)dup(F->line_map_in, (size_t)nl * 4) : nullptr;
+  const int zero = 0;
+  PLTrackLocal DL = *L;
+  DL.pt_offset = &zero; DL.ln_offset = &zero; DL.cap_local_points = cLP; DL.cap_local_lines = cLL;
+  DL.n_pt_index = (int)lp; DL.n_ln_index = (int)ll;
+  DL.pt_index = lp ? (const int*)dup(L->pt_index + L->pt_offset[0], lp * 4) : nullptr;
+  DL.ln_index = ll ? (const int*)dup(L->ln_index + L->ln_offset[0], ll * 4) : nullptr;
+  struct Field { void* host; size_t bytes; void* dev; };
+  std::vector<Field> outs;
+  // required outputs always get a device array; optional ones only when asked for
+  auto dout = [&](void* h, size_t bytes, size_t alloc) -> void* {
+    if (!h) return nullptr;
+    void* d = dal(alloc); outs.push_back({h, bytes, d}); return d;
+  };
+  int ok_h = 0;
+  PLTrackOut DO;
+  DO.Tcw = (float*)dout(O->Tcw, 64, 64); DO.ok = (int*)dout(&ok_h, 4, 4); DO.inliers = (int*)dout(O->inliers, 8, 8);
+  DO.point_map = (int*)dout(O->point_map, (size_t)n * 4, (size_t)cap * 4); DO.point_outlier = (uint8_t*)dout(O->point_outlier, n, cap);
+  DO.line_map = (int*)dout(O->line_map, (size_t)nl * 4, (size_t)capL * 4); DO.line_outlier = (uint8_t*)dout(O->line_outlier, nl, capL);
+  DO.pt_in_view = (uint8_t*)dout(O->pt_in_view, lp, cLP); DO.pt_proj = (float*)dout(O->pt_proj, lp * 8, (size_t)cLP * 8);
+  DO.pt_level = (int*)dout(O->pt_level, lp * 4, (size_t)cLP * 4); DO.pt_view_cos = (float*)dout(O->pt_view_cos, lp * 4, (size_t)cLP * 4);
+  DO.ln_in_view = (uint8_t*)dout(O->ln_in_view, ll, cLL); DO.ln_proj = (float*)dout(O->ln_proj, ll * 16, (size_t)cLL * 16);
+  DO.ln_level = (int*)dout(O->ln_level, ll * 4, (size_t)cLL * 4); DO.ln_view_cos = (float*)dout(O->ln_view_cos, ll * 4, (size_t)cLL * 4);
+  DO.pt_match = (int*)dout(O->pt_match, (size_t)n * 4, (size_t)cap * 4); DO.ln_match = (int*)dout(O->ln_match, (size_t)nl * 4, (size_t)capL * 4);
+  DO.prob_n_points = (int*)dout(O->prob_n_points, 4, 4); DO.prob_n_lines = (int*)dout(O->prob_n_lines, 4, 4);
+  DO.prob_pt_obs = (float*)dout(O->prob_pt_obs, (size_t)n * 8, (size_t)cap * 8);
+  DO.prob_pt_inv_sigma2 = (float*)dout(O->prob_pt_inv_sigma2, (size_t)n * 4, (size_t)cap * 4);
+  DO.prob_pt_Xw = (float*)dout(O->prob_pt_Xw, (size_t)n * 12, (size_t)cap * 12);
+  DO.prob_line_func = (double*)dout(O->prob_line_func, (size_t)nl * 24, (size_t)capL * 24);
+  DO.prob_line_Xw = (double*)dout(O->prob_line_Xw, (size_t)nl * 48, (size_t)capL * 48);
+  void* scr = dal(pl_track_local_map_scratch_bytes(1, cap, capL, cLP, cLL));
+  int ret = PL_ERR_CUDA;
+  if (e != cudaSuccess || !scr) set_error("track_local_map: %s", cudaGetErrorString(e));
+  else {
+    ret = pl_track_local_map_dev(map, &D, &DL, &DO, scr, map->stream);
+    if (ret == PL_OK) {
+      e = cudaStreamSynchronize(map->stream);
+      for (const Field& f : outs) if (e == cudaSuccess && f.bytes) e = cudaMemcpy(f.host, f.dev, f.bytes, cudaMemcpyDeviceToHost);
+      if (e != cudaSuccess) { set_error("track_local_map: %s", cudaGetErrorString(e)); ret = PL_ERR_CUDA; }
+    }
+  }
+  for (void* p : fr) cudaFree(p);
+  if (ret != PL_OK) return ret;
+  if ((rc = pl_map_check_indices(map))) return rc;
+  return ok_h;
+}
