@@ -550,6 +550,12 @@ int pl_track_local_map_dev(PLMap* map, const PLTrackFrames* frames, const PLTrac
 /* The same for ONE frame on host pointers (frames->B must be 1; caps = the counts, or larger); synchronous.  Returns ok (0 / 1)
  * or an error. */
 int pl_track_local_map(PLMap* map, const PLTrackFrames* frames, const PLTrackLocal* local, const PLTrackOut* out);
+/* The same step after pl_track_motion_model_dev: point_seen [B][cap_points] / line_seen [B][cap_lines] (device, may be NULL) are
+ * the motion model's outputs of the same names, the map entries it discarded as outliers (-1 none).  Such an entry is skipped by
+ * the frustum test exactly like a held match (in_view = 0: the reference stamped it mnLastFrameSeen = mnId, :1384-1390, :1778,
+ * :1833) but is not pre-assigned in the search.  With both NULL this is pl_track_local_map_dev, bit for bit. */
+int pl_track_local_map_seen_dev(PLMap* map, const PLTrackFrames* frames, const int* point_seen, const int* line_seen,
+                                const PLTrackLocal* local, const PLTrackOut* out, void* scratch, void* stream);
 /* The step on the features of the front end's LAST step (pl_frontend_run / run_dev / submit): frames 0 .. B-1 of that step
  * (PL_ERR_ARG if B exceeds that step's batch or no step has run), with the
  * handle's bounds and ORB tables; Tcw0 / K / point_map_in / line_map_in are device arrays ([B][capK] / [B][capL] layouts of
@@ -557,6 +563,58 @@ int pl_track_local_map(PLMap* map, const PLTrackFrames* frames, const PLTrackLoc
 int pl_frontend_track_local_map_dev(PLFrontend* h, PLMap* map, int B, const float* Tcw0, const float* K, const int* point_map_in,
                                     const int* line_map_in, const PLTrackLocal* local, const PLTrackOut* out, void* scratch,
                                     void* stream);
+
+/* ------------------------------------------------------------------ the constant-velocity motion model against a fixed map
+ * Tracking::TrackWithMotionModel (src/Tracking.cc:1316-1431), monocular, in localisation mode, for B independent frames.
+ *
+ * The last frames ([B][cap] device arrays, host with B = 1 for pl_track_motion_model), with the caps of the current frames:
+ *   keys_un = mLastFrame.mvKeysUn (octave and angle are read), n = N; keylines = mvKeylinesUn (lineLength is read), nl = NL;
+ *   point_map / point_outlier = mvpMapPoints (map index, -1 none) / mvbOutlier; line_map / line_outlier likewise for lines;
+ *   Tcw [B][16] = mLastFrame.mTcw after the caller's UpdateLastFrame (Tlr * pRef->GetPose(), :1242-1245); velocity [B][16] =
+ *   mVelocity.  A -1 or outlier entry is skipped; a non-negative index outside the map sets the map's index flag and is skipped. */
+typedef struct PLTrackLast {
+  const PLKeyPoint* keys_un; const int* n; const void* keylines; const int* nl;
+  const int* point_map; const uint8_t* point_outlier; const int* line_map; const uint8_t* line_outlier;
+  const float* Tcw; const float* velocity;
+} PLTrackLast;
+/* Results (device arrays, host for pl_track_motion_model).  Always written: Tcw [B][16]; point_map [B][cap_points] / line_map
+ * [B][cap_lines] = mvpMapPoints / mvpMapLines (map index or -1) after the discard; point_seen / line_seen (same layouts) = the map
+ * index of a match discarded as an outlier (mnLastFrameSeen = mnId, mbTrackInView = false; :1384-1390, :1404-1409), else -1 - pass
+ * them to pl_track_local_map_seen_dev; nmatches [B][2] = {nmatches, lmatches} after the discard; ok [B] = the return value
+ * (nmatches > 20); vo [B] (in / out) = mbVO = nmatchesMap < 10, written only by frames that reach the pose optimisation.  A fixed
+ * map's entries all have Observations() > 0, so nmatchesMap counts every match left.  There are no outlier outputs: after the
+ * discard every mvbOutlier / mvbLineOutlier is false, and a frame that returned early still has a new Frame's all-false flags.
+ * Optional (NULL = kept in the scratch): guess [B][16] = mVelocity * mLastFrame.mTcw; pt_match [B][cap_points] = the search at
+ * th = 15 and pt_match_retry = the search at 30 (last-frame keypoint index or -1; written only for frames with retried [B] = 1);
+ * ln_match [B][cap_lines] (last-frame line index or -1); the line candidates per LAST-frame line, ln_in_view / ln_proj [.][4] /
+ * ln_level / ln_view_cos [B][cap_lines] (isInFrustum at the guess; 0 for skipped lines); and the PoseOptimization problem exactly as
+ * pl_pose_optimization_dev reads it (empty for a frame that returned early). */
+typedef struct PLTrackMotionOut {
+  float* Tcw; int* point_map; int* line_map; int* point_seen; int* line_seen; int* nmatches; int* ok; int* vo;
+  float* guess; int* pt_match; int* pt_match_retry; uint8_t* retried; int* ln_match;
+  uint8_t* ln_in_view; float* ln_proj; int* ln_level; float* ln_view_cos;
+  int* prob_n_points; float* prob_pt_obs; float* prob_pt_inv_sigma2; float* prob_pt_Xw;
+  int* prob_n_lines; double* prob_line_func; double* prob_line_Xw;
+} PLTrackMotionOut;
+/* Per frame b, in the reference's order: the guess mVelocity * mLastFrame.mTcw (cv::Mat's fp32 4x4 product, :1332); ORBmatcher(0.9,
+ * true).SearchByProjection(Current, Last, 15, mono) (ORBmatcher.cc:1441-1585) and LSDmatcher().SearchByProjection(Current, Last, 15)
+ * (LSDmatcher.cpp:95-190, candidates isInFrustum(pML, 0.5) at the guess with frame b's K); the point search again at 30 if it found
+ * under 20 (:1354-1358; lines are not searched again); nmatches < 20 && lmatches < 5: return false with the guess and the search's
+ * matches (:1360-1361); PoseOptimization (mode 0, from the guess); the outliers discarded (:1376-1419), mbVO and the return value.
+ * frames: PLTrackFrames with Tcw0, point_map_in and line_map_in NULL (PL_ERR_ARG otherwise: the guess is computed and the matches
+ * start empty).  PL_ERR_ARG before anything is enqueued for a NULL required pointer, cap_points outside 1..6144 or cap_lines outside
+ * 1..32768.  The caller keeps the map statistics and the LOST / no-velocity / mbVO branches (Relocalization, TrackReferenceKeyFrame).
+ * Scratch: pl_track_motion_model_scratch_bytes(B, caps) bytes of device memory (16-byte aligned).  Asynchronous on `stream` (NULL =
+ * the map's stream); call pl_map_check_indices after synchronising. */
+size_t pl_track_motion_model_scratch_bytes(int B, int cap_points, int cap_lines);
+int pl_track_motion_model_dev(PLMap* map, const PLTrackFrames* frames, const PLTrackLast* last, const PLTrackMotionOut* out,
+                              void* scratch, void* stream);
+/* The same for ONE frame on host pointers (B = 1; the counts of both frames within the caps); synchronous.  Returns ok (0 / 1) or
+ * an error (PL_ERR_ARG also when the index flag was set). */
+int pl_track_motion_model(PLMap* map, const PLTrackFrames* frames, const PLTrackLast* last, const PLTrackMotionOut* out);
+/* mVelocity = mCurrentFrame.mTcw * LastTwc (Tracking.cc:492-501), LastTwc = [Rcw^T | Ow] of Tcw_last (Ow as Frame::UpdatePoseMatrices
+ * computes it), with the guess's fp32 4x4 product; velocity[b] is written only where ok[b].  Device arrays [B][16], ok [B]. */
+int pl_track_velocity_dev(int B, const float* Tcw, const float* Tcw_last, const int* ok, float* velocity, void* stream);
 
 /* ------------------------------------------------------------------ multi-GPU exchange (SURVEY.md §8e)
  * Frames shard across the GPUs of one box with no data-path collective; the ONE exchange is an all-gather of the per-frame

@@ -920,6 +920,12 @@ def _track_lib():
         L.pl_track_local_map_dev.argtypes = [vp, C.POINTER(PLTrackFrames), C.POINTER(PLTrackLocal), C.POINTER(PLTrackOut), vp, vp]
         L.pl_track_local_map.argtypes = [vp, C.POINTER(PLTrackFrames), C.POINTER(PLTrackLocal), C.POINTER(PLTrackOut)]
         L.pl_frontend_track_local_map_dev.argtypes = [vp, vp, C.c_int, vp, vp, vp, vp, C.POINTER(PLTrackLocal), C.POINTER(PLTrackOut), vp, vp]
+        L.pl_track_local_map_seen_dev.argtypes = [vp, C.POINTER(PLTrackFrames), vp, vp, C.POINTER(PLTrackLocal), C.POINTER(PLTrackOut), vp, vp]
+        L.pl_track_motion_model_scratch_bytes.argtypes = [C.c_int] * 3
+        L.pl_track_motion_model_scratch_bytes.restype = C.c_size_t
+        L.pl_track_motion_model_dev.argtypes = [vp, C.POINTER(PLTrackFrames), C.POINTER(PLTrackLast), C.POINTER(PLTrackMotionOut), vp, vp]
+        L.pl_track_motion_model.argtypes = [vp, C.POINTER(PLTrackFrames), C.POINTER(PLTrackLast), C.POINTER(PLTrackMotionOut)]
+        L.pl_track_velocity_dev.argtypes = [C.c_int, vp, vp, vp, vp, vp]
         L._track_types = True
     return L
 
@@ -1009,14 +1015,16 @@ def _run_dev(call, B, cap, capL, cLP, cLL, taps, keep, torch):
     return out
 
 
-def track_local_map(map, frames, local, taps=False, host=False):
+def track_local_map(map, frames, local, taps=False, host=False, seen=None):
     """Tracking::TrackLocalMapWithLines (localisation mode) for B frames against `map` (pl_track_local_map_dev).
 
     frames: dict(keys_un [B][cap] KP_DTYPE, desc [B][cap][32], n [B], keylines [B][capL] KEYLINE_DTYPE, line_func [B][capL][3],
     line_desc [B][capL][32], nl [B], bounds [4], scale_factors, inv_level_sigma2, log_scale_factor, Tcw0 [B][4][4], K [B][4],
     point_map_in / line_map_in ([B][cap] map index or -1; optional)).  local: see _local_struct.
     Returns dict(Tcw, point_map, point_outlier, line_map, line_outlier, inliers [B][2], ok [B]) plus, with taps=True, the
-    intermediates of PLTrackOut.  host=True (B = 1 only) calls the host-pointer entry pl_track_local_map instead."""
+    intermediates of PLTrackOut.  host=True (B = 1 only) calls the host-pointer entry pl_track_local_map instead.
+    seen: dict with point_seen [B][cap] / line_seen [B][capL] (track_motion_model's outputs): the map entries the motion model
+    discarded, skipped by the frustum test like held matches (pl_track_local_map_seen_dev); not with host=True."""
     L = _track_lib()
     B, cap = frames["keys_un"].shape[:2]
     capL = frames["keylines"].shape[1]
@@ -1031,6 +1039,8 @@ def track_local_map(map, frames, local, taps=False, host=False):
             arr[k] = np.ascontiguousarray(frames[k], np.int32)
     if host:
         assert B == 1
+        if seen is not None:
+            raise ValueError("track_local_map: seen= needs the device entry (host=False)")
         keep = []
         s, cLP, cLL = _local_struct(local, 1, keep, lambda a: (a, _p(a)))
         F = PLTrackFrames(1, _p(arr["keys_un"]), _p(arr["desc"]), _p(arr["n"]), cap, _p(arr["keylines"]), _p(arr["line_func"]),
@@ -1051,8 +1061,13 @@ def track_local_map(map, frames, local, taps=False, host=False):
     F = PLTrackFrames(B, d["keys_un"], d["desc"], d["n"], cap, d["keylines"], d["line_func"], d["line_desc"], d["nl"], capL, d["bounds"],
                       d["scale_factors"], d["inv_level_sigma2"], nlev, float(frames["log_scale_factor"]), d["Tcw0"], d["K"],
                       d.get("point_map_in"), d.get("line_map_in"))
-    out = _run_dev(lambda o, scr: L.pl_track_local_map_dev(map._h, C.byref(F), C.byref(s), C.byref(o), scr, None),
-                   B, cap, capL, cLP, cLL, taps, keep, torch)
+    if seen is None:
+        call = lambda o, scr: L.pl_track_local_map_dev(map._h, C.byref(F), C.byref(s), C.byref(o), scr, None)   # noqa: E731
+    else:
+        ps = to_dev(np.ascontiguousarray(seen["point_seen"], np.int32).reshape(B, cap))[1]
+        ls = to_dev(np.ascontiguousarray(seen["line_seen"], np.int32).reshape(B, capL))[1]
+        call = lambda o, scr: L.pl_track_local_map_seen_dev(map._h, C.byref(F), ps, ls, C.byref(s), C.byref(o), scr, None)   # noqa: E731
+    out = _run_dev(call, B, cap, capL, cLP, cLL, taps, keep, torch)
     map.check_indices()
     return out
 
@@ -1074,3 +1089,103 @@ def _frontend_track_local_map(self, map, Tcw0, K, local, point_map_in=None, line
 
 
 Frontend.track_local_map = _frontend_track_local_map
+
+
+# ---------------------------------------------------------------------------------------------- the constant-velocity motion model
+class PLTrackLast(C.Structure):
+    _fields_ = [(k, vp) for k in ("keys_un", "n", "keylines", "nl", "point_map", "point_outlier", "line_map", "line_outlier", "Tcw",
+                                  "velocity")]
+
+
+_MM_OUT = ["Tcw", "point_map", "line_map", "point_seen", "line_seen", "nmatches", "ok", "vo", "guess", "pt_match", "pt_match_retry",
+           "retried", "ln_match", "ln_in_view", "ln_proj", "ln_level", "ln_view_cos", "prob_n_points", "prob_pt_obs", "prob_pt_inv_sigma2",
+           "prob_pt_Xw", "prob_n_lines", "prob_line_func", "prob_line_Xw"]
+
+
+class PLTrackMotionOut(C.Structure):
+    _fields_ = [(k, vp) for k in _MM_OUT]
+
+
+def _mm_shapes(B, cap, capL):
+    return dict(Tcw=((B, 4, 4), np.float32), point_map=((B, cap), np.int32), line_map=((B, capL), np.int32), point_seen=((B, cap), np.int32),
+                line_seen=((B, capL), np.int32), nmatches=((B, 2), np.int32), ok=((B,), np.int32), vo=((B,), np.int32),
+                guess=((B, 4, 4), np.float32), pt_match=((B, cap), np.int32), pt_match_retry=((B, cap), np.int32), retried=((B,), np.uint8),
+                ln_match=((B, capL), np.int32), ln_in_view=((B, capL), np.uint8), ln_proj=((B, capL, 4), np.float32),
+                ln_level=((B, capL), np.int32), ln_view_cos=((B, capL), np.float32), prob_n_points=((B,), np.int32),
+                prob_pt_obs=((B, cap, 2), np.float32), prob_pt_inv_sigma2=((B, cap), np.float32), prob_pt_Xw=((B, cap, 3), np.float32),
+                prob_n_lines=((B,), np.int32), prob_line_func=((B, capL, 3), np.float64), prob_line_Xw=((B, capL, 6), np.float64))
+
+
+def track_motion_model(map, frames, last, taps=False, host=False):
+    """Tracking::TrackWithMotionModel (monocular, localisation mode) for B frames against `map` (pl_track_motion_model_dev).
+
+    frames: as for track_local_map, without Tcw0 / point_map_in / line_map_in.  last: dict(keys_un [B][cap], n [B], keylines
+    [B][capL], nl [B], point_map / point_outlier [B][cap], line_map / line_outlier [B][capL], Tcw [B][4][4] (after UpdateLastFrame),
+    velocity [B][4][4], vo [B] (optional, the mbVO passed in; default 0)), with the caps of `frames`.
+    Returns dict(Tcw, point_map, line_map, point_seen, line_seen, nmatches [B][2], ok [B], vo [B]) plus, with taps=True, the
+    intermediates of PLTrackMotionOut.  host=True (B = 1 only) calls the host-pointer entry pl_track_motion_model instead."""
+    L = _track_lib()
+    B, cap = frames["keys_un"].shape[:2]
+    capL = frames["keylines"].shape[1]
+    assert last["keys_un"].shape[:2] == (B, cap) and last["keylines"].shape[:2] == (B, capL)
+    nlev = len(frames["scale_factors"])
+    arr = dict(keys_un=np.ascontiguousarray(frames["keys_un"], KP_DTYPE), desc=np.ascontiguousarray(frames["desc"], np.uint8),
+               n=np.ascontiguousarray(frames["n"], np.int32), keylines=np.ascontiguousarray(frames["keylines"], KEYLINE_DTYPE),
+               line_func=np.ascontiguousarray(frames["line_func"], np.float64), line_desc=np.ascontiguousarray(frames["line_desc"], np.uint8),
+               nl=np.ascontiguousarray(frames["nl"], np.int32), bounds=_f32(frames["bounds"]), scale_factors=_f32(frames["scale_factors"]),
+               inv_level_sigma2=_f32(frames["inv_level_sigma2"]), K=_f32(frames["K"]).reshape(B, 4),
+               l_keys_un=np.ascontiguousarray(last["keys_un"], KP_DTYPE), l_n=np.ascontiguousarray(last["n"], np.int32),
+               l_keylines=np.ascontiguousarray(last["keylines"], KEYLINE_DTYPE), l_nl=np.ascontiguousarray(last["nl"], np.int32),
+               l_point_map=np.ascontiguousarray(last["point_map"], np.int32), l_point_outlier=np.ascontiguousarray(last["point_outlier"], np.uint8),
+               l_line_map=np.ascontiguousarray(last["line_map"], np.int32), l_line_outlier=np.ascontiguousarray(last["line_outlier"], np.uint8),
+               l_Tcw=_f32(last["Tcw"]).reshape(B, 16), l_velocity=_f32(last["velocity"]).reshape(B, 16))
+    vo_in = np.ascontiguousarray(last.get("vo", np.zeros(B)), np.int32).reshape(B)
+    shapes = _mm_shapes(B, cap, capL)
+    names = _MM_OUT if taps else _MM_OUT[:8]
+
+    def structs(d):
+        F = PLTrackFrames(B, d["keys_un"], d["desc"], d["n"], cap, d["keylines"], d["line_func"], d["line_desc"], d["nl"], capL, d["bounds"],
+                          d["scale_factors"], d["inv_level_sigma2"], nlev, float(frames["log_scale_factor"]), None, d["K"], None, None)
+        Ls = PLTrackLast(*[d["l_" + k] for k, _ in PLTrackLast._fields_])
+        return F, Ls
+    if host:
+        assert B == 1
+        F, Ls = structs({k: _p(v) for k, v in arr.items()})
+        out = {k: np.zeros(shp, dt) for k, (shp, dt) in shapes.items()}
+        out["vo"][:] = vo_in
+        o = PLTrackMotionOut(*[_p(out[k]) if (k in names and k != "ok") else None for k in _MM_OUT])
+        out["ok"][0] = check(L.pl_track_motion_model(map._h, C.byref(F), C.byref(Ls), C.byref(o)))
+        return {k: out[k] for k in names}
+    torch, keep, to_dev = _torch_dev()
+    F, Ls = structs({k: to_dev(v)[1] for k, v in arr.items()})
+    dev = {}
+    for k in names:
+        shp, dt = shapes[k]
+        dev[k] = torch.zeros(max(int(np.prod(shp)) * np.dtype(dt).itemsize, 16), dtype=torch.uint8, device="cuda")
+    dev["vo"][:4 * B].copy_(torch.from_numpy(vo_in.view(np.uint8)))
+    o = PLTrackMotionOut(*[vp(dev[k].data_ptr()) if k in dev else None for k in _MM_OUT])
+    scratch = torch.empty(int(L.pl_track_motion_model_scratch_bytes(B, cap, capL)), dtype=torch.uint8, device="cuda")
+    torch.cuda.synchronize()
+    check(L.pl_track_motion_model_dev(map._h, C.byref(F), C.byref(Ls), C.byref(o), vp(scratch.data_ptr()), None))
+    torch.cuda.synchronize()
+    out = {}
+    for k in names:
+        shp, dt = shapes[k]
+        out[k] = dev[k][:int(np.prod(shp)) * np.dtype(dt).itemsize].cpu().numpy().view(dt).reshape(shp)
+    map.check_indices()
+    return out
+
+
+def track_velocity(Tcw, Tcw_last, ok, velocity):
+    """mVelocity = mCurrentFrame.mTcw * LastTwc for B frames (pl_track_velocity_dev): returns `velocity` [B][4][4] with the frames
+    where ok[b] replaced."""
+    import torch
+    B = len(Tcw)
+    L = _track_lib()
+    t = [torch.from_numpy(np.ascontiguousarray(a)).cuda() for a in
+         (_f32(Tcw).reshape(B, 16), _f32(Tcw_last).reshape(B, 16), np.ascontiguousarray(ok, np.int32).reshape(B),
+          _f32(velocity).reshape(B, 16).copy())]
+    torch.cuda.synchronize()
+    check(L.pl_track_velocity_dev(B, *[vp(x.data_ptr()) for x in t], None))
+    torch.cuda.synchronize()
+    return t[3].cpu().numpy().reshape(B, 4, 4)

@@ -316,6 +316,8 @@ struct ProjLastArgs {
   // batched retry (Tracking.cc:1352-1357: "if(nmatches<20) { fill(mvpMapPoints, NULL); SearchByProjection(..., 2*th) }"): frame b runs
   // only if gate[b] < gate_min; the kernel re-initialises its matches, which is the fill
   const int* gate = nullptr; int gate_min = 0;
+  // [B][cap_last] row of last_pos / last_desc for each last-frame keypoint (NULL: the keypoint's own [B][cap_last] row)
+  const int* last_row = nullptr;
 };
 
 __global__ void __launch_bounds__(32) k_search_proj_last(ProjLastArgs A) {
@@ -345,7 +347,8 @@ __global__ void __launch_bounds__(32) k_search_proj_last(ProjLastArgs A) {
   const float fx = Kb[0], fy = Kb[1], cx = Kb[2], cy = Kb[3];
   for (int i = 0; i < NL; i++) {
     if (!A.last_valid[lb + i]) continue;
-    const float* X = A.last_pos + (lb + i) * 3;
+    const long long row = A.last_row ? (long long)A.last_row[lb + i] : lb + i;
+    const float* X = A.last_pos + row * 3;
     float xc = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(T[0], X[0]), __fmul_rn(T[1], X[1])), __fmul_rn(T[2], X[2])), T[3]);
     float yc = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(T[4], X[0]), __fmul_rn(T[5], X[1])), __fmul_rn(T[6], X[2])), T[7]);
     float zc = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(T[8], X[0]), __fmul_rn(T[9], X[1])), __fmul_rn(T[10], X[2])), T[11]);
@@ -365,7 +368,7 @@ __global__ void __launch_bounds__(32) k_search_proj_last(ProjLastArgs A) {
       if (oct < 0) oct = 0; else if (oct >= A.nlevels) oct = A.nlevels - 1;
     } else oct = A.last_octave[lb + i];
     const float radius = __fmul_rn(A.th, A.scaleFactors[oct]);
-    Top2 t = window_top2(kc, dc, sg.start, sg.items, g, u, v, radius, oct - 1, oct + 1, A.last_desc + (lb + i) * 32,
+    Top2 t = window_top2(kc, dc, sg.start, sg.items, g, u, v, radius, oct - 1, oct + 1, A.last_desc + row * 32,
                          skip, lane, packed);
     if (t.best == KEY_NONE) continue;
     const int bestDist = key_dist(t.best), bestIdx2 = key_idx(t.best);
@@ -1204,9 +1207,20 @@ extern "C" int pl_orb_search_by_projection_last_dev(const PLKeyPoint* keys_cur, 
                                                     const float* last_angle, float th, int check_orientation,
                                                     const uint8_t* cur_preassigned, const int* gate_nmatches, int gate_min,
                                                     int* cur_match, int* nmatches, void* stream) {
+  return search_by_projection_last_launch(keys_cur, desc_cur, n_cur, cap, B, bounds, Tcw, K, scale_factors, nlevels, n_last, cap_last,
+                                          last_valid, last_pos, last_desc, nullptr, last_octave, last_angle, th, check_orientation,
+                                          cur_preassigned, gate_nmatches, gate_min, cur_match, nmatches, stream);
+}
+int pl::search_by_projection_last_launch(const PLKeyPoint* keys_cur, const uint8_t* desc_cur, const int* n_cur, int cap, int B,
+                                         const float* bounds, const float* Tcw, const float* K, const float* scale_factors, int nlevels,
+                                         const int* n_last, int cap_last, const uint8_t* last_valid, const float* last_pos,
+                                         const uint8_t* last_desc, const int* last_row, const int* last_octave, const float* last_angle,
+                                         float th, int check_orientation, const uint8_t* cur_preassigned, const int* gate_nmatches,
+                                         int gate_min, int* cur_match, int* nmatches, void* stream) {
   PL_ARG(keys_cur && desc_cur && n_cur && bounds && Tcw && K && scale_factors && n_last && last_valid && last_pos && last_desc &&
          last_octave && last_angle && cur_match && nmatches && B >= 1 && cap >= 1 && cap <= 6144 && cap_last >= 1);
   ProjLastArgs A;
+  A.last_row = last_row;
   A.keys = keys_cur; A.desc = desc_cur; A.n = n_cur; A.cap = cap; A.bounds = bounds; A.Tcw = Tcw; A.K = K; A.scaleFactors = scale_factors;
   A.nlevels = nlevels; A.n_last = n_last; A.cap_last = cap_last; A.last_valid = last_valid; A.last_pos = last_pos; A.last_desc = last_desc;
   A.last_octave = last_octave; A.last_angle = last_angle; A.th = th; A.checkOri = check_orientation; A.preassigned = cur_preassigned;

@@ -2,11 +2,19 @@
 //   th_frame  [B]       th of each frame (NULL: the scalar th for every frame)
 //   desc_row  [B][cap]  row of the descriptor array that entry (b, i) compares with (NULL: row b * cap + i)
 // pl_track_local_map_dev (track.cu) uses them to search every frame with its own th against the map's descriptors, read
-// through the frame's local-map list instead of a [B][cap_local] gather.
+// through the frame's local-map list instead of a [B][cap_local] gather.  The last-frame search takes last_row the same way
+// (position and descriptor of last-frame keypoint (b, i) from row last_row[b][i] of the map's arrays): pl_track_motion_model_dev
+// passes the last frame's matches there.
 #pragma once
 #include "common.cuh"
 
 namespace pl {
+int search_by_projection_last_launch(const PLKeyPoint* keys_cur, const uint8_t* desc_cur, const int* n_cur, int cap, int B,
+                                     const float* bounds, const float* Tcw, const float* K, const float* scale_factors, int nlevels,
+                                     const int* n_last, int cap_last, const uint8_t* last_valid, const float* last_pos,
+                                     const uint8_t* last_desc, const int* last_row, const int* last_octave, const float* last_angle,
+                                     float th, int check_orientation, const uint8_t* cur_preassigned, const int* gate_nmatches,
+                                     int gate_min, int* cur_match, int* nmatches, void* stream);
 int search_by_projection_points_launch(const PLKeyPoint* keys, const uint8_t* desc, const int* n, int cap, int B,
                                        const float* bounds, const float* scale_factors, const int* n_mp, int cap_mp,
                                        const uint8_t* in_view, const float* proj, const int* level, const float* view_cos,

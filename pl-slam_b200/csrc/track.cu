@@ -28,9 +28,12 @@ struct PLMap {
 namespace pl {
 constexpr int kTrackThreads = 256;
 
-// Sorted map indices of the matches frame b holds (INT_MAX padded) and the pre-assigned flags the searches take.
-__global__ void __launch_bounds__(kTrackThreads) k_track_held(const int* __restrict__ map_in, const int* __restrict__ n, int cap, int n_map,
-                                                              int pow2, int* __restrict__ held, int* __restrict__ n_held,
+// Sorted map indices of the matches frame b holds (INT_MAX padded) and the pre-assigned flags the searches take.  seen (may be
+// NULL): the entries TrackWithMotionModel discarded as outliers of feature i (-1 none); a feature without a held match contributes
+// its seen entry to the sorted list (skipped by the frustum test) but is not pre-assigned.
+__global__ void __launch_bounds__(kTrackThreads) k_track_held(const int* __restrict__ map_in, const int* __restrict__ seen,
+                                                              const int* __restrict__ n, int cap, int n_map, int pow2,
+                                                              int* __restrict__ held, int* __restrict__ n_held,
                                                               uint8_t* __restrict__ pre, int* __restrict__ flag) {
   extern __shared__ int s[];
   __shared__ int cnt;
@@ -41,13 +44,20 @@ __global__ void __launch_bounds__(kTrackThreads) k_track_held(const int* __restr
   __syncthreads();
   for (int i = tid; i < pow2; i += kTrackThreads) {
     int v = INT_MAX;
-    if (map_in && i < N) {
-      const int m = map_in[o + i];
+    uint8_t p = 0;
+    if (i < N) {
+      const int m = map_in ? map_in[o + i] : -1;
       if (m >= n_map) atomicOr(flag, 1);
-      else if (m >= 0) { v = m; atomicAdd(&cnt, 1); }
+      else if (m >= 0) { v = m; p = 1; }
+      else if (seen) {
+        const int q = seen[o + i];
+        if (q >= n_map) atomicOr(flag, 1);
+        else if (q >= 0) v = q;
+      }
+      if (v != INT_MAX) atomicAdd(&cnt, 1);
     }
     s[i] = v;
-    if (i < cap) pre[o + i] = v != INT_MAX;
+    if (i < cap) pre[o + i] = p;
   }
   __syncthreads();
   for (int k = 2; k <= pow2; k <<= 1)
@@ -140,25 +150,31 @@ struct TrackBuildArgs {
   const float* map_pt; const double* map_ln;
   int* point_map; int* line_map; int* pslot; int* lslot;
   int* np; float* obs; float* w; float* X; int* nlp; double* lf; double* lX;
+  // TrackWithMotionModel (NULL for the local-map step): frames with use_alt[b] take their point matches from pmatch_alt (the
+  // retry at 2 th), and frames with solve[b] == 0 (the early return) build an empty problem; point_map / line_map are written
+  const uint8_t* use_alt = nullptr; const int* pmatch_alt = nullptr; const uint8_t* solve = nullptr;
 };
 // mvpMapPoints / mvpMapLines after the searches, and the problem in feature order: points then lines
 __global__ void __launch_bounds__(kTrackThreads) k_track_build(TrackBuildArgs A) {
   __shared__ int warp_tot[kTrackThreads / 32];
   const int b = blockIdx.x;
+  const bool solve = !A.solve || A.solve[b];
   {
     const int N = min(A.n[b], A.cap);
     const long long o = (long long)b * A.cap;
+    const int* pmatch = A.use_alt && A.use_alt[b] ? A.pmatch_alt : A.pmatch;
     int base = 0;
     for (int c = 0; c < A.cap; c += kTrackThreads) {
       const int i = c + threadIdx.x;
       int fm = -1;
       if (i < N) {
-        const int mm = A.pmatch[o + i];
+        const int mm = pmatch[o + i];
         fm = mm == -2 ? A.pmap_in[o + i] : mm >= 0 ? A.prow[(long long)b * A.cap_lp + mm] : -1;
       }
-      const int slot = block_slot(fm >= 0, warp_tot, base);
-      if (i < A.cap) { A.point_map[o + i] = fm; A.pslot[o + i] = fm >= 0 ? slot : -1; }
-      if (fm >= 0) {
+      const bool use = solve && fm >= 0;
+      const int slot = block_slot(use, warp_tot, base);
+      if (i < A.cap) { A.point_map[o + i] = fm; A.pslot[o + i] = use ? slot : -1; }
+      if (use) {
         const PLKeyPoint k = A.keys[o + i];
         const long long s = o + slot;
         A.obs[2 * s] = k.x; A.obs[2 * s + 1] = k.y; A.w[s] = A.inv_sigma2[k.octave];
@@ -178,9 +194,10 @@ __global__ void __launch_bounds__(kTrackThreads) k_track_build(TrackBuildArgs A)
         const int mm = A.lmatch[o + i];
         fm = mm == -2 ? A.lmap_in[o + i] : mm >= 0 ? A.lrow[(long long)b * A.cap_ll + mm] : -1;
       }
-      const int slot = block_slot(fm >= 0, warp_tot, base);
-      if (i < A.capL) { A.line_map[o + i] = fm; A.lslot[o + i] = fm >= 0 ? slot : -1; }
-      if (fm >= 0) {
+      const bool use = solve && fm >= 0;
+      const int slot = block_slot(use, warp_tot, base);
+      if (i < A.capL) { A.line_map[o + i] = fm; A.lslot[o + i] = use ? slot : -1; }
+      if (use) {
         const long long s = o + slot;
         for (int d = 0; d < 3; d++) A.lf[3 * s + d] = A.lfunc[3 * (o + i) + d];
         for (int d = 0; d < 6; d++) A.lX[6 * s + d] = A.map_ln[6 * (long long)fm + d];
@@ -303,7 +320,7 @@ extern "C" int pl_map_check_indices(PLMap* m) {
   PL_CUDA(cudaMemcpy(&f, m->flag, 4, cudaMemcpyDeviceToHost));
   if (!f) return PL_OK;
   PL_CUDA(cudaMemset(m->flag, 0, 4));
-  set_error("track_local_map: a local-map entry or a held match named an index outside the map");
+  set_error("track: a local-map entry, a held or discarded match or a last-frame match named an index outside the map");
   return PL_ERR_ARG;
 }
 
@@ -314,6 +331,10 @@ extern "C" size_t pl_track_local_map_scratch_bytes(int B, int cap_points, int ca
 
 extern "C" int pl_track_local_map_dev(PLMap* map, const PLTrackFrames* F, const PLTrackLocal* L, const PLTrackOut* O, void* scratch,
                                       void* stream_) {
+  return pl_track_local_map_seen_dev(map, F, nullptr, nullptr, L, O, scratch, stream_);
+}
+extern "C" int pl_track_local_map_seen_dev(PLMap* map, const PLTrackFrames* F, const int* point_seen, const int* line_seen,
+                                           const PLTrackLocal* L, const PLTrackOut* O, void* scratch, void* stream_) {
   PL_ARG(map && F && L && O && scratch);
   const int B = F->B, cap = F->cap_points, capL = F->cap_lines;
   // cap_points: the point search's limit; cap_lines: k_track_held sorts a frame's held lines in shared memory (4 B per
@@ -370,9 +391,11 @@ extern "C" int pl_track_local_map_dev(PLMap* map, const PLTrackFrames* F, const 
   // 1. matches already held
   const int p2 = pow2_at_least(cap), l2 = pow2_at_least(capL);
   PL_CUDA(cudaFuncSetAttribute(k_track_held, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(std::max(p2, l2) * 4)));
-  k_track_held<<<B, kTrackThreads, p2 * 4, st>>>(F->point_map_in, F->n, cap, map->n_points, p2, s.pheld, s.nph, s.ppre, map->flag);
+  k_track_held<<<B, kTrackThreads, p2 * 4, st>>>(F->point_map_in, point_seen, F->n, cap, map->n_points, p2, s.pheld, s.nph, s.ppre,
+                                                  map->flag);
   PL_LAUNCH_CHECK();
-  k_track_held<<<B, kTrackThreads, l2 * 4, st>>>(F->line_map_in, F->nl, capL, map->n_lines, l2, s.lheld, s.nlh, s.lpre, map->flag);
+  k_track_held<<<B, kTrackThreads, l2 * 4, st>>>(F->line_map_in, line_seen, F->nl, capL, map->n_lines, l2, s.lheld, s.nlh, s.lpre,
+                                                  map->flag);
   PL_LAUNCH_CHECK();
   // 2. isInFrustum(., 0.5) per (frame, local entry)
   TrackFrustumArgs A;
@@ -490,4 +513,335 @@ extern "C" int pl_track_local_map(PLMap* map, const PLTrackFrames* F, const PLTr
   if (ret != PL_OK) return ret;
   if ((rc = pl_map_check_indices(map))) return rc;
   return ok_h;
+}
+
+// ---- Tracking::TrackWithMotionModel (src/Tracking.cc:1316-1431) for a batch of frames, monocular, localisation mode:
+//   k_mm_prep                mVelocity * mLastFrame.mTcw (:1332); the last frame's valid keypoints (mvpMapPoints[i] && !mvbOutlier[i],
+//                            ORBmatcher.cc:1441-1585) and the LSDmatcher candidates: mvpMapLines[i] && !mvbLineOutlier[i] &&
+//                            CurrentFrame.isInFrustum(pML, 0.5) at the guess (LSDmatcher.cpp:95-107)
+//   k_search_proj_last       ORBmatcher(0.9, true).SearchByProjection(Current, Last, 15, mono), position and descriptor read
+//                            through the last frame's map index; then again at 30 for frames under 20 matches (:1354-1358)
+//   k_line_search            LSDmatcher().SearchByProjection(Current, Last, 15)                          (variant 0)
+//   k_mm_gate                the retried flag, the counts and the early return (nmatches < 20 && lmatches < 5, :1360-1361)
+//   k_track_build            the PoseOptimization problem in feature order (empty for early-return frames)
+//   k_pose_opt               Optimizer::PoseOptimization (lm.cu, mode 0, unchanged)
+//   k_mm_discard             the outliers dropped (:1376-1419), mbVO and the return value (:1424-1428)
+namespace pl {
+// cv::Mat's fp32 4x4 product, element (i, j): ((a0 b0 + a1 b1) + a2 b2) + a3 b3 with every operation rounded (cv::gemm's order for
+// small matrices, as in the oracle's Mat::operator*; tests/golden/mat4_cv2.npz pins it against cv2)
+__device__ __forceinline__ float mat4_elem(const float* A, const float* Bm, int i, int j) {
+  float s = __fmul_rn(A[4 * i], Bm[j]);
+  for (int k = 1; k < 4; k++) s = __fadd_rn(s, __fmul_rn(A[4 * i + k], Bm[4 * k + j]));
+  return s;
+}
+
+struct MMPrepArgs {
+  const float* Tlast; const float* V; const float* K; const float* bounds; float logScaleFactor;
+  const PLKeyPoint* keys; const int* n; int cap; const int* pmap; const uint8_t* pout; int n_pts;
+  const void* keylines; const int* nl; int capL; const int* lmap; const uint8_t* lout; int n_lns;
+  const double* ln_pos; const double* ln_normal; const float* ln_min; const float* ln_max;
+  float* guess; uint8_t* pvalid; int* poct; float* pang;
+  uint8_t* liv; float* lproj; int* llev; float* lvc; float* llen; int* flag;
+};
+// A -1 or outlier entry is skipped without a look at the map; a non-negative index outside the map sets the flag and is skipped.
+__global__ void __launch_bounds__(kTrackThreads) k_mm_prep(MMPrepArgs A) {
+  __shared__ float G[16];
+  const int b = blockIdx.x, tid = threadIdx.x;
+  if (tid < 16) {
+    const float g = mat4_elem(A.V + 16 * b, A.Tlast + 16 * b, tid >> 2, tid & 3);
+    G[tid] = g; A.guess[16 * b + tid] = g;
+  }
+  __syncthreads();
+  {
+    const int N = min(A.n[b], A.cap);
+    const long long o = (long long)b * A.cap;
+    for (int i = tid; i < A.cap; i += kTrackThreads) {
+      uint8_t v = 0; int oct = 0; float ang = 0.f;
+      if (i < N) {
+        const int m = A.pmap[o + i];
+        if (m >= 0 && !A.pout[o + i]) { if (m >= A.n_pts) atomicOr(A.flag, 1); else v = 1; }
+        oct = A.keys[o + i].octave; ang = A.keys[o + i].angle;
+      }
+      A.pvalid[o + i] = v; A.poct[o + i] = oct; A.pang[o + i] = ang;
+    }
+  }
+  const int N = min(A.nl[b], A.capL);
+  const long long o = (long long)b * A.capL;
+  FrustumArgs F;
+  for (int k = 0; k < 16; k++) F.T[k] = G[k];
+  camera_center(F.T, F.Ow);
+  for (int k = 0; k < 4; k++) { F.K[k] = A.K[4 * b + k]; F.bounds[k] = A.bounds[k]; }
+  F.logScaleFactor = A.logScaleFactor; F.viewingCosLimit = 0.5f; F.nScaleLevels = 1; F.n = 0;
+  for (int i = tid; i < A.capL; i += kTrackThreads) {
+    const long long q = o + i;
+    A.liv[q] = 0; for (int k = 0; k < 4; k++) A.lproj[4 * q + k] = 0; A.llev[q] = 0; A.lvc[q] = 0; A.llen[q] = 0;
+    if (i >= N) continue;
+    const int m = A.lmap[q];
+    if (m < 0 || A.lout[q]) continue;
+    if (m >= A.n_lns) { atomicOr(A.flag, 1); continue; }
+    A.llen[q] = *(const float*)((const char*)A.keylines + 68 * q + 60);   // mvKeylinesUn[i].lineLength
+    float pr[4], vc; int l;
+    if (!frustum_line(F, A.ln_pos + 6 * (long long)m, A.ln_normal + 3 * (long long)m, A.ln_min[m], A.ln_max[m], pr, l, vc)) continue;
+    A.liv[q] = 1; for (int k = 0; k < 4; k++) A.lproj[4 * q + k] = pr[k];
+    A.llev[q] = l; A.lvc[q] = vc;
+  }
+}
+
+// nmatches after the retry, the retried flag, and solve = !(nmatches < 20 && lmatches < 5)
+__global__ void __launch_bounds__(128) k_mm_gate(int B, const int* __restrict__ pnm, const int* __restrict__ pnm_retry,
+                                                 const int* __restrict__ lnm, uint8_t* __restrict__ retried, int* __restrict__ counts,
+                                                 uint8_t* __restrict__ solve) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  const bool r = pnm[b] < 20;
+  const int nm = r ? pnm_retry[b] : pnm[b], lm = lnm[b];
+  retried[b] = r; counts[2 * b] = nm; counts[2 * b + 1] = lm; solve[b] = !(nm < 20 && lm < 5);
+}
+
+// Discard outliers (:1376-1419): a matched outlier loses its match (its map index goes to point_seen / line_seen, else -1) and
+// is taken off nmatches / lmatches; nmatchesMap counts the matches left (every entry of a fixed map has Observations() > 0).
+// Frames that returned early have an empty problem, so nothing is discarded and ok = 0 with vo as passed.
+__global__ void __launch_bounds__(kTrackThreads) k_mm_discard(const int* __restrict__ pslot, const uint8_t* __restrict__ pout, int cap,
+                                                              const int* __restrict__ lslot, const uint8_t* __restrict__ lout, int capL,
+                                                              const uint8_t* __restrict__ solve, const int* __restrict__ counts,
+                                                              int* __restrict__ point_map, int* __restrict__ line_map,
+                                                              int* __restrict__ point_seen, int* __restrict__ line_seen,
+                                                              int* __restrict__ nmatches, int* __restrict__ ok, int* __restrict__ vo) {
+  __shared__ int cnt[3];
+  const int b = blockIdx.x;
+  if (threadIdx.x < 3) cnt[threadIdx.x] = 0;
+  __syncthreads();
+  int dp = 0, dl = 0, kept = 0;
+  for (int i = threadIdx.x; i < cap; i += kTrackThreads) {
+    const long long o = (long long)b * cap + i;
+    const int s = pslot[o], m = point_map[o];
+    int seen = -1;
+    if (s >= 0 && pout[(long long)b * cap + s]) { seen = m; point_map[o] = -1; dp++; }
+    else kept += m >= 0;
+    point_seen[o] = seen;
+  }
+  for (int i = threadIdx.x; i < capL; i += kTrackThreads) {
+    const long long o = (long long)b * capL + i;
+    const int s = lslot[o], m = line_map[o];
+    int seen = -1;
+    if (s >= 0 && lout[(long long)b * capL + s]) { seen = m; line_map[o] = -1; dl++; }
+    line_seen[o] = seen;
+  }
+  dp = warp_sum(dp); dl = warp_sum(dl); kept = warp_sum(kept);
+  if ((threadIdx.x & 31) == 0) { atomicAdd(&cnt[0], dp); atomicAdd(&cnt[1], dl); atomicAdd(&cnt[2], kept); }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    const int nm = counts[2 * b] - cnt[0];
+    nmatches[2 * b] = nm; nmatches[2 * b + 1] = counts[2 * b + 1] - cnt[1];
+    if (solve[b]) { vo[b] = cnt[2] < 10; ok[b] = nm > 20; }
+    else ok[b] = 0;
+  }
+}
+
+// mVelocity = mCurrentFrame.mTcw * LastTwc, LastTwc = [Rcw^T | Ow] of the last frame (Tracking.cc:492-501), where ok[b]
+__global__ void __launch_bounds__(128) k_track_velocity(int B, const float* __restrict__ T, const float* __restrict__ Tl,
+                                                        const int* __restrict__ ok, float* __restrict__ V) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B || !ok[b]) return;
+  float L[16], W[16], C[16], Ow[3];
+  for (int k = 0; k < 16; k++) { L[k] = Tl[16 * b + k]; C[k] = T[16 * b + k]; }
+  camera_center(L, Ow);
+  for (int i = 0; i < 3; i++) {
+    for (int j = 0; j < 3; j++) W[4 * i + j] = L[4 * j + i];
+    W[4 * i + 3] = Ow[i];
+  }
+  W[12] = W[13] = W[14] = 0.f; W[15] = 1.f;
+  for (int k = 0; k < 16; k++) V[16 * b + k] = mat4_elem(C, W, k >> 2, k & 3);
+}
+
+struct MMScratch {
+  float* guess; uint8_t* pvalid; int* poct; float* pang;
+  uint8_t* liv; float* lproj; int* llev; float* lvc; float* llen;
+  int *pm, *pnm, *pm2, *pnm2, *lmatch, *lnm; void* lsd;
+  uint8_t *retried, *solve; int* counts;
+  int *np, *nl; float *obs, *w, *X; double *lf, *lX;
+  int *pslot, *lslot; uint8_t *pout, *lout; int *inl, *its; double* lm;
+};
+static size_t carve_mm(void* base, int B, int cap, int capL, MMScratch* t) {
+  size_t off = 0;
+  auto take = [&](size_t bytes) { void* p = base ? (char*)base + off : nullptr; off += (bytes + 15) / 16 * 16; return p; };
+  const size_t b = B, k = cap, l = capL;
+  MMScratch s;
+  s.guess = (float*)take(b * 64); s.pvalid = (uint8_t*)take(b * k); s.poct = (int*)take(b * k * 4); s.pang = (float*)take(b * k * 4);
+  s.liv = (uint8_t*)take(b * l); s.lproj = (float*)take(b * l * 16); s.llev = (int*)take(b * l * 4); s.lvc = (float*)take(b * l * 4);
+  s.llen = (float*)take(b * l * 4);
+  s.pm = (int*)take(b * k * 4); s.pnm = (int*)take(b * 4); s.pm2 = (int*)take(b * k * 4); s.pnm2 = (int*)take(b * 4);
+  s.lmatch = (int*)take(b * l * 4); s.lnm = (int*)take(b * 4);
+  s.lsd = take(pl_lsd_search_scratch_bytes(capL, B));
+  s.retried = (uint8_t*)take(b); s.solve = (uint8_t*)take(b); s.counts = (int*)take(b * 8);
+  s.np = (int*)take(b * 4); s.nl = (int*)take(b * 4);
+  s.obs = (float*)take(b * k * 8); s.w = (float*)take(b * k * 4); s.X = (float*)take(b * k * 12);
+  s.lf = (double*)take(b * l * 24); s.lX = (double*)take(b * l * 48);
+  s.pslot = (int*)take(b * k * 4); s.lslot = (int*)take(b * l * 4); s.pout = (uint8_t*)take(b * k); s.lout = (uint8_t*)take(b * l);
+  s.inl = (int*)take(b * 4); s.its = (int*)take(b * 4);
+  s.lm = (double*)take(pl_pose_optimization_scratch_doubles(B, cap, capL) * 8);
+  if (t) *t = s;
+  return off;
+}
+}  // namespace pl
+
+extern "C" size_t pl_track_motion_model_scratch_bytes(int B, int cap_points, int cap_lines) {
+  if (B < 1 || cap_points < 1 || cap_lines < 1) return 0;
+  return carve_mm(nullptr, B, cap_points, cap_lines, nullptr);
+}
+
+extern "C" int pl_track_motion_model_dev(PLMap* map, const PLTrackFrames* F, const PLTrackLast* Ls, const PLTrackMotionOut* O,
+                                         void* scratch, void* stream_) {
+  PL_ARG(map && F && Ls && O && scratch);
+  const int B = F->B, cap = F->cap_points, capL = F->cap_lines;
+  PL_ARG(B >= 1 && cap >= 1 && cap <= 6144 && capL >= 1 && capL <= 32768 && F->nlevels >= 1);
+  PL_ARG(F->keys_un && F->desc && F->n && F->keylines && F->line_func && F->line_desc && F->nl && F->bounds && F->scale_factors &&
+         F->inv_level_sigma2 && F->K);
+  // the guess is computed and the current frame's matches start empty (:1332-1335)
+  PL_ARG(!F->Tcw0 && !F->point_map_in && !F->line_map_in);
+  PL_ARG(Ls->keys_un && Ls->n && Ls->keylines && Ls->nl && Ls->point_map && Ls->point_outlier && Ls->line_map && Ls->line_outlier &&
+         Ls->Tcw && Ls->velocity);
+  PL_ARG(O->Tcw && O->point_map && O->line_map && O->point_seen && O->line_seen && O->nmatches && O->ok && O->vo);
+  cudaStream_t st = stream_ ? (cudaStream_t)stream_ : map->stream;
+  MMScratch s;
+  carve_mm(scratch, B, cap, capL, &s);
+  float* guess = O->guess ? O->guess : s.guess;
+  uint8_t* liv = O->ln_in_view ? O->ln_in_view : s.liv; float* lproj = O->ln_proj ? O->ln_proj : s.lproj;
+  int* llev = O->ln_level ? O->ln_level : s.llev; float* lvc = O->ln_view_cos ? O->ln_view_cos : s.lvc;
+  int* pm = O->pt_match ? O->pt_match : s.pm; int* pm2 = O->pt_match_retry ? O->pt_match_retry : s.pm2;
+  int* lmatch = O->ln_match ? O->ln_match : s.lmatch; uint8_t* retried = O->retried ? O->retried : s.retried;
+  int* np = O->prob_n_points ? O->prob_n_points : s.np; int* nl = O->prob_n_lines ? O->prob_n_lines : s.nl;
+  float* obs = O->prob_pt_obs ? O->prob_pt_obs : s.obs; float* w = O->prob_pt_inv_sigma2 ? O->prob_pt_inv_sigma2 : s.w;
+  float* X = O->prob_pt_Xw ? O->prob_pt_Xw : s.X;
+  double* lf = O->prob_line_func ? O->prob_line_func : s.lf; double* lX = O->prob_line_Xw ? O->prob_line_Xw : s.lX;
+
+  // 1. the guess, the last frame's valid keypoints and its line candidates at the guess
+  MMPrepArgs P;
+  P.Tlast = Ls->Tcw; P.V = Ls->velocity; P.K = F->K; P.bounds = F->bounds; P.logScaleFactor = F->log_scale_factor;
+  P.keys = Ls->keys_un; P.n = Ls->n; P.cap = cap; P.pmap = Ls->point_map; P.pout = Ls->point_outlier; P.n_pts = map->n_points;
+  P.keylines = Ls->keylines; P.nl = Ls->nl; P.capL = capL; P.lmap = Ls->line_map; P.lout = Ls->line_outlier; P.n_lns = map->n_lines;
+  P.ln_pos = map->ln_pos; P.ln_normal = map->ln_normal; P.ln_min = map->ln_min; P.ln_max = map->ln_max;
+  P.guess = guess; P.pvalid = s.pvalid; P.poct = s.poct; P.pang = s.pang;
+  P.liv = liv; P.lproj = lproj; P.llev = llev; P.lvc = lvc; P.llen = s.llen; P.flag = map->flag;
+  k_mm_prep<<<B, kTrackThreads, 0, st>>>(P);
+  PL_LAUNCH_CHECK();
+  // 2. the searches: points at th = 15, lines at 15, points again at 30 for frames under 20 point matches
+  int rc;
+  if ((rc = search_by_projection_last_launch(F->keys_un, F->desc, F->n, cap, B, F->bounds, guess, F->K, F->scale_factors, F->nlevels,
+                                             Ls->n, cap, s.pvalid, map->pt_pos, map->pt_desc, Ls->point_map, s.poct, s.pang, 15.0f, 1,
+                                             nullptr, nullptr, 0, pm, s.pnm, st))) return rc;
+  if ((rc = lsd_search_by_projection_launch(0, F->keylines, F->line_func, F->line_desc, F->nl, capL, B, F->bounds, Ls->nl, capL, liv,
+                                            lproj, map->ln_desc, s.llen, 15.0f, nullptr, Ls->line_map, 0.f, nullptr, lmatch, s.lnm, s.lsd,
+                                            st))) return rc;
+  if ((rc = search_by_projection_last_launch(F->keys_un, F->desc, F->n, cap, B, F->bounds, guess, F->K, F->scale_factors, F->nlevels,
+                                             Ls->n, cap, s.pvalid, map->pt_pos, map->pt_desc, Ls->point_map, s.poct, s.pang, 30.0f, 1,
+                                             nullptr, s.pnm, 20, pm2, s.pnm2, st))) return rc;
+  k_mm_gate<<<(B + 127) / 128, 128, 0, st>>>(B, s.pnm, s.pnm2, s.lnm, retried, s.counts, s.solve);
+  PL_LAUNCH_CHECK();
+  // 3. the pose problem (rows: the last frame's matches, since a search result is a last-frame index), then PoseOptimization
+  TrackBuildArgs Bd;
+  Bd.keys = F->keys_un; Bd.n = F->n; Bd.cap = cap; Bd.inv_sigma2 = F->inv_level_sigma2; Bd.lfunc = F->line_func; Bd.nl = F->nl; Bd.capL = capL;
+  Bd.pmap_in = nullptr; Bd.lmap_in = nullptr; Bd.pmatch = pm; Bd.lmatch = lmatch;
+  Bd.prow = Ls->point_map; Bd.cap_lp = cap; Bd.lrow = Ls->line_map; Bd.cap_ll = capL; Bd.map_pt = map->pt_pos; Bd.map_ln = map->ln_pos;
+  Bd.point_map = O->point_map; Bd.line_map = O->line_map; Bd.pslot = s.pslot; Bd.lslot = s.lslot;
+  Bd.np = np; Bd.obs = obs; Bd.w = w; Bd.X = X; Bd.nlp = nl; Bd.lf = lf; Bd.lX = lX;
+  Bd.use_alt = retried; Bd.pmatch_alt = pm2; Bd.solve = s.solve;
+  k_track_build<<<B, kTrackThreads, 0, st>>>(Bd);
+  PL_LAUNCH_CHECK();
+  if ((rc = pl_pose_optimization_dev(0, B, guess, F->K, np, cap, obs, w, X, nl, capL, lf, lX, O->Tcw, s.pout, s.lout, s.inl, s.its, s.lm,
+                                     st))) return rc;
+  // 4. discard the outliers
+  k_mm_discard<<<B, kTrackThreads, 0, st>>>(s.pslot, s.pout, cap, s.lslot, s.lout, capL, s.solve, s.counts, O->point_map, O->line_map,
+                                            O->point_seen, O->line_seen, O->nmatches, O->ok, O->vo);
+  PL_LAUNCH_CHECK();
+  return PL_OK;
+}
+
+// B = 1 on host pointers: stage, run, copy back, check the index flag.  Both frames' device arrays are sized by the largest count.
+extern "C" int pl_track_motion_model(PLMap* map, const PLTrackFrames* F, const PLTrackLast* Ls, const PLTrackMotionOut* O) {
+  PL_ARG(map && F && Ls && O && F->B == 1 && F->n && F->nl && Ls->n && Ls->nl && F->nlevels >= 1);
+  PL_ARG(!F->Tcw0 && !F->point_map_in && !F->line_map_in);
+  PL_ARG(O->Tcw && O->point_map && O->line_map && O->point_seen && O->line_seen && O->nmatches && O->vo);
+  const int n = *F->n, nl = *F->nl, n0 = *Ls->n, nl0 = *Ls->nl;
+  PL_ARG(n >= 0 && nl >= 0 && n0 >= 0 && nl0 >= 0 && n <= F->cap_points && nl <= F->cap_lines && n0 <= F->cap_points &&
+         nl0 <= F->cap_lines);
+  int rc = require_device(); if (rc) return rc;
+  const int cap = std::max(std::max(n, n0), 1), capL = std::max(std::max(nl, nl0), 1);
+  std::vector<void*> fr;
+  cudaError_t e = cudaSuccess;
+  auto dal = [&](size_t bytes) -> void* {
+    void* p = nullptr;
+    if (e == cudaSuccess) e = cudaMalloc(&p, std::max<size_t>(bytes, 16));
+    if (e == cudaSuccess) { fr.push_back(p); e = cudaMemset(p, 0, std::max<size_t>(bytes, 16)); }
+    return e == cudaSuccess ? p : nullptr;
+  };
+  auto dup = [&](const void* h, size_t bytes) -> void* {
+    void* p = dal(bytes);
+    if (p && h && bytes) e = cudaMemcpy(p, h, bytes, cudaMemcpyHostToDevice);
+    return e == cudaSuccess ? p : nullptr;
+  };
+  PLTrackFrames D = *F;
+  D.cap_points = cap; D.cap_lines = capL;
+  D.keys_un = (const PLKeyPoint*)dup(F->keys_un, (size_t)n * sizeof(PLKeyPoint)); D.desc = (const uint8_t*)dup(F->desc, (size_t)n * 32);
+  D.n = (const int*)dup(&n, 4);
+  D.keylines = dup(F->keylines, (size_t)nl * 68); D.line_func = (const double*)dup(F->line_func, (size_t)nl * 24);
+  D.line_desc = (const uint8_t*)dup(F->line_desc, (size_t)nl * 32); D.nl = (const int*)dup(&nl, 4);
+  D.bounds = (const float*)dup(F->bounds, 16); D.scale_factors = (const float*)dup(F->scale_factors, (size_t)F->nlevels * 4);
+  D.inv_level_sigma2 = (const float*)dup(F->inv_level_sigma2, (size_t)F->nlevels * 4);
+  D.K = (const float*)dup(F->K, 16);
+  PLTrackLast DL;
+  DL.keys_un = (const PLKeyPoint*)dup(Ls->keys_un, (size_t)n0 * sizeof(PLKeyPoint)); DL.n = (const int*)dup(&n0, 4);
+  DL.keylines = dup(Ls->keylines, (size_t)nl0 * 68); DL.nl = (const int*)dup(&nl0, 4);
+  DL.point_map = (const int*)dup(Ls->point_map, (size_t)n0 * 4); DL.point_outlier = (const uint8_t*)dup(Ls->point_outlier, (size_t)n0);
+  DL.line_map = (const int*)dup(Ls->line_map, (size_t)nl0 * 4); DL.line_outlier = (const uint8_t*)dup(Ls->line_outlier, (size_t)nl0);
+  DL.Tcw = (const float*)dup(Ls->Tcw, 64); DL.velocity = (const float*)dup(Ls->velocity, 64);
+  struct Field { void* host; size_t bytes; void* dev; };
+  std::vector<Field> outs;
+  auto dout = [&](void* h, size_t bytes, size_t alloc) -> void* {
+    if (!h) return nullptr;
+    void* d = dal(alloc); outs.push_back({h, bytes, d}); return d;
+  };
+  int ok_h = 0;
+  PLTrackMotionOut DO;
+  DO.Tcw = (float*)dout(O->Tcw, 64, 64); DO.ok = (int*)dout(&ok_h, 4, 4); DO.nmatches = (int*)dout(O->nmatches, 8, 8);
+  DO.vo = (int*)dout(O->vo, 4, 4);
+  if (DO.vo && e == cudaSuccess) e = cudaMemcpy(DO.vo, O->vo, 4, cudaMemcpyHostToDevice);   // in / out
+  DO.point_map = (int*)dout(O->point_map, (size_t)n * 4, (size_t)cap * 4); DO.line_map = (int*)dout(O->line_map, (size_t)nl * 4, (size_t)capL * 4);
+  DO.point_seen = (int*)dout(O->point_seen, (size_t)n * 4, (size_t)cap * 4);
+  DO.line_seen = (int*)dout(O->line_seen, (size_t)nl * 4, (size_t)capL * 4);
+  DO.guess = (float*)dout(O->guess, 64, 64);
+  DO.pt_match = (int*)dout(O->pt_match, (size_t)n * 4, (size_t)cap * 4);
+  DO.pt_match_retry = (int*)dout(O->pt_match_retry, (size_t)n * 4, (size_t)cap * 4);
+  DO.retried = (uint8_t*)dout(O->retried, 1, 1); DO.ln_match = (int*)dout(O->ln_match, (size_t)nl * 4, (size_t)capL * 4);
+  DO.ln_in_view = (uint8_t*)dout(O->ln_in_view, nl0, capL); DO.ln_proj = (float*)dout(O->ln_proj, (size_t)nl0 * 16, (size_t)capL * 16);
+  DO.ln_level = (int*)dout(O->ln_level, (size_t)nl0 * 4, (size_t)capL * 4);
+  DO.ln_view_cos = (float*)dout(O->ln_view_cos, (size_t)nl0 * 4, (size_t)capL * 4);
+  DO.prob_n_points = (int*)dout(O->prob_n_points, 4, 4); DO.prob_n_lines = (int*)dout(O->prob_n_lines, 4, 4);
+  DO.prob_pt_obs = (float*)dout(O->prob_pt_obs, (size_t)n * 8, (size_t)cap * 8);
+  DO.prob_pt_inv_sigma2 = (float*)dout(O->prob_pt_inv_sigma2, (size_t)n * 4, (size_t)cap * 4);
+  DO.prob_pt_Xw = (float*)dout(O->prob_pt_Xw, (size_t)n * 12, (size_t)cap * 12);
+  DO.prob_line_func = (double*)dout(O->prob_line_func, (size_t)nl * 24, (size_t)capL * 24);
+  DO.prob_line_Xw = (double*)dout(O->prob_line_Xw, (size_t)nl * 48, (size_t)capL * 48);
+  void* scr = dal(pl_track_motion_model_scratch_bytes(1, cap, capL));
+  int ret = PL_ERR_CUDA;
+  if (e != cudaSuccess || !scr) set_error("track_motion_model: %s", cudaGetErrorString(e));
+  else {
+    ret = pl_track_motion_model_dev(map, &D, &DL, &DO, scr, map->stream);
+    if (ret == PL_OK) {
+      e = cudaStreamSynchronize(map->stream);
+      for (const Field& f : outs) if (e == cudaSuccess && f.bytes) e = cudaMemcpy(f.host, f.dev, f.bytes, cudaMemcpyDeviceToHost);
+      if (e != cudaSuccess) { set_error("track_motion_model: %s", cudaGetErrorString(e)); ret = PL_ERR_CUDA; }
+    }
+  }
+  for (void* p : fr) cudaFree(p);
+  if (ret != PL_OK) return ret;
+  if ((rc = pl_map_check_indices(map))) return rc;
+  return ok_h;
+}
+
+extern "C" int pl_track_velocity_dev(int B, const float* Tcw, const float* Tcw_last, const int* ok, float* velocity, void* stream) {
+  PL_ARG(B >= 1 && Tcw && Tcw_last && ok && velocity);
+  k_track_velocity<<<(B + 127) / 128, 128, 0, (cudaStream_t)stream>>>(B, Tcw, Tcw_last, ok, velocity);
+  PL_LAUNCH_CHECK();
+  return PL_OK;
 }
