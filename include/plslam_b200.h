@@ -616,6 +616,76 @@ int pl_track_motion_model(PLMap* map, const PLTrackFrames* frames, const PLTrack
  * computes it), with the guess's fp32 4x4 product; velocity[b] is written only where ok[b].  Device arrays [B][16], ok [B]. */
 int pl_track_velocity_dev(int B, const float* Tcw, const float* Tcw_last, const int* ok, float* velocity, void* stream);
 
+/* ------------------------------------------------------------------ the local map from the keyframe graph
+ * Tracking::UpdateLocalMap (src/Tracking.cc:1899-2081) for B frames on the device, so that a localisation-mode frame in state OK
+ * runs from UpdateLastFrame to the stored relative pose with no host synchronisation.
+ *
+ * The keyframe graph of the fixed map (pl_map_set_keyframes, host arrays; the handle keeps device copies, a second call replaces
+ * the graph).  NUMBERING: keyframes are 0 .. n_kf-1 in ascending KeyFrame* address, the order in which map<KeyFrame*,int> and
+ * set<KeyFrame*> iterate (the reference's keyframeCounter and mspChildrens); numbering by mnId gives other lists wherever the
+ * allocator did not hand out increasing addresses.  Per keyframe: Tcw [16] = GetPose(), Twc [16] = GetPoseInverse() (both as
+ * stored, row-major), bad (NULL = none bad) = isBad(), parent = GetParent() (-1 none).  CSR rows (offsets [n_kf + 1]):
+ * pt_slot = GetMapPointMatches() in feature order (map-point index or -1, also for a bad point), ln_slot = GetMapLineMatches(),
+ * cov = mvpOrderedConnectedKeyFrames as stored (the first 10 are read), child = mspChildrens (any order; sorted at upload).  Per
+ * map point (offsets [n_points + 1]): obs = the keyframes of GetObservations().
+ * Limits, from the kernel's shared memory (4 B per keyframe and 1 bit per keyframe, 1 bit per map point or line): n_kf 1 ..
+ * 16384 and the map's n_points, n_lines up to 2^20.  PL_ERR_ARG for a graph over them, an index out of range, or CSR offsets that
+ * do not start at 0 or are not monotone; the previous graph is then kept. */
+typedef struct PLKeyFrameGraphDesc {
+  int n_kf;
+  const float* Tcw /*[n_kf][16]*/; const float* Twc /*[n_kf][16]*/; const uint8_t* bad /*[n_kf] or NULL*/; const int* parent;
+  const int* pt_slot_offset; const int* pt_slot;
+  const int* ln_slot_offset; const int* ln_slot;
+  const int* cov_offset; const int* cov;
+  const int* child_offset; const int* child;
+  const int* obs_offset /*[n_points + 1]*/; const int* obs;
+} PLKeyFrameGraphDesc;
+int pl_map_set_keyframes(PLMap* m, const PLKeyFrameGraphDesc* graph);
+/* Sticky flag of pl_track_update_local_map_dev since the last check: PL_ERR_ARG if a list outgrew its capacity (the counts
+ * still hold the true sizes; entries past a capacity were not written), else PL_OK; clears the flag.  Synchronises the device. */
+int pl_map_check_capacity(PLMap* m);
+
+/* The local map of B frames (device arrays):
+ *   kf [B][cap_kf], n_kf [B] = mvpLocalKeyFrames and ref_kf [B] = mpReferenceKF (keyframe index): IN / OUT, since a frame whose
+ *   matches vote for no keyframe keeps both (:1995-1996);
+ *   pt_index [B][cap_local_points], pt_count [B] = mvpLocalMapPoints (map-point indices); ln_index / ln_count likewise for lines. */
+typedef struct PLLocalMap {
+  int* kf; int* n_kf; int cap_kf; int* ref_kf;
+  int* pt_index; int* pt_count; int cap_local_points;
+  int* ln_index; int* ln_count; int cap_local_lines;
+} PLLocalMap;
+/* UpdateLocalKeyFrames, UpdateLocalPoints, UpdateLocalLines per frame b on point_map [B][cap_points] (mvpMapPoints as map indices,
+ * -1 none; every entry is read, as the motion model writes them): each matched point votes once per keyframe of its observations
+ * (lines do not vote); the good voters enter the list in index order and ref_kf = the first strict maximum among them; then, for
+ * the original voters only while the list holds at most 80, the first good covisible (of the first 10) not yet in, the first
+ * good child not yet in, and the parent if not yet in (not checked for isBad; adding it ends the expansion); no vote at all
+ * leaves kf, n_kf and ref_kf as passed.  The points and lines are the first occurrences over the list in list order, then slot
+ * order.  A count holds the true size; entries past a capacity are not written and set the flag of pl_map_check_capacity.
+ * Gate (device, each may be NULL): frame b runs only if ok[b] && !vo[b] (Tracking.cc:476); a frame that does not run keeps its
+ * kf / n_kf / ref_kf and gets pt_count = ln_count = 0.  A point_map entry or stale kf entry outside the map sets the index flag
+ * and is skipped.  Needs no scratch; deterministic (integer votes, results independent of the order of atomics).  Asynchronous
+ * on `stream` (NULL = the map's stream). */
+int pl_track_update_local_map_dev(PLMap* map, int B, const int* point_map, int cap_points, const int* ok, const int* vo,
+                                  const PLLocalMap* local, void* stream);
+/* pl_track_local_map_seen_dev on the device lists of pl_track_update_local_map_dev: frame b's list is pt_index[b][0 .. pt_count[b])
+ * (counts clamped to the capacities), frames_since_reloc [B] is a device array, and the same optional ok / vo gate applies: a
+ * frame gated off passes through with Tcw = Tcw0, its held matches as point_map / line_map, outlier flags 0, inliers 0 and
+ * ok = ok[b] (1 if ok is NULL); out->ok may be the ok array itself.  Frames that run compute exactly what
+ * pl_track_local_map_seen_dev computes on the same lists.  B * cap_local_points and B * cap_local_lines must fit an int.
+ * Scratch: pl_track_local_map_lists_scratch_bytes(B, caps) bytes.  Enqueues kernels only. */
+size_t pl_track_local_map_lists_scratch_bytes(int B, int cap_points, int cap_lines, int cap_local_points, int cap_local_lines);
+int pl_track_local_map_lists_dev(PLMap* map, const PLTrackFrames* frames, const int* point_seen, const int* line_seen,
+                                 const PLLocalMap* local, const int* frames_since_reloc, int max_frames, const int* ok, const int* vo,
+                                 const PLTrackOut* out, void* scratch, void* stream);
+/* The reference-keyframe bookkeeping with cv::Mat's fp32 4x4 product (device arrays [B][16], ref_kf [B]):
+ *   relative pose  Tcr = Tcw * Twc[ref_kf]       (mlRelativeFramePoses, Tracking.cc:582)
+ *   last pose      Tcw_last = Tcr * Tcw[ref_kf]   (the monocular UpdateLastFrame, :1242-1245)
+ * A ref_kf outside the graph sets the index flag and leaves that frame's output unwritten.
+ * The OK-state frame is then, on one stream: last pose -> pl_track_motion_model_dev -> pl_track_update_local_map_dev (gated by its
+ * ok / vo) -> pl_track_local_map_lists_dev (same gate) -> pl_track_velocity_dev -> relative pose. */
+int pl_track_relative_pose_dev(PLMap* map, int B, const float* Tcw, const int* ref_kf, float* Tcr, void* stream);
+int pl_track_last_pose_dev(PLMap* map, int B, const float* Tcr, const int* ref_kf, float* Tcw_last, void* stream);
+
 /* ------------------------------------------------------------------ multi-GPU exchange (SURVEY.md §8e)
  * Frames shard across the GPUs of one box with no data-path collective; the ONE exchange is an all-gather of the per-frame
  * pose records (64 B per frame) over NCCL / NVLink so that the rank running the sequential Tracking logic (Tracking.cc:329)

@@ -926,6 +926,15 @@ def _track_lib():
         L.pl_track_motion_model_dev.argtypes = [vp, C.POINTER(PLTrackFrames), C.POINTER(PLTrackLast), C.POINTER(PLTrackMotionOut), vp, vp]
         L.pl_track_motion_model.argtypes = [vp, C.POINTER(PLTrackFrames), C.POINTER(PLTrackLast), C.POINTER(PLTrackMotionOut)]
         L.pl_track_velocity_dev.argtypes = [C.c_int, vp, vp, vp, vp, vp]
+        L.pl_map_set_keyframes.argtypes = [vp, C.POINTER(PLKeyFrameGraphDesc)]
+        L.pl_map_check_capacity.argtypes = [vp]
+        L.pl_track_update_local_map_dev.argtypes = [vp, C.c_int, vp, C.c_int, vp, vp, C.POINTER(PLLocalMap), vp]
+        L.pl_track_local_map_lists_scratch_bytes.argtypes = [C.c_int] * 5
+        L.pl_track_local_map_lists_scratch_bytes.restype = C.c_size_t
+        L.pl_track_local_map_lists_dev.argtypes = [vp, C.POINTER(PLTrackFrames), vp, vp, C.POINTER(PLLocalMap), vp, C.c_int, vp, vp,
+                                                   C.POINTER(PLTrackOut), vp, vp]
+        L.pl_track_relative_pose_dev.argtypes = [vp, C.c_int, vp, vp, vp, vp]
+        L.pl_track_last_pose_dev.argtypes = [vp, C.c_int, vp, vp, vp, vp]
         L._track_types = True
     return L
 
@@ -953,6 +962,25 @@ class Map:
     def check_indices(self):
         """PL_ERR_ARG (raised) if a call since the last check met an index outside the map."""
         check(_track_lib().pl_map_check_indices(self._h))
+
+    def set_keyframes(self, graph):
+        """Upload the keyframe graph (pl_map_set_keyframes; keyframes numbered in ascending KeyFrame* address).  graph: dict(Tcw,
+        Twc [K][4][4], bad [K] (optional), parent [K] (-1 none), and the CSR pairs pt_slot_offset / pt_slot, ln_slot_offset /
+        ln_slot, cov_offset / cov, child_offset / child ([K + 1] offsets) and obs_offset [n_points + 1] / obs)."""
+        Tcw = _f32(graph["Tcw"]).reshape(-1, 16)
+        K = len(Tcw)
+        a = dict(Tcw=Tcw, Twc=_f32(graph["Twc"]).reshape(-1, 16), parent=_i32(graph["parent"]))
+        if graph.get("bad") is not None:
+            a["bad"] = np.ascontiguousarray(graph["bad"], np.uint8)
+        for k in ("pt_slot", "ln_slot", "cov", "child", "obs"):
+            a[k + "_offset"] = _i32(graph[k + "_offset"]); a[k] = _i32(graph[k])
+        self._graph = a
+        d = PLKeyFrameGraphDesc(K, *[_p(a.get(f)) for f, _ in PLKeyFrameGraphDesc._fields_[1:]])
+        check(_track_lib().pl_map_set_keyframes(self._h, C.byref(d)))
+
+    def check_capacity(self):
+        """PL_ERR_ARG (raised) if a local list outgrew its capacity since the last check."""
+        check(_track_lib().pl_map_check_capacity(self._h))
 
 
 def _local_struct(local, B, keep, to_dev):
@@ -995,7 +1023,7 @@ def _torch_dev():
     return torch, keep, to_dev
 
 
-def _run_dev(call, B, cap, capL, cLP, cLL, taps, keep, torch):
+def _run_dev(call, B, cap, capL, cLP, cLL, taps, keep, torch, scratch_query=None):
     shapes = _out_shapes(B, cap, capL, cLP, cLL)
     names = _TRACK_OUT if taps else _TRACK_OUT[:7]
     dev = {}
@@ -1003,7 +1031,8 @@ def _run_dev(call, B, cap, capL, cLP, cLL, taps, keep, torch):
         shp, dt = shapes[k]
         dev[k] = torch.zeros(max(int(np.prod(shp)) * np.dtype(dt).itemsize, 16), dtype=torch.uint8, device="cuda")
     o = PLTrackOut(*[vp(dev[k].data_ptr()) if k in dev else None for k in _TRACK_OUT])
-    scratch = torch.empty(int(_track_lib().pl_track_local_map_scratch_bytes(B, cap, capL, cLP, cLL)), dtype=torch.uint8, device="cuda")
+    query = scratch_query or _track_lib().pl_track_local_map_scratch_bytes
+    scratch = torch.empty(int(query(B, cap, capL, cLP, cLL)), dtype=torch.uint8, device="cuda")
     torch.cuda.synchronize()
     check(call(o, vp(scratch.data_ptr())))
     torch.cuda.synchronize()
@@ -1189,3 +1218,225 @@ def track_velocity(Tcw, Tcw_last, ok, velocity):
     check(L.pl_track_velocity_dev(B, *[vp(x.data_ptr()) for x in t], None))
     torch.cuda.synchronize()
     return t[3].cpu().numpy().reshape(B, 4, 4)
+
+
+# ---------------------------------------------------------------------------------------------- the local map from the keyframe graph
+class PLKeyFrameGraphDesc(C.Structure):
+    _fields_ = [("n_kf", C.c_int)] + [(k, vp) for k in ("Tcw", "Twc", "bad", "parent", "pt_slot_offset", "pt_slot", "ln_slot_offset",
+                                                        "ln_slot", "cov_offset", "cov", "child_offset", "child", "obs_offset", "obs")]
+
+
+class PLLocalMap(C.Structure):
+    _fields_ = [("kf", vp), ("n_kf", vp), ("cap_kf", C.c_int), ("ref_kf", vp), ("pt_index", vp), ("pt_count", vp),
+                ("cap_local_points", C.c_int), ("ln_index", vp), ("ln_count", vp), ("cap_local_lines", C.c_int)]
+
+
+def _local_map_struct(t, cap_kf, cLP, cLL):
+    """t: dict of torch tensors kf, n_kf, ref_kf, pt_index, pt_count, ln_index, ln_count."""
+    a = {k: vp(v.data_ptr()) for k, v in t.items()}
+    return PLLocalMap(a["kf"], a["n_kf"], cap_kf, a["ref_kf"], a["pt_index"], a["pt_count"], cLP, a["ln_index"], a["ln_count"], cLL)
+
+
+def _opt_dev(a, B, to_dev):
+    return None if a is None else to_dev(np.ascontiguousarray(a, np.int32).reshape(B))[1]
+
+
+def update_local_map(map, point_map, kf, n_kf, ref_kf, cap_local_points, cap_local_lines, ok=None, vo=None):
+    """Tracking::UpdateLocalMap for B frames (pl_track_update_local_map_dev) on point_map [B][cap] (map index or -1).
+    kf [B][cap_kf], n_kf [B] and ref_kf [B] are the local keyframe lists and reference keyframes passed in (kept by a frame whose
+    matches vote for no keyframe); ok / vo (optional [B]): frame b runs only if ok[b] and not vo[b].  Returns dict(kf, n_kf, ref_kf,
+    pt_index [B][cap_local_points], pt_count [B], ln_index [B][cap_local_lines], ln_count [B]); counts are the true sizes, entries
+    past a capacity are left 0 and Map.check_capacity() raises."""
+    import torch
+    point_map = np.ascontiguousarray(point_map, np.int32)
+    B, cap = point_map.shape
+    kf = np.ascontiguousarray(kf, np.int32).reshape(B, -1)
+    _, keep, to_dev = _torch_dev()
+    t = dict(kf=torch.from_numpy(kf.copy()).cuda(), n_kf=torch.from_numpy(_i32(n_kf).reshape(B).copy()).cuda(),
+             ref_kf=torch.from_numpy(_i32(ref_kf).reshape(B).copy()).cuda(),
+             pt_index=torch.zeros((B, cap_local_points), dtype=torch.int32, device="cuda"), pt_count=torch.zeros(B, dtype=torch.int32, device="cuda"),
+             ln_index=torch.zeros((B, cap_local_lines), dtype=torch.int32, device="cuda"), ln_count=torch.zeros(B, dtype=torch.int32, device="cuda"))
+    s = _local_map_struct(t, kf.shape[1], cap_local_points, cap_local_lines)
+    pm = to_dev(point_map)[1]
+    torch.cuda.synchronize()
+    check(_track_lib().pl_track_update_local_map_dev(map._h, B, pm, cap, _opt_dev(ok, B, to_dev), _opt_dev(vo, B, to_dev), C.byref(s), None))
+    torch.cuda.synchronize()
+    out = {k: v.cpu().numpy() for k, v in t.items()}
+    map.check_indices()
+    return out
+
+
+def track_local_map_lists(map, frames, local, frames_since_reloc, max_frames, taps=False, seen=None, ok=None, vo=None):
+    """track_local_map on device lists (pl_track_local_map_lists_dev): local = dict(pt_index [B][cap_local_points], pt_count [B],
+    ln_index [B][cap_local_lines], ln_count [B]) as update_local_map returns them (counts over a capacity are clamped);
+    frames_since_reloc [B]; ok / vo (optional [B]) gate the frames: a frame gated off passes through (Tcw = Tcw0, held matches
+    kept, outlier flags 0, ok = ok[b])."""
+    L = _track_lib()
+    B, cap = frames["keys_un"].shape[:2]
+    capL = frames["keylines"].shape[1]
+    nlev = len(frames["scale_factors"])
+    arr = dict(keys_un=np.ascontiguousarray(frames["keys_un"], KP_DTYPE), desc=np.ascontiguousarray(frames["desc"], np.uint8),
+               n=np.ascontiguousarray(frames["n"], np.int32), keylines=np.ascontiguousarray(frames["keylines"], KEYLINE_DTYPE),
+               line_func=np.ascontiguousarray(frames["line_func"], np.float64), line_desc=np.ascontiguousarray(frames["line_desc"], np.uint8),
+               nl=np.ascontiguousarray(frames["nl"], np.int32), bounds=_f32(frames["bounds"]), scale_factors=_f32(frames["scale_factors"]),
+               inv_level_sigma2=_f32(frames["inv_level_sigma2"]), Tcw0=_f32(frames["Tcw0"]).reshape(B, 16), K=_f32(frames["K"]).reshape(B, 4))
+    for k in ("point_map_in", "line_map_in"):
+        if frames.get(k) is not None:
+            arr[k] = np.ascontiguousarray(frames[k], np.int32)
+    torch, keep, to_dev = _torch_dev()
+    d = {k: to_dev(v)[1] for k, v in arr.items()}
+    F = PLTrackFrames(B, d["keys_un"], d["desc"], d["n"], cap, d["keylines"], d["line_func"], d["line_desc"], d["nl"], capL, d["bounds"],
+                      d["scale_factors"], d["inv_level_sigma2"], nlev, float(frames["log_scale_factor"]), d["Tcw0"], d["K"],
+                      d.get("point_map_in"), d.get("line_map_in"))
+    pi = np.ascontiguousarray(local["pt_index"], np.int32).reshape(B, -1); li = np.ascontiguousarray(local["ln_index"], np.int32).reshape(B, -1)
+    cLP, cLL = pi.shape[1], li.shape[1]
+    one = to_dev(np.zeros(B, np.int32))[1]
+    s = PLLocalMap(one, one, 1, one, to_dev(pi)[1], _opt_dev(local["pt_count"], B, to_dev), cLP, to_dev(li)[1],
+                   _opt_dev(local["ln_count"], B, to_dev), cLL)
+    since = _opt_dev(frames_since_reloc, B, to_dev)
+    ps = ls = None
+    if seen is not None:
+        ps = to_dev(np.ascontiguousarray(seen["point_seen"], np.int32).reshape(B, cap))[1]
+        ls = to_dev(np.ascontiguousarray(seen["line_seen"], np.int32).reshape(B, capL))[1]
+    okd, vod = _opt_dev(ok, B, to_dev), _opt_dev(vo, B, to_dev)
+    out = _run_dev(lambda o, scr: L.pl_track_local_map_lists_dev(map._h, C.byref(F), ps, ls, C.byref(s), since, int(max_frames), okd, vod,
+                                                                 C.byref(o), scr, None),
+                   B, cap, capL, cLP, cLL, taps, keep, torch, L.pl_track_local_map_lists_scratch_bytes)
+    map.check_indices()
+    return out
+
+
+def _ref_pose(fn, map, P, ref_kf, out=None):
+    import torch
+    B = len(ref_kf)
+    t = [torch.from_numpy(np.ascontiguousarray(a)).cuda() for a in
+         (_f32(P).reshape(B, 16), _i32(ref_kf).reshape(B), np.zeros((B, 16), np.float32) if out is None else _f32(out).reshape(B, 16).copy())]
+    torch.cuda.synchronize()
+    check(fn(map._h, B, *[vp(x.data_ptr()) for x in t], None))
+    torch.cuda.synchronize()
+    return t[2].cpu().numpy().reshape(B, 4, 4)
+
+
+def relative_pose(map, Tcw, ref_kf, out=None):
+    """Tcr = Tcw * Twc[ref_kf] for B frames (pl_track_relative_pose_dev, Tracking.cc:582).  A frame whose ref_kf is outside the
+    graph keeps `out`'s value (zeros if None) and Map.check_indices() raises."""
+    return _ref_pose(_track_lib().pl_track_relative_pose_dev, map, Tcw, ref_kf, out)
+
+
+def last_pose(map, Tcr, ref_kf, out=None):
+    """mLastFrame.mTcw = Tcr * Tcw[ref_kf] for B frames (pl_track_last_pose_dev, the monocular UpdateLastFrame, :1242-1245)."""
+    return _ref_pose(_track_lib().pl_track_last_pose_dev, map, Tcr, ref_kf, out)
+
+
+class LocalizationChain:
+    """The OK-state localisation frame for B independent streams against a fixed map with its keyframe graph, every buffer on the
+    device and allocated once, so that localization_step() only enqueues work (it may be captured into a CUDA graph):
+
+        last pose -> motion model -> update local map -> local-map step -> velocity -> relative pose
+
+    set_frames() uploads the current frames' features; set_state() the streams' state (the last frames, as TrackLocalMapWithLines
+    left them, Tcr, ref_kf, velocity, vo, the local keyframe lists).  After a step, fetch() returns every stage's outputs; the
+    current frames have become the last frames.  frames_since_reloc [B] (device tensor) is the caller's to update."""
+
+    def __init__(self, map, B, cap, capL, cap_kf, cap_local_points, cap_local_lines, bounds, scale_factors, inv_level_sigma2,
+                 log_scale_factor, max_frames=30):
+        import torch
+        self.map, self.B, self.cap, self.capL, self.cap_kf, self.cLP, self.cLL = map, B, cap, capL, cap_kf, cap_local_points, cap_local_lines
+        self.max_frames, self.log_scale_factor, self.nlev = int(max_frames), float(log_scale_factor), len(scale_factors)
+        dev = dict(device="cuda")
+        z = lambda shape, dt: torch.zeros(shape, dtype=dt, **dev)   # noqa: E731
+        u8, i32, f32, f64 = torch.uint8, torch.int32, torch.float32, torch.float64
+        kp, kl = np.dtype(KP_DTYPE).itemsize, np.dtype(KEYLINE_DTYPE).itemsize
+        self.tab = {k: torch.from_numpy(np.ascontiguousarray(v)).cuda() for k, v in
+                    (("bounds", _f32(bounds)), ("scale_factors", _f32(scale_factors)), ("inv_level_sigma2", _f32(inv_level_sigma2)))}
+        self.cur = dict(keys_un=z((B, cap * kp), u8), desc=z((B, cap, 32), u8), n=z(B, i32), keylines=z((B, capL * kl), u8),
+                        line_func=z((B, capL, 3), f64), line_desc=z((B, capL, 32), u8), nl=z(B, i32), K=z((B, 4), f32))
+        self.last = dict(keys_un=z((B, cap * kp), u8), n=z(B, i32), keylines=z((B, capL * kl), u8), nl=z(B, i32), point_map=z((B, cap), i32),
+                         point_outlier=z((B, cap), u8), line_map=z((B, capL), i32), line_outlier=z((B, capL), u8), Tcw=z((B, 16), f32),
+                         velocity=z((B, 16), f32))
+        self.state = dict(Tcr=z((B, 16), f32), vo=z(B, i32), frames_since_reloc=z(B, i32))
+        self.local = dict(kf=z((B, cap_kf), i32), n_kf=z(B, i32), ref_kf=z(B, i32), pt_index=z((B, cap_local_points), i32),
+                          pt_count=z(B, i32), ln_index=z((B, cap_local_lines), i32), ln_count=z(B, i32))
+        self.mm = {k: z(((B,) + shp[1:]) if len(shp) > 1 else B, getattr(torch, np.dtype(dt).name)) for k, (shp, dt) in
+                   _mm_shapes(B, cap, capL).items() if k in _MM_OUT[:8]}
+        self.mm["vo"] = self.state["vo"]                                       # mbVO is in / out
+        sh = _out_shapes(B, cap, capL, cap_local_points, cap_local_lines)
+        self.lo = {k: z(sh[k][0], getattr(torch, np.dtype(sh[k][1]).name)) for k in _TRACK_OUT[:7]}
+        L = _track_lib()
+        self.mm_scratch = torch.empty(int(L.pl_track_motion_model_scratch_bytes(B, cap, capL)), dtype=u8, **dev)
+        self.lo_scratch = torch.empty(int(L.pl_track_local_map_lists_scratch_bytes(B, cap, capL, cap_local_points, cap_local_lines)),
+                                      dtype=u8, **dev)
+        p = lambda t: vp(t.data_ptr())   # noqa: E731
+        c, la, tb = self.cur, self.last, self.tab
+
+        def frames(Tcw0, pm, lm):
+            return PLTrackFrames(B, p(c["keys_un"]), p(c["desc"]), p(c["n"]), cap, p(c["keylines"]), p(c["line_func"]), p(c["line_desc"]),
+                                 p(c["nl"]), capL, p(tb["bounds"]), p(tb["scale_factors"]), p(tb["inv_level_sigma2"]), self.nlev,
+                                 self.log_scale_factor, Tcw0, p(c["K"]), pm, lm)
+        self._F_mm = frames(None, None, None)
+        self._F_lo = frames(p(self.mm["Tcw"]), p(self.mm["point_map"]), p(self.mm["line_map"]))
+        self._last = PLTrackLast(*[p(la[k]) for k, _ in PLTrackLast._fields_])
+        self._mm_out = PLTrackMotionOut(*[p(self.mm[k]) if k in self.mm else None for k in _MM_OUT])
+        self._lo_out = PLTrackOut(*[p(self.lo[k]) if k in self.lo else None for k in _TRACK_OUT])
+        self._local = _local_map_struct(self.local, cap_kf, cap_local_points, cap_local_lines)
+
+    def set_frames(self, frames):
+        """frames: the current frames as for track_motion_model (keys_un, desc, n, keylines, line_func, line_desc, nl, K)."""
+        import torch
+        for k in ("keys_un", "desc", "n", "keylines", "line_func", "line_desc", "nl", "K"):
+            a = np.ascontiguousarray(frames[k])
+            self.cur[k].copy_(torch.from_numpy(a.view(np.uint8).reshape(self.cur[k].shape) if a.dtype.fields else
+                                               a.astype(np.dtype(str(self.cur[k].dtype).replace("torch.", ""))).reshape(self.cur[k].shape)))
+
+    def set_state(self, last, Tcr, ref_kf, velocity, kf, n_kf, vo=None, frames_since_reloc=None):
+        """last: the last frames as for track_motion_model (keys_un, n, keylines, nl, point_map, point_outlier, line_map,
+        line_outlier); Tcr [B][4][4] and ref_kf [B] of the last frames; velocity [B][4][4]; kf [B][cap_kf] / n_kf [B] the local
+        keyframe lists."""
+        import torch
+        B = self.B
+        put = lambda t, a: t.copy_(torch.from_numpy(np.ascontiguousarray(a).view(np.uint8).reshape(t.shape) if np.asarray(a).dtype.fields   # noqa: E731
+                                                   else np.ascontiguousarray(a).astype(np.dtype(str(t.dtype).replace("torch.", ""))).reshape(t.shape)))
+        for k in ("keys_un", "n", "keylines", "nl", "point_map", "point_outlier", "line_map", "line_outlier"):
+            put(self.last[k], last[k])
+        put(self.last["velocity"], _f32(velocity).reshape(B, 16)); put(self.state["Tcr"], _f32(Tcr).reshape(B, 16))
+        put(self.local["ref_kf"], _i32(ref_kf)); put(self.local["kf"], _i32(kf)); put(self.local["n_kf"], _i32(n_kf))
+        put(self.state["vo"], np.zeros(B, np.int32) if vo is None else _i32(vo))
+        put(self.state["frames_since_reloc"], np.full(B, 1 << 20, np.int32) if frames_since_reloc is None else _i32(frames_since_reloc))
+
+    def localization_step(self, stream=None):
+        """Enqueue one frame of every stream on `stream` (a torch.cuda.Stream; default the current stream).  No host
+        synchronisation and no host-to-device copy: only kernels and device-to-device copies."""
+        import torch
+        st = stream or torch.cuda.current_stream()
+        h = vp(st.cuda_stream or 1)      # the default stream as cudaStreamLegacy: NULL would select the map's own stream
+
+        L, M, B, p = _track_lib(), self.map._h, self.B, (lambda t: vp(t.data_ptr()))
+        la, mm, lo, loc = self.last, self.mm, self.lo, self.local
+        check(L.pl_track_last_pose_dev(M, B, p(self.state["Tcr"]), p(loc["ref_kf"]), p(la["Tcw"]), h))
+        check(L.pl_track_motion_model_dev(M, C.byref(self._F_mm), C.byref(self._last), C.byref(self._mm_out), p(self.mm_scratch), h))
+        check(L.pl_track_update_local_map_dev(M, B, p(mm["point_map"]), self.cap, p(mm["ok"]), p(mm["vo"]), C.byref(self._local), h))
+        check(L.pl_track_local_map_lists_dev(M, C.byref(self._F_lo), p(mm["point_seen"]), p(mm["line_seen"]), C.byref(self._local),
+                                             p(self.state["frames_since_reloc"]), self.max_frames, p(mm["ok"]), p(mm["vo"]),
+                                             C.byref(self._lo_out), p(self.lo_scratch), h))
+        check(L.pl_track_velocity_dev(B, p(lo["Tcw"]), p(la["Tcw"]), p(lo["ok"]), p(la["velocity"]), h))
+        check(L.pl_track_relative_pose_dev(M, B, p(lo["Tcw"]), p(loc["ref_kf"]), p(self.state["Tcr"]), h))
+        # the current frames become the last frames (mLastFrame = Frame(mCurrentFrame))
+        with torch.cuda.stream(st):
+            for k in ("keys_un", "n", "keylines", "nl"):
+                la[k].copy_(self.cur[k])
+            for k in ("point_map", "point_outlier", "line_map", "line_outlier"):
+                la[k].copy_(lo[k])
+
+    def fetch(self):
+        """Every stage's outputs as numpy: Tlast (the last pose of this step), mm (motion model), local (the local map), lo (the
+        local-map step), velocity and Tcr."""
+        import torch
+        torch.cuda.synchronize()
+        B = self.B
+        n = lambda t: t.cpu().numpy()   # noqa: E731
+        mm = {k: n(v) for k, v in self.mm.items()}
+        mm["Tcw"] = mm["Tcw"].reshape(B, 4, 4)
+        lo = {k: n(v) for k, v in self.lo.items()}
+        lo["Tcw"] = lo["Tcw"].reshape(B, 4, 4)
+        return dict(Tlast=n(self.last["Tcw"]).reshape(B, 4, 4), mm=mm, local={k: n(v) for k, v in self.local.items()}, lo=lo,
+                    velocity=n(self.last["velocity"]).reshape(B, 4, 4), Tcr=n(self.state["Tcr"]).reshape(B, 4, 4))

@@ -12,6 +12,7 @@
 #include "frustum.cuh"
 #include "search.cuh"
 #include <limits.h>
+#include <algorithm>
 #include <vector>
 
 struct PLMap {
@@ -21,8 +22,14 @@ struct PLMap {
   double *ln_pos = nullptr, *ln_normal = nullptr;
   float *ln_min = nullptr, *ln_max = nullptr;
   uint8_t* ln_desc = nullptr;
-  int* flag = nullptr;            // sticky: an index outside the map was met
+  int* flag = nullptr;            // sticky: [0] an index outside the map was met, [1] a local list outgrew its capacity
   cudaStream_t stream = nullptr;
+  // the keyframe graph (pl_map_set_keyframes); CSR rows per keyframe, obs per map point
+  int n_kf = 0;
+  float *kf_Tcw = nullptr, *kf_Twc = nullptr;
+  uint8_t* kf_bad = nullptr;
+  int *kf_parent = nullptr, *kf_pt_off = nullptr, *kf_pt = nullptr, *kf_ln_off = nullptr, *kf_ln = nullptr;
+  int *kf_cov_off = nullptr, *kf_cov = nullptr, *kf_child_off = nullptr, *kf_child = nullptr, *obs_off = nullptr, *obs = nullptr;
 };
 
 namespace pl {
@@ -212,7 +219,7 @@ __global__ void __launch_bounds__(kTrackThreads) k_track_writeback(const int* __
                                                                    const int* __restrict__ lslot, const uint8_t* __restrict__ lout, int capL,
                                                                    const int* __restrict__ min_inliers, uint8_t* __restrict__ point_outlier,
                                                                    uint8_t* __restrict__ line_outlier, int* __restrict__ inliers,
-                                                                   int* __restrict__ ok) {
+                                                                   const uint8_t* solve, const int* ok_in, int* ok) {
   __shared__ int cnt[2];
   const int b = blockIdx.x;
   if (threadIdx.x < 2) cnt[threadIdx.x] = 0;
@@ -237,7 +244,9 @@ __global__ void __launch_bounds__(kTrackThreads) k_track_writeback(const int* __
   __syncthreads();
   if (threadIdx.x == 0) {
     inliers[2 * b] = cnt[0]; inliers[2 * b + 1] = cnt[1];
-    ok[b] = cnt[0] >= min_inliers[b];   // < 50 shortly after a relocalisation, < 30 otherwise: false (:1555-1561)
+    // < 50 shortly after a relocalisation, < 30 otherwise: false (:1555-1561); a frame gated off keeps bOK (:476)
+    if (!solve || solve[b]) ok[b] = cnt[0] >= min_inliers[b];
+    else ok[b] = ok_in ? ok_in[b] : 1;
   }
 }
 
@@ -277,11 +286,25 @@ static size_t carve(void* base, int B, int cap, int capL, int cLP, int cLL, Trac
   return off;
 }
 static int pow2_at_least(int n) { int p = 1; while (p < n) p <<= 1; return p; }
+static int track_local_map_run(PLMap* map, const PLTrackFrames* F, const int* point_seen, const int* line_seen, const int* pt_index,
+                               int cLP, const int* ln_index, int cLL, const uint8_t* solve, const int* ok_in, const PLTrackOut* O,
+                               const TrackScratch& s, cudaStream_t st);
 }  // namespace pl
 using namespace pl;
 
+static void free_keyframes(PLMap* m) {
+  for (void* p : {(void*)m->kf_Tcw, (void*)m->kf_Twc, (void*)m->kf_bad, (void*)m->kf_parent, (void*)m->kf_pt_off, (void*)m->kf_pt,
+                  (void*)m->kf_ln_off, (void*)m->kf_ln, (void*)m->kf_cov_off, (void*)m->kf_cov, (void*)m->kf_child_off,
+                  (void*)m->kf_child, (void*)m->obs_off, (void*)m->obs})
+    cudaFree(p);
+  m->kf_Tcw = m->kf_Twc = nullptr; m->kf_bad = nullptr;
+  m->kf_parent = m->kf_pt_off = m->kf_pt = m->kf_ln_off = m->kf_ln = m->kf_cov_off = m->kf_cov = nullptr;
+  m->kf_child_off = m->kf_child = m->obs_off = m->obs = nullptr;
+  m->n_kf = 0;
+}
 extern "C" void pl_map_destroy(PLMap* m) {
   if (!m) return;
+  free_keyframes(m);
   for (void* p : {(void*)m->pt_pos, (void*)m->pt_normal, (void*)m->pt_min, (void*)m->pt_max, (void*)m->pt_desc, (void*)m->ln_pos,
                   (void*)m->ln_normal, (void*)m->ln_min, (void*)m->ln_max, (void*)m->ln_desc, (void*)m->flag})
     cudaFree(p);
@@ -306,8 +329,8 @@ extern "C" int pl_map_create(const PLMapDesc* d, PLMap** out) {
   up(&m->pt_min, d->pt_min_dist, np * 4, P * 4); up(&m->pt_max, d->pt_max_dist, np * 4, P * 4); up(&m->pt_desc, d->pt_desc, np * 32, P * 32);
   up(&m->ln_pos, d->ln_pos, nl * 48, L * 48); up(&m->ln_normal, d->ln_normal, nl * 24, L * 24);
   up(&m->ln_min, d->ln_min_dist, nl * 4, L * 4); up(&m->ln_max, d->ln_max_dist, nl * 4, L * 4); up(&m->ln_desc, d->ln_desc, nl * 32, L * 32);
-  up(&m->flag, nullptr, 4, 0);
-  if (e == cudaSuccess) e = cudaMemset(m->flag, 0, 4);
+  up(&m->flag, nullptr, 8, 0);
+  if (e == cudaSuccess) e = cudaMemset(m->flag, 0, 8);
   if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking);
   if (e != cudaSuccess) { set_error("pl_map_create: %s", cudaGetErrorString(e)); pl_map_destroy(m); return PL_ERR_CUDA; }
   *out = m;
@@ -375,6 +398,17 @@ extern "C" int pl_track_local_map_seen_dev(PLMap* map, const PLTrackFrames* F, c
   // pageable sources: the copies are staged before cudaMemcpyAsync returns, so the vectors may go
   PL_CUDA(cudaMemcpyAsync(s.tab, tab.data(), tab.size() * 4, cudaMemcpyHostToDevice, st));
   PL_CUDA(cudaMemcpyAsync(s.th, th.data(), th.size() * 4, cudaMemcpyHostToDevice, st));
+  return track_local_map_run(map, F, point_seen, line_seen, L->pt_index, cLP, L->ln_index, cLL, nullptr, nullptr, O, s, st);
+}
+
+namespace pl {
+// The body of the local-map step once the per-frame table is on the device: s.tab = [5][B] {pt_off, pt_cnt, ln_off, ln_cnt,
+// min_inliers} and s.th [B].  solve (may be NULL): frames with solve[b] == 0 build an empty problem, keep their pose and matches,
+// and get ok = ok_in[b] (1 if ok_in is NULL).
+static int track_local_map_run(PLMap* map, const PLTrackFrames* F, const int* point_seen, const int* line_seen, const int* pt_index,
+                               int cLP, const int* ln_index, int cLL, const uint8_t* solve, const int* ok_in, const PLTrackOut* O,
+                               const TrackScratch& s, cudaStream_t st) {
+  const int B = F->B, cap = F->cap_points, capL = F->cap_lines;
   const int* d_poff = s.tab; const int* d_pcnt = s.tab + B; const int* d_loff = s.tab + 2 * B; const int* d_lcnt = s.tab + 3 * B;
   const int* d_min_inl = s.tab + 4 * B;
   // outputs the caller asked for are the working arrays themselves
@@ -400,11 +434,11 @@ extern "C" int pl_track_local_map_seen_dev(PLMap* map, const PLTrackFrames* F, c
   // 2. isInFrustum(., 0.5) per (frame, local entry)
   TrackFrustumArgs A;
   A.Tcw0 = F->Tcw0; A.K = F->K; A.bounds = F->bounds; A.logScaleFactor = F->log_scale_factor; A.nlevels = F->nlevels; A.flag = map->flag;
-  A.off = d_poff; A.cnt = d_pcnt; A.index = L->pt_index; A.n_map = map->n_points; A.cap_local = cLP; A.held = s.pheld; A.n_held = s.nph;
+  A.off = d_poff; A.cnt = d_pcnt; A.index = pt_index; A.n_map = map->n_points; A.cap_local = cLP; A.held = s.pheld; A.n_held = s.nph;
   A.cap = cap; A.in_view = piv; A.proj = pproj; A.level = plev; A.view_cos = pvc; A.row = s.prow;
   k_track_frustum_points<<<dim3((cLP + 127) / 128, B), 128, 0, st>>>(A, map->pt_pos, map->pt_normal, map->pt_min, map->pt_max);
   PL_LAUNCH_CHECK();
-  A.off = d_loff; A.cnt = d_lcnt; A.index = L->ln_index; A.n_map = map->n_lines; A.cap_local = cLL; A.held = s.lheld; A.n_held = s.nlh;
+  A.off = d_loff; A.cnt = d_lcnt; A.index = ln_index; A.n_map = map->n_lines; A.cap_local = cLL; A.held = s.lheld; A.n_held = s.nlh;
   A.cap = capL; A.in_view = liv; A.proj = lproj; A.level = llev; A.view_cos = lvc; A.row = s.lrow;
   k_track_frustum_lines<<<dim3((cLL + 127) / 128, B), 128, 0, st>>>(A, map->ln_pos, map->ln_normal, map->ln_min, map->ln_max);
   PL_LAUNCH_CHECK();
@@ -421,16 +455,18 @@ extern "C" int pl_track_local_map_seen_dev(PLMap* map, const PLTrackFrames* F, c
   Bd.prow = s.prow; Bd.cap_lp = cLP; Bd.lrow = s.lrow; Bd.cap_ll = cLL; Bd.map_pt = map->pt_pos; Bd.map_ln = map->ln_pos;
   Bd.point_map = O->point_map; Bd.line_map = O->line_map; Bd.pslot = s.pslot; Bd.lslot = s.lslot;
   Bd.np = np; Bd.obs = obs; Bd.w = w; Bd.X = X; Bd.nlp = nl; Bd.lf = lf; Bd.lX = lX;
+  Bd.solve = solve;
   k_track_build<<<B, kTrackThreads, 0, st>>>(Bd);
   PL_LAUNCH_CHECK();
   if ((rc = pl_pose_optimization_dev(0, B, F->Tcw0, F->K, np, cap, obs, w, X, nl, capL, lf, lX, O->Tcw, s.pout, s.lout, s.inl, s.its, s.lm,
                                      st))) return rc;
   // 5. write back per feature
   k_track_writeback<<<B, kTrackThreads, 0, st>>>(s.pslot, s.pout, cap, s.lslot, s.lout, capL, d_min_inl, O->point_outlier, O->line_outlier,
-                                                  O->inliers, O->ok);
+                                                  O->inliers, solve, ok_in, O->ok);
   PL_LAUNCH_CHECK();
   return PL_OK;
 }
+}  // namespace pl
 
 // B = 1 on host pointers: stage, run, copy back, check the index flag.  The device arrays are sized by the counts.
 extern "C" int pl_track_local_map(PLMap* map, const PLTrackFrames* F, const PLTrackLocal* L, const PLTrackOut* O) {
@@ -842,6 +878,345 @@ extern "C" int pl_track_motion_model(PLMap* map, const PLTrackFrames* F, const P
 extern "C" int pl_track_velocity_dev(int B, const float* Tcw, const float* Tcw_last, const int* ok, float* velocity, void* stream) {
   PL_ARG(B >= 1 && Tcw && Tcw_last && ok && velocity);
   k_track_velocity<<<(B + 127) / 128, 128, 0, (cudaStream_t)stream>>>(B, Tcw, Tcw_last, ok, velocity);
+  PL_LAUNCH_CHECK();
+  return PL_OK;
+}
+
+// ---- Tracking::UpdateLocalMap (src/Tracking.cc:1899-2081) for a batch of frames against the map's keyframe graph:
+//   k_update_local_map       one CTA per frame: UpdateLocalKeyFrames (votes, first maximum, the bounded expansion), then
+//                            UpdateLocalPoints / UpdateLocalLines (first occurrences in list order, then slot order)
+//   k_ref_pose               Tcr = Tcw * Twc[ref] (:582) and the monocular UpdateLastFrame, Tcr * Tcw[ref] (:1242-1245)
+// Shared memory per CTA: 4 B per keyframe (the votes, then the local keyframe list), 1 bit per keyframe (mnTrackReferenceForFrame
+// of the keyframes) and 1 bit per map point or map line (mnTrackReferenceForFrame of the entries, points and lines in turn).
+namespace pl {
+constexpr int kMaxGraphKF = 16384;           // 64 KB of votes + 2 KB of keyframe bits
+constexpr int kMaxGraphEntries = 1 << 20;    // map points and map lines each: 128 KB of bits
+constexpr int kLocalKFLimit = 80;            // if(mvpLocalKeyFrames.size()>80) break (:2027)
+
+struct ULMArgs {
+  int n_kf, n_points, n_lines, bit_words;
+  const uint8_t* bad; const int* parent;
+  const int *pt_off, *pt, *ln_off, *ln, *cov_off, *cov, *child_off, *child, *obs_off, *obs;
+  const int* point_map; int cap; const int* ok; const int* vo;
+  int* kf; int* n_kf_out; int cap_kf; int* ref_kf;
+  int* lp; int* n_lp; int cap_lp; int* ll; int* n_ll; int cap_ll;
+  int* flag;                                  // [0] index, [1] capacity
+};
+
+__device__ __forceinline__ bool bit_test(const unsigned* bits, int i) { return (bits[i >> 5] >> (i & 31)) & 1u; }
+
+// First occurrences over the local keyframes list[0..nlist) in list order, then in slot order (mnTrackReferenceForFrame,
+// :1916-1971), into out[b][cap_out]; the true count goes to n_out[b].  A chunk of slots claims its entries with atomicOr; when an
+// entry occurs twice in one chunk the claim may go to the later slot, so such a chunk decides by slot order instead.
+__device__ void local_entries(const ULMArgs& A, const int* list, int nlist, const int* off, const int* slot, unsigned* bits,
+                              int* s_val, int* warp_tot, int* out, int* n_out, int cap_out) {
+  const int b = blockIdx.x, tid = threadIdx.x;
+  __syncthreads();
+  for (int w = tid; w < A.bit_words; w += kTrackThreads) bits[w] = 0u;
+  __syncthreads();
+  int base = 0;
+  for (int j = 0; j < nlist; j++) {
+    const int k = list[j];
+    const int s1 = off[k + 1];
+    for (int c = off[k]; c < s1; c += kTrackThreads) {
+      const int i = c + tid;
+      const int m = i < s1 ? slot[i] : -1;          // in range: pl_map_set_keyframes checked every slot
+      const bool fresh = m >= 0 && !bit_test(bits, m);
+      __syncthreads();                                  // every test of this chunk before its claims
+      bool first = false;
+      if (fresh) first = !(atomicOr(&bits[m >> 5], 1u << (m & 31)) & (1u << (m & 31)));
+      if (__syncthreads_or(fresh && !first)) {
+        s_val[tid] = fresh ? m : -1;
+        __syncthreads();
+        first = fresh;
+        for (int t = 0; t < tid && first; t++) first = s_val[t] != m;
+        __syncthreads();
+      }
+      const int pos = block_slot(first, warp_tot, base);
+      if (first && pos < cap_out) out[(long long)b * cap_out + pos] = m;
+    }
+  }
+  if (tid == 0) {
+    n_out[b] = base;
+    if (base > cap_out) atomicOr(A.flag + 1, 1);
+  }
+}
+
+__global__ void __launch_bounds__(kTrackThreads) k_update_local_map(ULMArgs A) {
+  extern __shared__ int smem[];
+  int* list = smem;                                               // [n_kf]: the votes, then mvpLocalKeyFrames
+  unsigned* kfbits = (unsigned*)(smem + A.n_kf);                  // [(n_kf + 31) / 32]
+  unsigned* bits = kfbits + (A.n_kf + 31) / 32;                   // [bit_words]
+  __shared__ int warp_tot[kTrackThreads / 32], s_val[kTrackThreads], red_v[kTrackThreads / 32], red_k[kTrackThreads / 32];
+  __shared__ int s_size;
+  const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  if ((A.ok && !A.ok[b]) || (A.vo && A.vo[b])) {                 // if(bOK && !mbVO) TrackLocalMapWithLines() (:476)
+    if (tid == 0) { A.n_lp[b] = 0; A.n_ll[b] = 0; }
+    return;
+  }
+  // 1. keyframeCounter: one vote per observation of every matched point (:1977-1993); lines do not vote
+  for (int k = tid; k < A.n_kf; k += kTrackThreads) list[k] = 0;
+  for (int w = tid; w < (A.n_kf + 31) / 32; w += kTrackThreads) kfbits[w] = 0u;
+  __syncthreads();
+  for (int i = tid; i < A.cap; i += kTrackThreads) {
+    const int m = A.point_map[(long long)b * A.cap + i];
+    if (m < 0) continue;
+    if (m >= A.n_points) { atomicOr(A.flag, 1); continue; }
+    for (int o = A.obs_off[m]; o < A.obs_off[m + 1]; o++) atomicAdd(&list[A.obs[o]], 1);
+  }
+  __syncthreads();
+  bool any = false;
+  for (int k = tid; k < A.n_kf; k += kTrackThreads) any |= list[k] > 0;
+  int nlist;
+  if (__syncthreads_or(any)) {
+    // 2. the good voters in index order (map<KeyFrame*,int> order), and pKFmax = the first strict maximum among them (:2005-2020)
+    int bv = 0, bk = -1;
+    for (int k = tid; k < A.n_kf; k += kTrackThreads) {
+      const int v = list[k];
+      if (v > bv && !(A.bad && A.bad[k])) { bv = v; bk = k; }
+    }
+    for (int d = 16; d; d >>= 1) {
+      const int ov = __shfl_down_sync(0xffffffffu, bv, d), ok_ = __shfl_down_sync(0xffffffffu, bk, d);
+      if (ov > bv || (ov == bv && ok_ >= 0 && (bk < 0 || ok_ < bk))) { bv = ov; bk = ok_; }
+    }
+    if (lane == 0) { red_v[warp] = bv; red_k[warp] = bk; }
+    __syncthreads();
+    if (tid == 0) {
+      for (int w = 1; w < kTrackThreads / 32; w++)
+        if (red_v[w] > bv || (red_v[w] == bv && red_k[w] >= 0 && (bk < 0 || red_k[w] < bk))) { bv = red_v[w]; bk = red_k[w]; }
+      if (bk >= 0) A.ref_kf[b] = bk;                               // if(pKFmax) mpReferenceKF = pKFmax (:2076-2080)
+    }
+    // compact the good voters in place: a voter's position is at most its index, and a chunk reads before it writes
+    int base = 0;
+    for (int c = 0; c < A.n_kf; c += kTrackThreads) {
+      const int k = c + tid;
+      const bool f = k < A.n_kf && list[k] > 0 && !(A.bad && A.bad[k]);
+      const int pos = block_slot(f, warp_tot, base);
+      if (f) { list[pos] = k; atomicOr(&kfbits[k >> 5], 1u << (k & 31)); }
+    }
+    __syncthreads();
+    const int nvot = base;
+    // 3. neighbours of the ORIGINAL voters only: itEndKF is fixed before the push_backs (:2024-2074)
+    if (warp == 0) {
+      int size = nvot;
+      for (int i = 0; i < nvot; i++) {
+        if (size > kLocalKFLimit) break;
+        const int k = list[i];
+        // the first of GetBestCovisibilityKeyFrames(10) that is good and not yet in
+        const int c0 = A.cov_off[k], nc = min(A.cov_off[k + 1] - c0, 10);
+        int c = lane < nc ? A.cov[c0 + lane] : -1;
+        unsigned bal = __ballot_sync(0xffffffffu, c >= 0 && !(A.bad && A.bad[c]) && !bit_test(kfbits, c));
+        if (bal) {
+          c = __shfl_sync(0xffffffffu, c, __ffs(bal) - 1);
+          if (lane == 0) { list[size] = c; kfbits[c >> 5] |= 1u << (c & 31); }
+          size++;
+        }
+        __syncwarp();
+        // the first child in set order that is good and not yet in
+        const int h1 = A.child_off[k + 1];
+        for (int j = A.child_off[k]; j < h1; j += 32) {
+          int h = j + lane < h1 ? A.child[j + lane] : -1;
+          bal = __ballot_sync(0xffffffffu, h >= 0 && !(A.bad && A.bad[h]) && !bit_test(kfbits, h));
+          if (bal) {
+            h = __shfl_sync(0xffffffffu, h, __ffs(bal) - 1);
+            if (lane == 0) { list[size] = h; kfbits[h >> 5] |= 1u << (h & 31); }
+            size++;
+            break;
+          }
+        }
+        __syncwarp();
+        // the parent, not checked for isBad; its break ends the whole expansion
+        const int p = A.parent[k];
+        if (p >= 0 && !bit_test(kfbits, p)) {
+          if (lane == 0) list[size] = p;
+          size++;
+          break;
+        }
+      }
+      if (lane == 0) s_size = size;
+    }
+    __syncthreads();
+    nlist = s_size;
+    for (int j = tid; j < min(nlist, A.cap_kf); j += kTrackThreads) A.kf[(long long)b * A.cap_kf + j] = list[j];
+    if (tid == 0) {
+      A.n_kf_out[b] = nlist;
+      if (nlist > A.cap_kf) atomicOr(A.flag + 1, 1);
+    }
+  } else {
+    // keyframeCounter.empty(): return early; mvpLocalKeyFrames and mpReferenceKF keep their values and the points and lines are
+    // rebuilt from that list (:1995-1996)
+    nlist = min(min(A.n_kf_out[b], A.cap_kf), A.n_kf);
+    __syncthreads();
+    for (int j = tid; j < nlist; j += kTrackThreads) {
+      int k = A.kf[(long long)b * A.cap_kf + j];
+      if (k < 0 || k >= A.n_kf) { atomicOr(A.flag, 1); k = -1; }
+      list[j] = k;
+    }
+    __syncthreads();
+    // an index outside the graph is dropped from the walk, keeping the order of the others
+    if (tid == 0) {
+      int w = 0;
+      for (int j = 0; j < nlist; j++) if (list[j] >= 0) list[w++] = list[j];
+      s_size = w;
+    }
+    __syncthreads();
+    nlist = s_size;
+  }
+  // 4. mvpLocalMapPoints and mvpLocalMapLines
+  local_entries(A, list, nlist, A.pt_off, A.pt, bits, s_val, warp_tot, A.lp, A.n_lp, A.cap_lp);
+  local_entries(A, list, nlist, A.ln_off, A.ln, bits, s_val, warp_tot, A.ll, A.n_ll, A.cap_ll);
+}
+
+// out[b] = P[b] * Q[ref[b]] with cv::Mat's fp32 product; a ref outside the graph sets the index flag and leaves out[b]
+__global__ void __launch_bounds__(128) k_ref_pose(int B, const float* __restrict__ P, const int* __restrict__ ref, const float* __restrict__ Q,
+                                                  int n_kf, float* __restrict__ out, int* __restrict__ flag) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  const int r = ref[b];
+  if (r < 0 || r >= n_kf) { atomicOr(flag, 1); return; }
+  float L[16], R[16];
+  for (int k = 0; k < 16; k++) { L[k] = P[16 * b + k]; R[k] = Q[16 * (long long)r + k]; }
+  for (int k = 0; k < 16; k++) out[16 * b + k] = mat4_elem(L, R, k >> 2, k & 3);
+}
+
+// the per-frame table of the local-map step from device lists: offsets b * cap, counts clamped to the capacity (0 for a frame
+// gated off), min inliers and th from frames_since_reloc, and the gate itself
+__global__ void __launch_bounds__(128) k_lists_prep(int B, const int* __restrict__ pcnt, int cLP, const int* __restrict__ lcnt, int cLL,
+                                                    const int* __restrict__ since, int max_frames, const int* __restrict__ ok,
+                                                    const int* __restrict__ vo, int* __restrict__ tab, float* __restrict__ th,
+                                                    uint8_t* __restrict__ solve) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  const bool run = (!ok || ok[b]) && (!vo || !vo[b]);
+  tab[b] = b * cLP; tab[B + b] = run ? min(max(pcnt[b], 0), cLP) : 0;
+  tab[2 * B + b] = b * cLL; tab[3 * B + b] = run ? min(max(lcnt[b], 0), cLL) : 0;
+  tab[4 * B + b] = since[b] < max_frames ? 50 : 30;
+  th[b] = since[b] < 2 ? 5.0f : 1.0f;
+  solve[b] = run;
+}
+
+static size_t up_bytes(size_t n) { return (n + 15) / 16 * 16; }
+}  // namespace pl
+
+extern "C" int pl_map_set_keyframes(PLMap* m, const PLKeyFrameGraphDesc* g) {
+  PL_ARG(m && g && g->n_kf >= 1 && g->n_kf <= kMaxGraphKF);
+  PL_ARG(m->n_points <= kMaxGraphEntries && m->n_lines <= kMaxGraphEntries);
+  PL_ARG(g->Tcw && g->Twc && g->parent && g->pt_slot_offset && g->ln_slot_offset && g->cov_offset && g->child_offset && g->obs_offset);
+  const int K = g->n_kf;
+  // every CSR starts at 0 and is monotone; every index is in range
+  auto csr = [](const int* off, int rows, const int* idx, int lo, int hi, const char* what) -> bool {
+    if (off[0] != 0) { set_error("keyframe graph: %s offsets must start at 0", what); return false; }
+    for (int r = 0; r < rows; r++)
+      if (off[r + 1] < off[r]) { set_error("keyframe graph: %s offsets are not monotone at row %d", what, r); return false; }
+    if (off[rows] > 0 && !idx) { set_error("keyframe graph: %s has entries but no index array", what); return false; }
+    for (int i = 0; i < off[rows]; i++)
+      if (idx[i] < lo || idx[i] >= hi) { set_error("keyframe graph: %s entry %d = %d is outside [%d, %d)", what, i, idx[i], lo, hi); return false; }
+    return true;
+  };
+  if (!csr(g->pt_slot_offset, K, g->pt_slot, -1, m->n_points, "point slots") ||
+      !csr(g->ln_slot_offset, K, g->ln_slot, -1, m->n_lines, "line slots") || !csr(g->cov_offset, K, g->cov, 0, K, "covisibles") ||
+      !csr(g->child_offset, K, g->child, 0, K, "children") || !csr(g->obs_offset, m->n_points, g->obs, 0, K, "observations"))
+    return PL_ERR_ARG;
+  for (int k = 0; k < K; k++)
+    if (g->parent[k] < -1 || g->parent[k] >= K) { set_error("keyframe graph: parent of %d = %d is outside the graph", k, g->parent[k]); return PL_ERR_ARG; }
+  int rc = require_device(); if (rc) return rc;
+  // mspChildrens iterates in KeyFrame* order, which is index order
+  std::vector<int> child(g->child, g->child + g->child_offset[K]);
+  for (int k = 0; k < K; k++) std::sort(child.begin() + g->child_offset[k], child.begin() + g->child_offset[k + 1]);
+  std::vector<uint8_t> bad(K, 0);
+  if (g->bad) for (int k = 0; k < K; k++) bad[k] = g->bad[k] != 0;
+  free_keyframes(m);
+  cudaError_t e = cudaSuccess;
+  auto up = [&](auto** dst, const void* src, size_t bytes) {
+    if (e == cudaSuccess) e = cudaMalloc((void**)dst, std::max<size_t>(bytes, 16));
+    if (e == cudaSuccess && bytes) e = cudaMemcpy(*dst, src, bytes, cudaMemcpyHostToDevice);
+  };
+  const size_t k = K, np = m->n_points;
+  up(&m->kf_Tcw, g->Tcw, k * 64); up(&m->kf_Twc, g->Twc, k * 64); up(&m->kf_bad, bad.data(), k); up(&m->kf_parent, g->parent, k * 4);
+  up(&m->kf_pt_off, g->pt_slot_offset, (k + 1) * 4); up(&m->kf_pt, g->pt_slot, (size_t)g->pt_slot_offset[K] * 4);
+  up(&m->kf_ln_off, g->ln_slot_offset, (k + 1) * 4); up(&m->kf_ln, g->ln_slot, (size_t)g->ln_slot_offset[K] * 4);
+  up(&m->kf_cov_off, g->cov_offset, (k + 1) * 4); up(&m->kf_cov, g->cov, (size_t)g->cov_offset[K] * 4);
+  up(&m->kf_child_off, g->child_offset, (k + 1) * 4); up(&m->kf_child, child.data(), child.size() * 4);
+  up(&m->obs_off, g->obs_offset, (np + 1) * 4); up(&m->obs, g->obs, (size_t)g->obs_offset[np] * 4);
+  if (e != cudaSuccess) { set_error("pl_map_set_keyframes: %s", cudaGetErrorString(e)); free_keyframes(m); return PL_ERR_CUDA; }
+  m->n_kf = K;
+  return PL_OK;
+}
+
+extern "C" int pl_map_check_capacity(PLMap* m) {
+  PL_ARG(m);
+  int f = 0;
+  PL_CUDA(cudaDeviceSynchronize());
+  PL_CUDA(cudaMemcpy(&f, m->flag + 1, 4, cudaMemcpyDeviceToHost));
+  if (!f) return PL_OK;
+  PL_CUDA(cudaMemset(m->flag + 1, 0, 4));
+  set_error("track: a local keyframe, map point or map line list outgrew its capacity (the counts hold the true sizes)");
+  return PL_ERR_ARG;
+}
+
+extern "C" int pl_track_update_local_map_dev(PLMap* map, int B, const int* point_map, int cap_points, const int* ok, const int* vo,
+                                             const PLLocalMap* L, void* stream) {
+  PL_ARG(map && L && point_map && B >= 1 && cap_points >= 1);
+  if (map->n_kf < 1) { set_error("pl_track_update_local_map_dev: the map has no keyframe graph (pl_map_set_keyframes)"); return PL_ERR_ARG; }
+  PL_ARG(L->kf && L->n_kf && L->ref_kf && L->pt_index && L->pt_count && L->ln_index && L->ln_count);
+  PL_ARG(L->cap_kf >= 1 && L->cap_local_points >= 1 && L->cap_local_lines >= 1);
+  ULMArgs A;
+  A.n_kf = map->n_kf; A.n_points = map->n_points; A.n_lines = map->n_lines;
+  A.bit_words = (std::max(std::max(map->n_points, map->n_lines), 1) + 31) / 32;
+  A.bad = map->kf_bad; A.parent = map->kf_parent; A.pt_off = map->kf_pt_off; A.pt = map->kf_pt; A.ln_off = map->kf_ln_off; A.ln = map->kf_ln;
+  A.cov_off = map->kf_cov_off; A.cov = map->kf_cov; A.child_off = map->kf_child_off; A.child = map->kf_child;
+  A.obs_off = map->obs_off; A.obs = map->obs;
+  A.point_map = point_map; A.cap = cap_points; A.ok = ok; A.vo = vo;
+  A.kf = L->kf; A.n_kf_out = L->n_kf; A.cap_kf = L->cap_kf; A.ref_kf = L->ref_kf;
+  A.lp = L->pt_index; A.n_lp = L->pt_count; A.cap_lp = L->cap_local_points; A.ll = L->ln_index; A.n_ll = L->ln_count;
+  A.cap_ll = L->cap_local_lines; A.flag = map->flag;
+  const int smem = (A.n_kf + (A.n_kf + 31) / 32 + A.bit_words) * 4;
+  PL_CUDA(cudaFuncSetAttribute(k_update_local_map, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  k_update_local_map<<<B, kTrackThreads, smem, stream ? (cudaStream_t)stream : map->stream>>>(A);
+  PL_LAUNCH_CHECK();
+  return PL_OK;
+}
+
+extern "C" size_t pl_track_local_map_lists_scratch_bytes(int B, int cap_points, int cap_lines, int cap_local_points, int cap_local_lines) {
+  const size_t s = pl_track_local_map_scratch_bytes(B, cap_points, cap_lines, cap_local_points, cap_local_lines);
+  return s ? s + up_bytes(B) : 0;
+}
+
+extern "C" int pl_track_local_map_lists_dev(PLMap* map, const PLTrackFrames* F, const int* point_seen, const int* line_seen,
+                                            const PLLocalMap* L, const int* frames_since_reloc, int max_frames, const int* ok,
+                                            const int* vo, const PLTrackOut* O, void* scratch, void* stream_) {
+  PL_ARG(map && F && L && O && scratch && frames_since_reloc);
+  const int B = F->B, cap = F->cap_points, capL = F->cap_lines;
+  PL_ARG(B >= 1 && cap >= 1 && cap <= 6144 && capL >= 1 && capL <= 32768 && F->nlevels >= 1);
+  PL_ARG(F->keys_un && F->desc && F->n && F->keylines && F->line_func && F->line_desc && F->nl && F->bounds && F->scale_factors &&
+         F->inv_level_sigma2 && F->Tcw0 && F->K);
+  PL_ARG(L->pt_index && L->pt_count && L->ln_index && L->ln_count && L->cap_local_points >= 1 && L->cap_local_lines >= 1);
+  PL_ARG(O->Tcw && O->point_map && O->point_outlier && O->line_map && O->line_outlier && O->inliers && O->ok);
+  const int cLP = L->cap_local_points, cLL = L->cap_local_lines;
+  PL_ARG((long long)B * cLP <= INT_MAX && (long long)B * cLL <= INT_MAX);   // the frustum kernels index the lists with int offsets
+  cudaStream_t st = stream_ ? (cudaStream_t)stream_ : map->stream;
+  TrackScratch s;
+  const size_t off = carve(scratch, B, cap, capL, cLP, cLL, &s);
+  uint8_t* solve = (uint8_t*)scratch + off;
+  k_lists_prep<<<(B + 127) / 128, 128, 0, st>>>(B, L->pt_count, cLP, L->ln_count, cLL, frames_since_reloc, max_frames, ok, vo, s.tab, s.th,
+                                                solve);
+  PL_LAUNCH_CHECK();
+  return track_local_map_run(map, F, point_seen, line_seen, L->pt_index, cLP, L->ln_index, cLL, solve, ok, O, s, st);
+}
+
+extern "C" int pl_track_relative_pose_dev(PLMap* map, int B, const float* Tcw, const int* ref_kf, float* Tcr, void* stream) {
+  PL_ARG(map && B >= 1 && Tcw && ref_kf && Tcr);
+  if (map->n_kf < 1) { set_error("pl_track_relative_pose_dev: the map has no keyframe graph (pl_map_set_keyframes)"); return PL_ERR_ARG; }
+  k_ref_pose<<<(B + 127) / 128, 128, 0, stream ? (cudaStream_t)stream : map->stream>>>(B, Tcw, ref_kf, map->kf_Twc, map->n_kf, Tcr, map->flag);
+  PL_LAUNCH_CHECK();
+  return PL_OK;
+}
+
+extern "C" int pl_track_last_pose_dev(PLMap* map, int B, const float* Tcr, const int* ref_kf, float* Tcw_last, void* stream) {
+  PL_ARG(map && B >= 1 && Tcr && ref_kf && Tcw_last);
+  if (map->n_kf < 1) { set_error("pl_track_last_pose_dev: the map has no keyframe graph (pl_map_set_keyframes)"); return PL_ERR_ARG; }
+  k_ref_pose<<<(B + 127) / 128, 128, 0, stream ? (cudaStream_t)stream : map->stream>>>(B, Tcr, ref_kf, map->kf_Tcw, map->n_kf, Tcw_last,
+                                                                                      map->flag);
   PL_LAUNCH_CHECK();
   return PL_OK;
 }
