@@ -192,6 +192,10 @@ int pl_line_debug_segments(PLLine* h, int frame, float* out, int cap);
 int pl_line_debug_scaled(PLLine* h, int frame, uint8_t* out, int* sw, int* sh);
 int pl_line_debug_sobel(PLLine* h, int frame, short* dx, short* dy);
 int pl_line_debug_order(PLLine* h, int frame, unsigned* out, int cap);
+/* which sort built the seed order of the LAST call: 1 the cluster kernel k_lsd_seed_order, 0 k_lsd_hist/scan/scatter */
+int pl_line_debug_seed_path(PLLine* h);
+/* fill every byte of the seed order and of its lengths with `byte` (tests: a later call must rewrite all it reports) */
+int pl_line_debug_fill_order(PLLine* h, int byte);
 /* control words of the speculative region growing for one frame of the LAST call (counters; post-mortem of the watchdog) */
 int pl_line_debug_ctl(PLLine* h, int frame, int* out, int nwords);
 

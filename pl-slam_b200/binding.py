@@ -319,6 +319,8 @@ class LINEextractor:
         L.pl_line_debug_scaled.argtypes = [vp, C.c_int, vp, vp, vp]
         L.pl_line_debug_sobel.argtypes = [vp, C.c_int, vp, vp]
         L.pl_line_debug_order.argtypes = [vp, C.c_int, vp, C.c_int]
+        L.pl_line_debug_seed_path.argtypes = [vp]
+        L.pl_line_debug_fill_order.argtypes = [vp, C.c_int]
         check(L.pl_line_create(C.byref(self.cfg), C.byref(self._h)))
         self.capacity = check(L.pl_line_capacity(self._h))
 
@@ -377,6 +379,14 @@ class LINEextractor:
         out = np.zeros(max(n, 1), np.uint32)
         check(lib().pl_line_debug_order(self._h, frame, _p(out), n))
         return out[:n]
+
+    def debug_seed_path(self):
+        """1 if the last call sorted the seeds with the cluster kernel (k_lsd_seed_order), 0 with k_lsd_hist/scan/scatter."""
+        return check(lib().pl_line_debug_seed_path(self._h))
+
+    def debug_fill_order(self, byte=0xFF):
+        """Overwrite the seed order and its lengths with `byte`, so that the next call must write every entry it reports."""
+        check(lib().pl_line_debug_fill_order(self._h, byte))
 
 
 # ---------------------------------------------------------------------------------------------- front-end pipeline

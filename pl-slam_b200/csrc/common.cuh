@@ -12,6 +12,9 @@ namespace pl {
 void set_error(const char* fmt, ...);
 extern std::atomic<unsigned long long> g_launches;  // kernels launched by this library (any thread)
 inline void count_launch(int n = 1) { g_launches.fetch_add((unsigned long long)n, std::memory_order_relaxed); }
+// From this many frames per SM on, pl_frontend_run_dev runs its three chains on one stream (k_lsd_grow_ordered fills every
+// SM), and pl_line_extract_batch_dev sorts the LSD seeds with the cluster kernel, which loses beside the other streams
+constexpr int kSerialFramesPerSM = 32;
 
 #define PL_CUDA(expr)                                                                       \
   do {                                                                                      \

@@ -190,7 +190,7 @@ extern "C" int pl_frontend_create(const PLFrontendConfig* cfg, PLFrontend** out)
     int dev = 0, sms = 132;
     FE_CUDA(cudaGetDevice(&dev));
     FE_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    h->serial_batch = 32 * sms;
+    h->serial_batch = pl::kSerialFramesPerSM * sms;
   }
   if (const char* e = getenv("PLSLAM_FRONTEND_ORDER")) {
     const std::string o(e);

@@ -8,8 +8,10 @@
 // Kernel map (DESIGN.md §6)
 //   k_lsd_scale     7x7 sigma .75 Gaussian (8.8 fixed point) fused with the 0.8x INTER_LINEAR_EXACT resize, smem tiles
 //   k_lsd_grad      2x2 gradient -> one 16-byte record per pixel (angle, cos, sin, squared magnitude), per-frame max
-//   k_lsd_hist/scan/scatter   stable counting sort of the defined pixels into 1024 magnitude bins (descending),
-//                   equal bins keep row-major order == OpenCV 4.13's seed order (pinned in the oracle tests)
+//   k_lsd_seed_order  stable counting sort of the defined pixels into 1024 magnitude bins (descending),
+//                   equal bins keep row-major order == OpenCV 4.13's seed order (pinned in the oracle tests); one
+//                   8-CTA cluster per frame, the order assembled in distributed shared memory.  k_lsd_hist/scan/scatter:
+//                   the same sort through HBM (below 32 frames per SM, and frames too large for the cluster)
 //   k_lsd_grow      region growing + rectangle fit + density refinement; inherently ordered (a pixel consumed by an
 //                   earlier seed is unavailable to later ones) -> ONE warp per frame walks the seeds in order; the 32
 //                   lanes test the 3x3 neighbourhood, evaluate angles and reduce the rectangle moments in parallel.
@@ -22,6 +24,7 @@
 #include "common.cuh"
 #include "lsd_grow_core.cuh"
 #include "libm_glibc.cuh"
+#include <cooperative_groups.h>
 #include <math.h>
 #include <string.h>
 #include <stdlib.h>
@@ -30,6 +33,7 @@
 
 namespace pl {
 
+namespace cg = cooperative_groups;
 constexpr double kPI = 3.14159265358979323846;
 constexpr double kDegToRads = kPI / 180;
 constexpr int kBins = 1024;
@@ -308,6 +312,133 @@ __global__ void __launch_bounds__(128) k_lsd_scatter(LineParams P, const int* __
     if (bin >= 0 && (peers & lt) == 0) cnt[wid][bin] += (unsigned short)__popc(peers);
     __syncwarp();
   }
+}
+
+// K_CDE the same stable counting sort in one thread-block cluster per frame, on chip (the default from 32 frames per SM on,
+// see pl_line_extract_batch_dev).  The scatter above stores 4 bytes per pixel into ~50k (bin, chunk) runs of
+// 2-4 entries spread over the whole order array, so at full batches the order sectors leave L2 partly written.  Here:
+//   CTA r of the cluster covers the pixel range [r*Q, (r+1)*Q) of the frame (rows 0..sh-2, row-major), its warp w the
+//   w-th piece of U pixels of that range
+//   1. histogram   per-(warp, bin) counts in shared memory (16-bit, two per 32-bit word for the atomics)
+//   2. scan        counts -> within-CTA exclusive offsets over the warps; the CTA's per-bin totals are exchanged through
+//                  distributed shared memory, every CTA derives the (bin desc, CTA asc) bases itself; CTA 0 writes ndef
+//   3. scatter     each warp walks its piece in row-major order exactly like k_lsd_scatter and stores every entry into the
+//                  shared memory of the CTA that owns its output position (CTA q owns [q*S, (q+1)*S))
+//   4. flush       after a cluster barrier each CTA writes its slice of order [0, ndef) with 16-byte stores
+// S2 is read twice (the second pass finds it in L2: the cluster has just read it); order is written once, in full sectors.
+constexpr int kSeedCta = 8;       // CTAs per cluster (one cluster per frame)
+constexpr int kSeedWarps = 32;    // warps per CTA
+__device__ __forceinline__ int seed_bin(int sv, int s_th, double bin_coef) { return sv > s_th ? s_bin(sv, bin_coef) : -1; }
+
+__global__ void __cluster_dims__(kSeedCta, 1, 1) __launch_bounds__(kSeedWarps * 32, 1)
+k_lsd_seed_order(LineParams P, int Q, int U, int S, const int* __restrict__ S2, const int* __restrict__ maxs,
+                 unsigned* __restrict__ order, int* __restrict__ ndef) {
+  extern __shared__ __align__(16) unsigned char seed_smem[];
+  unsigned* slice = reinterpret_cast<unsigned*>(seed_smem);                     // [S] this CTA's part of the order
+  unsigned short* cnt = reinterpret_cast<unsigned short*>(slice + S);           // [kSeedWarps][kBins]
+  int* tot = reinterpret_cast<int*>(cnt + kSeedWarps * kBins);                  // [kBins] this CTA's count per bin
+  int* base = tot + kBins;                                                      // [kBins] first position of (bin, this CTA)
+  __shared__ int wsum[kSeedWarps];
+  __shared__ int s_nd;
+  cg::cluster_group cluster = cg::this_cluster();
+  const int r = (int)cluster.block_rank(), f = blockIdx.y;
+  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+  for (int i = tid; i < kSeedWarps * kBins / 2; i += kSeedWarps * 32) reinterpret_cast<unsigned*>(cnt)[i] = 0u;
+  const int ms = maxs[f];
+  const double max_grad = ms > 0 ? sqrt((double)ms / 4.0) : -1.0;
+  const double bin_coef = (max_grad > 0) ? (double)(kBins - 1) / max_grad : 0.0;
+  const int nrow = (P.sh - 1) * P.sw;                 // the last row is never defined
+  const int c1 = min((r + 1) * Q, nrow);
+  const int u0 = min(r * Q + wid * U, c1), u1 = min(u0 + U, c1);
+  const int* SS = S2 + (long long)f * P.npx;
+  __syncthreads();
+  // 1. histogram of this warp's piece (4 loads in flight per lane)
+  unsigned* cw = reinterpret_cast<unsigned*>(cnt + wid * kBins);
+  for (int i0 = u0; i0 < u1; i0 += 128) {
+    int sv[4];
+#pragma unroll
+    for (int k = 0; k < 4; k++) { const int i = i0 + 32 * k + lane; sv[k] = i < u1 ? SS[i] : 0; }
+#pragma unroll
+    for (int k = 0; k < 4; k++) {
+      const int b = seed_bin(sv[k], P.s_th, bin_coef);
+      if (b >= 0) atomicAdd(&cw[b >> 1], 1u << ((b & 1) * 16));
+    }
+  }
+  __syncthreads();
+  // 2. thread t <-> bin kBins-1-t: exclusive offsets over the warps, CTA totals, then the cluster-wide bases
+  const int bin = kBins - 1 - tid;
+  {
+    int run = 0;
+    for (int w = 0; w < kSeedWarps; w++) { unsigned short& c = cnt[w * kBins + bin]; const int v = c; c = (unsigned short)run; run += v; }
+    tot[bin] = run;
+  }
+  cluster.sync();
+  int pre = 0, all = 0;
+#pragma unroll
+  for (int q = 0; q < kSeedCta; q++) {
+    const int v = cluster.map_shared_rank(tot, q)[bin];
+    all += v;
+    if (q < r) pre += v;
+  }
+  int incl = all;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) { const int v = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += v; }
+  if (lane == 31) wsum[wid] = incl;
+  __syncthreads();
+  if (wid == 0) {
+    const int v = wsum[lane];
+    int in2 = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) { const int u = __shfl_up_sync(0xffffffffu, in2, o); if (lane >= o) in2 += u; }
+    wsum[lane] = in2 - v;
+    if (lane == 31) { s_nd = in2; if (r == 0) ndef[f] = in2; }
+  }
+  __syncthreads();
+  base[bin] = wsum[wid] + incl - all + pre;
+  __syncthreads();
+  // 3. stable scatter of this warp's piece into the owners' shared memory
+  unsigned short* wc = cnt + wid * kBins;
+  const unsigned lt = (1u << lane) - 1u;
+  int y = (u0 + lane) / P.sw, x = (u0 + lane) - y * P.sw;      // sw > 32: one wrap at most per 32 pixels
+  for (int i0 = u0; i0 < u1; i0 += 128) {
+    int sv[4];
+#pragma unroll
+    for (int k = 0; k < 4; k++) { const int i = i0 + 32 * k + lane; sv[k] = i < u1 ? SS[i] : 0; }
+#pragma unroll
+    for (int k = 0; k < 4; k++) {
+      const int b = seed_bin(sv[k], P.s_th, bin_coef);
+      const unsigned peers = __match_any_sync(0xffffffffu, b);
+      if (b >= 0) {
+        const int pos = base[b] + wc[b] + __popc(peers & lt);
+        const int q = pos / S;
+        cluster.map_shared_rank(slice, q)[pos - q * S] = (unsigned)(x | (y << 16));
+      }
+      __syncwarp();
+      if (b >= 0 && (peers & lt) == 0) wc[b] += (unsigned short)__popc(peers);
+      __syncwarp();
+      x += 32;
+      if (x >= P.sw) { x -= P.sw; y++; }
+    }
+  }
+  cluster.sync();
+  // 4. flush [r*S, min((r+1)*S, ndef)) to HBM: scalar head up to 16-byte alignment, 16-byte body, scalar tail
+  const int n = min(S, s_nd - r * S);
+  if (n <= 0) return;
+  unsigned* g = order + (long long)f * P.npx + (long long)r * S;
+  const int head = min(n, (int)((4u - (unsigned)((reinterpret_cast<uintptr_t>(g) >> 2) & 3u)) & 3u));
+  if (tid < head) g[tid] = slice[tid];
+  const int nv = (n - head) >> 2;
+  uint4* g4 = reinterpret_cast<uint4*>(g + head);
+  if (head == 0) {
+    const uint4* s4 = reinterpret_cast<const uint4*>(slice);
+    for (int k = tid; k < nv; k += kSeedWarps * 32) g4[k] = s4[k];
+  } else {
+    for (int k = tid; k < nv; k += kSeedWarps * 32) {
+      const unsigned* s = slice + head + 4 * k;
+      g4[k] = make_uint4(s[0], s[1], s[2], s[3]);
+    }
+  }
+  for (int k = head + 4 * nv + tid; k < n; k += kSeedWarps * 32) g[k] = slice[k];
 }
 
 // ---------------------------------------------------------------------------------------------- K_F region growing
@@ -861,7 +992,13 @@ struct PLLine {
   int4* d_rec = nullptr; int* d_sq = nullptr;
   unsigned *d_st = nullptr, *d_pool = nullptr, *d_lanebuf = nullptr; int* d_ctl = nullptr; double* d_wtab = nullptr;
   GradRec* d_gtab = nullptr; float2* d_gtab_seed = nullptr;   // (gx, gy) -> level-line record, built once (k_lsd_grad_table)
-  unsigned short* d_counts = nullptr;
+  // k_lsd_seed_order: pixels per CTA (Q) and per warp (U), order positions per CTA (S), dynamic shared memory, clusters
+  // resident on the device (0: the frame does not fit the cluster, k_lsd_hist/scan/scatter sort it)
+  int seed_q = 0, seed_u = 0, seed_s = 0, seed_clusters = 0;
+  int seed_min_batch = 132 * kSerialFramesPerSM;   // default: the cluster sort from this batch on
+  int last_seed_cluster = 0;            // the LAST call sorted with k_lsd_seed_order
+  size_t seed_smem = 0;
+  unsigned short* d_counts = nullptr;   // k_lsd_hist/scan/scatter
   int *d_offsets = nullptr, *d_ndef = nullptr, *d_maxs = nullptr, *d_nseg = nullptr, *d_overflow = nullptr;
   unsigned* d_order = nullptr;
   float4* d_segs = nullptr;
@@ -933,6 +1070,7 @@ extern "C" int pl_line_create(const PLLineConfig* cfg, PLLine** out) {
     int dev = 0, sms = 132;
     cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     h->grow_warps_target = sms * 16;
+    h->seed_min_batch = sms * kSerialFramesPerSM;
     if (const char* e = getenv("PLSLAM_LSD_GROW_WARPS")) { const int v = atoi(e); if (v > 0) h->grow_warps_target = v; }
     if (const char* e = getenv("PLSLAM_LSD_GROW_WPF")) { const int v = atoi(e); if (v > 0) h->grow_wpf_max = v; }
     if (const char* e = getenv("PLSLAM_LSD_GROW_SPEC_MAXB")) h->grow_spec_max_batch = atoi(e);
@@ -971,6 +1109,23 @@ extern "C" int pl_line_create(const PLLineConfig* cfg, PLLine** out) {
     LN_CUDA(cudaMemcpyToSymbol(c_comb, h_comb, sizeof(h_comb)));
   }
   LN_CUDA(cudaFuncSetAttribute(k_keylines, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->key_smem));
+  {  // seed order on chip: 8 CTAs share the frame's rows 0..sh-2 and its (sw-1)(sh-1) possible order positions
+    const int nrow = (P.sh - 1) * P.sw, maxdef = (P.sw - 1) * (P.sh - 1);
+    h->seed_q = (nrow + kSeedCta - 1) / kSeedCta;
+    h->seed_u = ((h->seed_q + kSeedWarps - 1) / kSeedWarps + 31) & ~31;
+    h->seed_s = ((maxdef + kSeedCta - 1) / kSeedCta + 3) & ~3;
+    h->seed_smem = (size_t)h->seed_s * sizeof(unsigned) + (size_t)kSeedWarps * kBins * sizeof(unsigned short) + 2 * kBins * sizeof(int);
+    int dev = 0, smem_max = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&smem_max, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
+    // 16-bit per-warp counters hold within-CTA offsets: at most 65535 pixels per CTA
+    if (h->seed_q <= 65535 && h->seed_smem + 2 * 1024 <= (size_t)smem_max) {
+      LN_CUDA(cudaFuncSetAttribute(k_lsd_seed_order, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->seed_smem));
+      cudaLaunchConfig_t lc = {};
+      lc.gridDim = dim3(kSeedCta, 1, 1); lc.blockDim = dim3(kSeedWarps * 32, 1, 1); lc.dynamicSmemBytes = h->seed_smem;
+      LN_CUDA(cudaOccupancyMaxActiveClusters(&h->seed_clusters, (void*)k_lsd_seed_order, &lc));
+    }
+  }
   // cfg->lsd_used_in_global is accepted for ABI compatibility and ignored: the USED state is the ownership word of the pixel record
   *out = h;
   return PL_OK;
@@ -999,9 +1154,23 @@ extern "C" int pl_line_extract_batch_dev(PLLine* h, const uint8_t* imgs, int str
                                          const uint8_t* mask, void* keylines, uint8_t* desc, double* linefunc, int* n,
                                          void* stream_) {
   PL_ARG(h && imgs && keylines && desc && linefunc && n && B >= 1 && B <= h->cfg.max_batch && stride >= h->cfg.width);
+  // The cluster sort by default from kSerialFramesPerSM frames per SM on, where the three-kernel scatter is slow and the
+  // front-end runs its chains on one stream (frontend.cu, serial_batch).  Below that, kernels of the other chains hold SMs
+  // beside it and an 8-SM cluster with up to 217 KB of shared memory per CTA waits for whole SMs to drain (KITTI
+  // configuration: 21 % slower, DESIGN.md §7).  PLSLAM_LSD_SEED_ORDER=legacy | cluster forces one of the two; a forced
+  // cluster sort the frame shape or the device cannot run is an error.
+  const char* so = getenv("PLSLAM_LSD_SEED_ORDER");
+  const bool force_cluster = so && strcmp(so, "cluster") == 0, force_legacy = so && strcmp(so, "legacy") == 0;
+  if (force_cluster && h->seed_clusters == 0) {
+    set_error("PLSLAM_LSD_SEED_ORDER=cluster: a %dx%d scaled frame does not fit k_lsd_seed_order (%zu B of shared memory, %d pixels per CTA)",
+              h->P.sw, h->P.sh, h->seed_smem, h->seed_q);
+    return PL_ERR_ARG;
+  }
+  const bool cluster = h->seed_clusters > 0 && !force_legacy && (force_cluster || B >= h->seed_min_batch);
   cudaStream_t st = stream_ ? (cudaStream_t)stream_ : h->stream;
   const LineParams& P = h->P;
   h->last_B = B;
+  h->last_seed_cluster = cluster;
   PL_CUDA(cudaMemsetAsync(h->d_maxs, 0, sizeof(int) * B, st));
   k_lsd_scale<<<dim3((P.sw + 31) / 32, (P.sh + 31) / 32, B), 256, 0, st>>>(P, imgs, stride, (long long)frame_stride, h->d_scaled);
   PL_LAUNCH_CHECK();
@@ -1013,12 +1182,18 @@ extern "C" int pl_line_extract_batch_dev(PLLine* h, const uint8_t* imgs, int str
       k_lsd_grad<false><<<grd, 256, 0, st>>>(P, h->d_scaled, reinterpret_cast<const float4*>(h->d_gtab), h->d_gtab_seed, h->d_rec, h->d_sq, h->d_seedcs, h->d_maxs);
   }
   PL_LAUNCH_CHECK();
-  k_lsd_hist<<<dim3(P.nchunk, B), 256, 0, st>>>(P, h->d_sq, h->d_maxs, h->d_counts);
-  PL_LAUNCH_CHECK();
-  k_lsd_scan<<<B, kBins, 0, st>>>(P, h->d_counts, h->d_offsets, h->d_ndef);
-  PL_LAUNCH_CHECK();
-  k_lsd_scatter<<<dim3((P.nchunk + 3) / 4, B), 128, 0, st>>>(P, h->d_sq, h->d_maxs, h->d_offsets, h->d_order);
-  PL_LAUNCH_CHECK();
+  if (cluster) {
+    k_lsd_seed_order<<<dim3(kSeedCta, B), kSeedWarps * 32, h->seed_smem, st>>>(P, h->seed_q, h->seed_u, h->seed_s, h->d_sq, h->d_maxs,
+                                                                             h->d_order, h->d_ndef);
+    PL_LAUNCH_CHECK();
+  } else {
+    k_lsd_hist<<<dim3(P.nchunk, B), 256, 0, st>>>(P, h->d_sq, h->d_maxs, h->d_counts);
+    PL_LAUNCH_CHECK();
+    k_lsd_scan<<<B, kBins, 0, st>>>(P, h->d_counts, h->d_offsets, h->d_ndef);
+    PL_LAUNCH_CHECK();
+    k_lsd_scatter<<<dim3((P.nchunk + 3) / 4, B), 128, 0, st>>>(P, h->d_sq, h->d_maxs, h->d_offsets, h->d_order);
+    PL_LAUNCH_CHECK();
+  }
   if (B <= h->grow_spec_max_batch) {
     // few frames: many regions of each frame in flight (ordered speculative execution, lsd_grow_core.cuh)
     PL_CUDA(cudaMemsetAsync(h->d_st, 0, sizeof(unsigned) * (size_t)P.npx * B, st));
@@ -1145,11 +1320,27 @@ extern "C" int pl_line_debug_ctl(PLLine* h, int frame, int* out, int nwords) {
   PL_CUDA(cudaMemcpy(out, h->d_ctl + (size_t)frame * lg::kCtlStride, sizeof(int) * nwords, cudaMemcpyDeviceToHost));
   return PL_OK;
 }
+// which sort built the seed order of the LAST call: 1 k_lsd_seed_order, 0 k_lsd_hist/scan/scatter
+extern "C" int pl_line_debug_seed_path(PLLine* h) {
+  PL_ARG(h);
+  return h->last_seed_cluster;
+}
+// fill every byte of the seed order and of ndef with `byte` (a test writes 0xff before a call: every position the call does
+// not write then reads back as an invalid entry, and an unwritten ndef as -1)
+extern "C" int pl_line_debug_fill_order(PLLine* h, int byte) {
+  PL_ARG(h);
+  PL_CUDA(cudaStreamSynchronize(h->stream));
+  PL_CUDA(cudaMemset(h->d_order, byte, sizeof(unsigned) * (size_t)h->P.npx * h->cfg.max_batch));
+  PL_CUDA(cudaMemset(h->d_ndef, byte, sizeof(int) * (size_t)h->cfg.max_batch));
+  PL_CUDA(cudaDeviceSynchronize());
+  return PL_OK;
+}
 extern "C" int pl_line_debug_order(PLLine* h, int frame, unsigned* out, int cap) {
   PL_ARG(h && frame >= 0 && frame < h->last_B);
   int n = 0;
   PL_CUDA(cudaStreamSynchronize(h->stream));
   PL_CUDA(cudaMemcpy(&n, h->d_ndef + frame, sizeof(int), cudaMemcpyDeviceToHost));
+  if (n < 0) { set_error("seed order of frame %d: ndef = %d was not written by the last call", frame, n); return PL_ERR_ARG; }
   if (out && n) {
     PL_CUDA(cudaMemcpy(out, h->d_order + (size_t)frame * h->P.npx, sizeof(unsigned) * std::min(n, cap), cudaMemcpyDeviceToHost));
     for (int i = 0; i < std::min(n, cap); i++) out[i] = (out[i] >> 16) * (unsigned)h->P.sw + (out[i] & 0xffffu);   // packed (x,y) -> y*sw+x
