@@ -185,7 +185,7 @@ int pl_line_extract_batch_dev(PLLine* h, const uint8_t* imgs, int stride, size_t
                               const uint8_t* mask, void* keylines, uint8_t* desc, double* linefunc, int* n, void* stream);
 /* parity taps of the LAST call: raw LSD segments (x1,y1,x2,y2 floats, detection order), the 0.8x scaled image,
  * the LBD Sobel pair, and the seed order (pixel indices y*sw+x of the scaled image). */
-/* Capacity flags since the last check (segment_cap exceeded / region growing gave a frame up): PL_ERR_CAPACITY or PL_OK;
+/* Capacity flag since the last check (segment_cap exceeded): PL_ERR_CAPACITY or PL_OK;
  * clears them.  For callers of pl_line_extract_batch_dev, after synchronising their stream. */
 int pl_line_check_overflow(PLLine* h);
 int pl_line_debug_segments(PLLine* h, int frame, float* out, int cap);
@@ -196,8 +196,6 @@ int pl_line_debug_order(PLLine* h, int frame, unsigned* out, int cap);
 int pl_line_debug_seed_path(PLLine* h);
 /* fill every byte of the seed order and of its lengths with `byte` (tests: a later call must rewrite all it reports) */
 int pl_line_debug_fill_order(PLLine* h, int byte);
-/* control words of the speculative region growing for one frame of the LAST call (counters; post-mortem of the watchdog) */
-int pl_line_debug_ctl(PLLine* h, int frame, int* out, int nwords);
 
 /* ------------------------------------------------------------------ per-frame front-end pipeline (batch of frames)
  * The hot-path calls Tracking makes for one frame (SURVEY.md §3.1), chained on one stream with all intermediates in
@@ -284,7 +282,7 @@ int pl_save_keyframe_trajectory_mono_kitti(const char* filename, const float* po
  * "PLSB200\x01", int32 B, then per field {int32 len, name, int32 len, numpy dtype text, int32 ndim, int64 shape[], bytes}. */
 int pl_frontend_dump(PLFrontend* h, int B, const char* path);
 
-/* measurement hooks (bench.py): CUDA-event timing of k_lsd_grow on its launching stream, its algorithmic bytes, and
+/* measurement hooks (bench.py): CUDA-event timing of k_lsd_grow_ordered on its launching stream, its algorithmic bytes, and
  * a device copy of the second-call poses [B][16] for the multi-GPU all-gather */
 int pl_line_set_timing(PLLine* h, int on);
 int pl_line_grow_ms(PLLine* h, float* ms);

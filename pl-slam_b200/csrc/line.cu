@@ -12,9 +12,9 @@
 //                   equal bins keep row-major order == OpenCV 4.13's seed order (pinned in the oracle tests); one
 //                   8-CTA cluster per frame, the order assembled in distributed shared memory.  k_lsd_hist/scan/scatter:
 //                   the same sort through HBM (below 32 frames per SM, and frames too large for the cluster)
-//   k_lsd_grow      region growing + rectangle fit + density refinement; inherently ordered (a pixel consumed by an
-//                   earlier seed is unavailable to later ones) -> ONE warp per frame walks the seeds in order; the 32
-//                   lanes test the 3x3 neighbourhood, evaluate angles and reduce the rectangle moments in parallel.
+//   k_lsd_grow_ordered  region growing + rectangle fit + density refinement (lsd_grow_ordered.cuh); inherently ordered (a
+//                   pixel consumed by an earlier seed is unavailable to later ones) -> ONE warp per frame walks the seeds in
+//                   order; the 32 lanes test the 3x3 neighbourhood, evaluate angles and reduce the rectangle moments in parallel.
 //   k_keylines      KeyLine records, mask filter, response sort (bitonic, ties keep detection order), truncation
 //                   quirk of LineExtractor.cpp:44-67, normalised 2-D line equations
 //   k_lbd_sobel     5x5 sigma 1 Gaussian (8.8 fixed point) fused with the 3x3 Sobel pair -> int16 dx, dy
@@ -22,7 +22,6 @@
 //                   reference's order, fp32 without FMA), band statistics, 72-float LBD, 32-byte binarisation
 
 #include "common.cuh"
-#include "lsd_grow_core.cuh"
 #include "libm_glibc.cuh"
 #include <cooperative_groups.h>
 #include <math.h>
@@ -55,12 +54,15 @@ struct LineParams {
   int min_reg_size;
   int seg_cap, capL, nfeatures;
   double min_line_length;
-  double prec, prec_hi, p, density_th;   // prec_hi: see region_grow_t
+  double prec, prec_hi, p, density_th;   // prec_hi: see region_grow (lsd_grow_ordered.cuh)
   float sure_ca2, sure_cn2;              // cos^2(prec -/+ 0.05 deg): lsd_grow_ordered.cuh Sure
 };
 
 // ---------------------------------------------------------------------------------------------- shared helpers
-__device__ __forceinline__ float fast_atan2_deg_l(float y, float x) {  // cv::fastAtan2, no FMA
+// ownership word of a pixel record (REC .x): free, or gradient undefined (never available); region growing marks USED with 0
+constexpr int kFree = 0x7fffffff;
+constexpr int kNotDef = -1;
+__device__ __forceinline__ float fast_atan2_deg(float y, float x) {  // cv::fastAtan2 (degrees), no FMA
   const float k = (float)(180.0 / 3.14159265358979323846);
   const float p1 = 0.9997878412794807f * k, p3 = -0.3258083974640975f * k;
   const float p5 = 0.1555786518463281f * k, p7 = -0.04432655554792128f * k;
@@ -74,16 +76,14 @@ __device__ __forceinline__ float fast_atan2_deg_l(float y, float x) {  // cv::fa
   if (y < 0) a = __fsub_rn(360.f, a);
   return a;
 }
-__device__ __forceinline__ double warp_max_d(double v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = fmax(v, __shfl_xor_sync(0xffffffffu, v, o));
-  return v;
+__device__ __forceinline__ double angle_diff_signed(double a, double b) {
+  double diff = a - b;
+  while (diff <= -kPI) diff += 2 * kPI;
+  while (diff > kPI) diff -= 2 * kPI;
+  return diff;
 }
-__device__ __forceinline__ double warp_min_d(double v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = fmin(v, __shfl_xor_sync(0xffffffffu, v, o));
-  return v;
-}
+__device__ __forceinline__ double dist_d(double x1, double y1, double x2, double y2) { return sqrt((x2 - x1) * (x2 - x1) + (y2 - y1) * (y2 - y1)); }
+__device__ __forceinline__ double dist_sq(double x1, double y1, double x2, double y2) { return (x2 - x1) * (x2 - x1) + (y2 - y1) * (y2 - y1); }
 
 // ---------------------------------------------------------------------------------------------- K_A scale
 // Output tile 32x32 of the 0.8x image <- 40x40 blurred pixels <- 44x44 raw pixels (taps at +-3 are zero).
@@ -133,8 +133,8 @@ __global__ void __launch_bounds__(256) k_lsd_scale(LineParams P, const uint8_t* 
 
 // ---------------------------------------------------------------------------------------------- K_B gradient
 // Per scaled pixel, what region growing needs:
-//   REC = 16-byte record {own, angle, cos, sin}: own = ownership word of the speculative growing (lsd_grow_core.cuh; free or
-//         NOTDEF here), angle = level-line angle in degrees (cv::fastAtan2(gx, -gy)), cos/sin of float(angle_rad) rounded
+//   REC = 16-byte record {own, angle, cos, sin}: own = ownership word of the region growing (kFree or kNotDef here),
+//         angle = level-line angle in degrees (cv::fastAtan2(gx, -gy)), cos/sin of float(angle_rad) rounded
 //         to fp32 (what region_grow adds to sumdx/sumdy) -> ONE 16-byte load per neighbour in the growing step
 //   S2  = s = gx^2+gy^2 (a pixel is defined iff s > s_th; modgrad = sqrt(s/4) comes from a table); seedcs: see grad_record
 constexpr float kNotDefDeg = -1024.f;
@@ -145,7 +145,7 @@ constexpr float kNotDefDeg = -1024.f;
 constexpr int kGradR = 510, kGradN = 2 * kGradR + 1;
 struct GradRec { float deg, c, s, pad; };
 __device__ __forceinline__ void grad_record(int gx, int gy, GradRec& rec, float2& scs) {
-  const float deg = fast_atan2_deg_l((float)gx, (float)(-gy));
+  const float deg = fast_atan2_deg((float)gx, (float)(-gy));
   const double af = (double)(float)((double)deg * kDegToRads);
   double sn, cs;
   sincos(af, &sn, &cs);
@@ -197,7 +197,7 @@ __global__ void __launch_bounds__(256) k_lsd_grad(LineParams P, const uint8_t* _
     int sq[4];
 #pragma unroll
     for (int k = 0; k < 4; k++) {
-      rec[k] = make_int4(lg::kNotDef, __float_as_int(kNotDefDeg), 0, 0); se[k][0] = se[k][1] = 0.f; sq[k] = 0;
+      rec[k] = make_int4(kNotDef, __float_as_int(kNotDefDeg), 0, 0); se[k][0] = se[k][1] = 0.f; sq[k] = 0;
       if (x0 + k < P.sw - 1 && !lastrow) {
         const int DA = r1[k + 1] - r0[k], BC = r0[k + 1] - r1[k];
         const int gx = DA + BC, gy = DA - BC;
@@ -207,7 +207,7 @@ __global__ void __launch_bounds__(256) k_lsd_grad(LineParams P, const uint8_t* _
           const int ti = (gx + kGradR) * kGradN + (gy + kGradR);
           const float4 t = __ldg(&T[ti]);
           const float2 scs = __ldg(&TS[ti]);
-          rec[k] = make_int4(lg::kFree, __float_as_int(t.x), __float_as_int(t.y), __float_as_int(t.z));
+          rec[k] = make_int4(kFree, __float_as_int(t.x), __float_as_int(t.y), __float_as_int(t.z));
           se[k][0] = scs.x; se[k][1] = scs.y;
           smx = max(smx, s);
         }
@@ -442,257 +442,8 @@ k_lsd_seed_order(LineParams P, int Q, int U, int S, const int* __restrict__ S2, 
 }
 
 // ---------------------------------------------------------------------------------------------- K_F region growing
-// Ordered speculative execution (lsd_grow_core.cuh has the protocol and everything a lane does).  Here: the warp loop.
-//   frame f is served by `wpf` consecutive warps (one warp per CTA); every LANE runs one region task at a time, so a
-//   warp is 32 regions in flight and the instruction stream is shared by 32 independent serial chains
-//   per iteration (converged):   commit   the warp that holds the frame's commit lock validates the next 32 status
-//                                         words in order (two passes around a fence), appends the segments of the
-//                                         newly final tasks in order, advances the frontier, and hands an invalid
-//                                         head task out for re-execution
-//                                feed     idle lanes: take the re-execution, else scan the next 32 seeds of the
-//                                         order (coalesced), retire the consumed ones, queue the rest for the lanes
-//                                step     every busy lane advances its task by one micro-step (lane_step)
-// Why it is fast where the previous one-warp-per-region kernel was not: a region is a serial chain (one angle update
-// per added pixel), so 32 lanes on ONE region idle; 32 regions on one warp keep all lanes on useful work, and the
-// number of regions in flight (32 x warps) no longer depends on the batch: B = 1 fills the GPU as well as a full batch.
-constexpr int kGrowQ = 256;
-constexpr int kCommitBatches = 4;
-constexpr unsigned kGrowWatchdog = 6u * 1000u * 1000u;
-__device__ __forceinline__ int first_zero(unsigned m) { return m == 0xffffffffu ? 32 : __ffs(~m) - 1; }
-
-__device__ __forceinline__ void warp_commit(const lg::Params& GP, const lg::Frame& Fm, float4* __restrict__ segs, int lane) {
-  using namespace lg;
-  const unsigned lt = (1u << lane) - 1u;
-  for (int round = 0; round < kCommitBatches; round++) {
-    const int F = ld_i(&Fm.ctl[C_FIN]);
-    if (F >= Fm.n) return;
-    const int i = F + lane;
-    const unsigned w1 = (i < Fm.n) ? ld_u(&Fm.st[i]) : 0u;
-    const unsigned s1 = w1 & ST_STATE;
-    const int pre1 = first_zero(__ballot_sync(0xffffffffu, s1 == ST_NOOP || s1 == ST_EATEN || s1 == ST_DONE));
-    if (pre1 == 0) return;
-    __threadfence();            // every claim / steal of the tasks seen DONE is visible to the second pass
-    unsigned w2 = 0u;
-    bool ok = false;
-    if (lane < pre1) { w2 = ld_u(&Fm.st[i]); ok = task_valid(GP, Fm, i, w2); }
-    const int pre2 = min(pre1, first_zero(__ballot_sync(0xffffffffu, ok)));
-    float4 sg;
-    const bool has = (lane < pre2) && task_has_segment(Fm, w2, sg);
-    const unsigned ms = __ballot_sync(0xffffffffu, has);
-    const int ns = ld_i(&Fm.ctl[C_NS]);
-    if (has) { const int slot = ns + __popc(ms & lt); if (slot < GP.seg_cap) segs[slot] = sg; }
-    __syncwarp();
-    if (lane == 0) {
-      st_i(&Fm.ctl[C_NS], ns + __popc(ms));
-      __threadfence();
-      a_max(&Fm.ctl[C_FIN], F + pre2);
-    }
-    if (pre2 < pre1) {          // the head is finished but not valid: it is executed again, now with nothing earlier in flight
-      // (an idle lane may be taking the same task off the redo ring right now: the compare-and-swap decides)
-      // only a task that is still finished (DONE / EATEN) in the second pass: between the passes an idle lane may have taken
-      // it off the redo ring and be running it already
-      const unsigned s2 = w2 & ST_STATE;
-      if (lane == pre2 && (s2 == ST_DONE || s2 == ST_EATEN) &&
-          (unsigned)a_cas(reinterpret_cast<int*>(&Fm.st[i]), (int)w2, (int)((w2 & ~(ST_STATE | ST_ABORT)) | ST_REDO)) == w2) {
-        __threadfence();
-        st_i(&Fm.ctl[C_REDO], i);
-      }
-      __syncwarp();
-      return;
-    }
-    __syncwarp();
-    if (pre2 < 32) return;
-  }
-}
-
-template <int kWPC>
-__global__ void __launch_bounds__(32 * kWPC) k_lsd_grow(LineParams P, lg::Params GP, int4* __restrict__ REC, const float2* __restrict__ seedcs,
-                                                        const int* __restrict__ SQ, const unsigned* __restrict__ order, const int* __restrict__ ndef,
-                                                        unsigned* __restrict__ ST, unsigned* __restrict__ POOL, int* __restrict__ CTL,
-                                                        unsigned* __restrict__ LANEBUF, const double* __restrict__ wtab,
-                                                        float4* __restrict__ segs, int* __restrict__ nseg, int* __restrict__ overflow,
-                                                        int nframes, int wpf) {
-  using namespace lg;
-  __shared__ int wq_all[kWPC][kGrowQ];
-  __shared__ unsigned ring_all[kWPC][32 * lg::kRing];
-  const int lane = threadIdx.x & 31, wic = threadIdx.x >> 5;
-  const long long gw = (long long)blockIdx.x * kWPC + wic;
-  const int f = (int)(gw / wpf), wif = (int)(gw % wpf);      // frame, warp inside the frame's group
-  if (f >= nframes) return;
-  int* wq = wq_all[wic];
-  Frame Fm;
-  Fm.rec = REC + (long long)f * P.npx; Fm.seedcs = seedcs + (long long)f * P.npx; Fm.sq = SQ + (long long)f * P.npx;
-  Fm.order = order + (long long)f * P.npx; Fm.n = ndef[f];
-  Fm.st = ST + (long long)f * P.npx; Fm.pool = POOL + (long long)f * GP.pool_cap; Fm.ctl = CTL + (long long)f * kCtlStride; Fm.wtab = wtab;
-  float4* S = segs + (long long)f * P.seg_cap;
-  const bool solo = (wpf == 1);
-  if (!solo && wif == 0) {
-    // ---- the COMMITTER of the frame: nothing but the in-order validation, as fast as the status words arrive
-    for (unsigned iter = 0;; iter++) {
-      __syncwarp();
-      const int F = __shfl_sync(0xffffffffu, ld_i(&Fm.ctl[C_FIN]), 0);
-      if (F >= Fm.n) break;
-      if (iter > 4u * kGrowWatchdog) {
-        if (lane == 0) { a_or(reinterpret_cast<unsigned*>(&Fm.ctl[C_ERR]), (unsigned)ERR_WATCHDOG); a_max(&Fm.ctl[C_FIN], Fm.n); }
-        break;
-      }
-      warp_commit(GP, Fm, S, lane);
-      if (__shfl_sync(0xffffffffu, ld_i(&Fm.ctl[C_FIN]), 0) == F) __nanosleep(200);   // the head is still running
-    }
-    if (lane == 0) {
-      __threadfence();
-      const int ns = ld_i(&Fm.ctl[C_NS]), err = ld_i(&Fm.ctl[C_ERR]);
-      nseg[f] = min(ns, P.seg_cap);
-      if (ns > P.seg_cap) atomicOr(overflow, 1);
-      if (err) atomicOr(overflow, 2);
-    }
-    return;
-  }
-  Lane L;
-  L.home = LANEBUF + ((size_t)gw * 32 + lane) * (size_t)GP.lane_cap; L.home_cap = GP.lane_cap;
-  L.buf = L.home; L.cap = L.home_cap;
-  L.ring = ring_all[wic] + lane * lg::kRing;
-  L.phase = P_IDLE; L.task = -1; L.fresh = 1; L.off = 0; L.j = 0; L.m = 0;
-  lane_reset(L);
-  const unsigned lt = (1u << lane) - 1u;
-  int whead = 0, wcount = 0, rsc = 0;
-  bool exhausted = false;
-  unsigned iter_total = 0; unsigned long long busy_total = 0;
-  for (unsigned iter = 0;; iter++) {
-    __syncwarp();
-    iter_total = iter;
-    const int F = __shfl_sync(0xffffffffu, ld_i(&Fm.ctl[C_FIN]), 0);
-    if (F >= Fm.n) break;
-    if (iter > kGrowWatchdog) {          // cannot happen (the head task always completes); never hang the GPU on a bug
-      // post-mortem for pl_line_debug_ctl(): where the frontier stood, what the head looked like, what this warp held
-      int first = 0;
-      if (lane == 0 && a_cas(&Fm.ctl[C_STAT0 + 7 - 1], 0, F + 1) == 0 && false) {
-        first = 1;
-        Fm.ctl[C_STAT0 + 6] = (int)ld_u(&Fm.st[F]);
-        Fm.ctl[C_WORDS + 0] = 0x7777; Fm.ctl[C_WORDS + 1] = wif; Fm.ctl[C_WORDS + 2] = wcount; Fm.ctl[C_WORDS + 3] = (int)exhausted;
-        Fm.ctl[C_WORDS + 4] = ld_i(&Fm.ctl[C_NXT]); Fm.ctl[C_WORDS + 5] = ld_i(&Fm.ctl[C_REDO]); Fm.ctl[C_WORDS + 6] = ld_i(&Fm.ctl[C_LOCK]);
-        Fm.ctl[C_WORDS + 7] = Fm.n;
-      }
-      first = __shfl_sync(0xffffffffu, first, 0);
-      if (first) { Fm.ctl[C_WORDS + 8 + 2 * lane] = L.phase; Fm.ctl[C_WORDS + 9 + 2 * lane] = L.task; }
-      __syncwarp();
-      if (lane == 0) { a_or(reinterpret_cast<unsigned*>(&Fm.ctl[C_ERR]), (unsigned)ERR_WATCHDOG); a_max(&Fm.ctl[C_FIN], Fm.n); }
-      break;
-    }
-    // ---- commit (only when this warp is the whole group)
-    if (solo) warp_commit(GP, Fm, S, lane);
-    // ---- feed
-    unsigned mi = __ballot_sync(0xffffffffu, L.phase == P_IDLE);
-    // a warp that carries a long region is on the frame's critical path (the chain of long, refine-heavy regions is what
-    // a single frame waits for): it looks for new work only every 8th iteration, the other warps feed the idle lanes
-    const bool heavy = __any_sync(0xffffffffu, L.phase != P_IDLE && L.hi >= 64);
-    if (mi && (!heavy || (iter & 7u) == 0u)) {
-      // lane 0 looks at the three hand-over words at once: the re-execution slot of the committer and the redo ring
-      int redo = -1, rqh = 0, rqt = 0;
-      if (lane == 0) { redo = ld_i(&Fm.ctl[C_REDO]); rqh = ld_i(&Fm.ctl[C_RQH]); rqt = ld_i(&Fm.ctl[C_RQT]); if (redo >= 0) redo = a_exch(&Fm.ctl[C_REDO], -1); }
-      redo = __shfl_sync(0xffffffffu, redo, 0);
-      if (redo >= 0) {
-        const int k = __ffs(mi) - 1;
-        if (lane == k) lane_take_redo(Fm, L, redo);
-        mi &= mi - 1u;
-      }
-      // aborted tasks that are already published: re-execute them now rather than when they reach the head
-      int pending = __shfl_sync(0xffffffffu, rqt - rqh, 0);
-      for (int tries = 0; tries < 2 && mi && pending > 0; tries++, pending--) {
-        int m = -1;
-        if (lane == 0) {
-          const int hq = a_add(&Fm.ctl[C_RQH], 1);
-          m = a_exch(&Fm.ctl[C_WORDS + (hq & (kRedoQ - 1))], 0) - 1;
-          if (m >= 0) {
-            const unsigned w = ld_u(&Fm.st[m]);
-            if ((w & ST_STATE) != ST_DONE || !(w & ST_ABORT) ||
-                (unsigned)a_cas(reinterpret_cast<int*>(&Fm.st[m]), (int)w, (int)((w & ~(ST_STATE | ST_ABORT)) | ST_REDO)) != w) m = -1;
-          }
-        }
-        m = __shfl_sync(0xffffffffu, m, 0);
-        if (m >= 0) {
-          const int k = __ffs(mi) - 1;
-          if (lane == k) lane_take_redo(Fm, L, m);
-          mi &= mi - 1u;
-        }
-      }
-      // new seeds: 4 x 32 entries of the order per scan (one atomic, the loads of the four batches overlap)
-      if (__popc(mi) > wcount && !exhausted) {
-        int base = -1;
-        if (lane == 0 && !(GP.window > 0 && ld_i(&Fm.ctl[C_NXT]) - F >= GP.window)) base = a_add(&Fm.ctl[C_NXT], 128);
-        base = __shfl_sync(0xffffffffu, base, 0);
-        if (base >= Fm.n) exhausted = true;
-        else if (base >= 0) {
-          unsigned pix[4]; int own[4];
-#pragma unroll
-          for (int q = 0; q < 4; q++) { const int i = base + 32 * q + lane; pix[q] = (i < Fm.n) ? ldg_u(&Fm.order[i]) : 0u; }
-#pragma unroll
-          for (int q = 0; q < 4; q++) { const int i = base + 32 * q + lane; own[q] = (i < Fm.n) ? ld_i(&Fm.rec[(int)(pix[q] >> 16) * P.sw + (int)(pix[q] & 0xffffu)].x) : 0; }
-#pragma unroll
-          for (int q = 0; q < 4; q++) {
-            const int i = base + 32 * q + lane;
-            bool cand = false;
-            if (i < Fm.n) {
-              if (own_candidate(own[q], 2 * i, F)) cand = true;
-              else st_u(&Fm.st[i], (!(own[q] & 1) && (own[q] >> 1) < F) ? ST_NOOP : ST_EATEN);
-            }
-            const unsigned mc = __ballot_sync(0xffffffffu, cand);
-            if (cand) wq[(whead + wcount + __popc(mc & lt)) & (kGrowQ - 1)] = i;
-            wcount += __popc(mc);
-          }
-          __syncwarp();
-        }
-      }
-      // lanes still idle: look again at seeds found consumed by a task that was not final then (it may have let go)
-      if (__popc(mi) > wcount && wcount <= kGrowQ - 32) {
-        const int hi = min(__shfl_sync(0xffffffffu, ld_i(&Fm.ctl[C_NXT]), 0), Fm.n);
-        if (hi > F) {
-          if (rsc < F || rsc >= hi) rsc = F;
-          const int i = rsc + lane;
-          rsc += 32;
-          bool cand = false;
-          if (i < hi) {
-            const unsigned w = ld_u(&Fm.st[i]);
-            if ((w & ST_STATE) == ST_EATEN) {
-              const unsigned pix = ldg_u(&Fm.order[i]);
-              const int o = ld_i(&Fm.rec[(int)(pix >> 16) * P.sw + (int)(pix & 0xffffu)].x);
-              if (own_candidate(o, 2 * i, F)) cand = ((unsigned)a_cas(reinterpret_cast<int*>(&Fm.st[i]), (int)w, (int)ST_RUN) == w);
-              else if (!(o & 1) && (o >> 1) < F) st_u(&Fm.st[i], ST_NOOP);
-            }
-          }
-          const unsigned mc = __ballot_sync(0xffffffffu, cand);
-          if (cand) wq[(whead + wcount + __popc(mc & lt)) & (kGrowQ - 1)] = i;
-          wcount += __popc(mc);
-          __syncwarp();
-        }
-      }
-      const int r = __popc(mi & lt);
-      if (((mi >> lane) & 1u) && r < wcount) lane_take_seed(L, wq[(whead + r) & (kGrowQ - 1)]);
-      const int taken = min(__popc(mi), wcount);
-      whead += taken; wcount -= taken;
-    }
-    // ---- step
-    busy_total += __popc(__ballot_sync(0xffffffffu, L.phase != P_IDLE));
-    if (L.phase != P_IDLE) lane_step<false>(GP, Fm, L);
-  }
-  if (lane == 0) { a_max(&Fm.ctl[C_STAT0 + 5], (int)iter_total); a_add(&Fm.ctl[C_STAT0 + 6], (int)(busy_total >> 5)); }
-  // frame finished (or given up): in a one-warp group the worker reports
-  if (solo && lane == 0) {
-    __threadfence();
-    const int ns = ld_i(&Fm.ctl[C_NS]), err = ld_i(&Fm.ctl[C_ERR]);
-    nseg[f] = min(ns, P.seg_cap);
-    if (ns > P.seg_cap) atomicOr(overflow, 1);
-    if (err) atomicOr(overflow, 2);
-  }
-}
-// per-frame control words of the grow kernel (re-armed before every launch)
-__global__ void k_lsd_grow_init(int* __restrict__ CTL, int nframes) {
-  const int f = blockIdx.x * blockDim.x + threadIdx.x;
-  if (f >= nframes) return;
-  int* c = CTL + (long long)f * lg::kCtlStride;
-  for (int k = 0; k < lg::kCtlStride; k++) c[k] = 0;
-  c[lg::C_REDO] = -1; c[lg::C_POOL] = 1;
-}
+// k_lsd_grow_ordered (lsd_grow_ordered.cuh, included below); here the table of gradient magnitudes it weights the
+// rectangle moments with: W[s] = sqrt(s / 4), s = gx^2 + gy^2
 __global__ void k_lsd_wtab(double* __restrict__ W, int n) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) W[i] = sqrt((double)i / 4.0);
@@ -980,17 +731,10 @@ struct PLLine {
   cudaStream_t stream = nullptr;
   uint8_t* d_scaled = nullptr;
   float2* d_seedcs = nullptr;
-  // region growing (lsd_grow_core.cuh): pixel records, status words, list pool, control words, lane buffers, weight table
-  lg::Params GP;
-  int grow_warps_target = 132 * 16;   // warps the grow kernel spreads over the GPU when the batch is small (env PLSLAM_LSD_GROW_WARPS)
-  int grow_wpf_max = 64;              // at most this many warps on one frame (env PLSLAM_LSD_GROW_WPF)
-  // batches up to this size use the speculative kernel, larger ones the ordered one (env PLSLAM_LSD_GROW_SPEC_MAXB).  Default 0:
-  // the speculative kernel wins on frames made of many small regions (DESIGN.md §6)
-  // and loses on frames whose long, refine-heavy regions form a dependency chain
-  int grow_spec_max_batch = 0;
-  size_t lane_warps = 0;              // lane buffers are allocated for this many warps
+  // region growing (lsd_grow_ordered.cuh): pixel records, squared gradients, region lists, far-pixel masks, weight table
   int4* d_rec = nullptr; int* d_sq = nullptr;
-  unsigned *d_st = nullptr, *d_pool = nullptr, *d_lanebuf = nullptr; int* d_ctl = nullptr; double* d_wtab = nullptr;
+  unsigned *d_region = nullptr, *d_far = nullptr; double* d_wtab = nullptr;
+  int region_stride = 0;                // words of d_region per frame
   GradRec* d_gtab = nullptr; float2* d_gtab_seed = nullptr;   // (gx, gy) -> level-line record, built once (k_lsd_grad_table)
   // k_lsd_seed_order: pixels per CTA (Q) and per warp (U), order positions per CTA (S), dynamic shared memory, clusters
   // resident on the device (0: the frame does not fit the cluster, k_lsd_hist/scan/scatter sort it)
@@ -1018,7 +762,7 @@ static const unsigned char h_comb[64] = {0, 1, 0, 2, 0, 3, 0, 4, 0, 5, 0, 6, 1, 
 
 extern "C" void pl_line_destroy(PLLine* h) {
   if (!h) return;
-  cudaFree(h->d_gtab); cudaFree(h->d_gtab_seed); cudaFree(h->d_scaled); cudaFree(h->d_seedcs); cudaFree(h->d_rec); cudaFree(h->d_sq); cudaFree(h->d_st); cudaFree(h->d_pool); cudaFree(h->d_lanebuf); cudaFree(h->d_ctl); cudaFree(h->d_wtab); cudaFree(h->d_counts); cudaFree(h->d_offsets);
+  cudaFree(h->d_gtab); cudaFree(h->d_gtab_seed); cudaFree(h->d_scaled); cudaFree(h->d_seedcs); cudaFree(h->d_rec); cudaFree(h->d_sq); cudaFree(h->d_region); cudaFree(h->d_far); cudaFree(h->d_wtab); cudaFree(h->d_counts); cudaFree(h->d_offsets);
   cudaFree(h->d_ndef); cudaFree(h->d_maxs); cudaFree(h->d_nseg); cudaFree(h->d_overflow); cudaFree(h->d_order);
   cudaFree(h->d_segs); cudaFree(h->d_dxy); cudaFree(h->d_img); cudaFree(h->d_kls);
   cudaFree(h->d_desc); cudaFree(h->d_lf); cudaFree(h->d_nl); cudaFree(h->d_mask);
@@ -1066,22 +810,13 @@ extern "C" int pl_line_create(const PLLineConfig* cfg, PLLine** out) {
   LN_CUDA(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
   LN_TRY(dev_alloc(&h->d_scaled, npx * B)); LN_TRY(dev_alloc(&h->d_seedcs, npx * B)); LN_TRY(dev_alloc(&h->d_rec, npx * B));
   LN_TRY(dev_alloc(&h->d_sq, npx * B));
-  {  // speculative region growing: geometry of the run-time structures
+  {
     int dev = 0, sms = 132;
     cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    h->grow_warps_target = sms * 16;
     h->seed_min_batch = sms * kSerialFramesPerSM;
-    if (const char* e = getenv("PLSLAM_LSD_GROW_WARPS")) { const int v = atoi(e); if (v > 0) h->grow_warps_target = v; }
-    if (const char* e = getenv("PLSLAM_LSD_GROW_WPF")) { const int v = atoi(e); if (v > 0) h->grow_wpf_max = v; }
-    if (const char* e = getenv("PLSLAM_LSD_GROW_SPEC_MAXB")) h->grow_spec_max_batch = atoi(e);
-    lg::Params& G = h->GP;
-    G.sw = P.sw; G.sh = P.sh; G.npx = P.npx; G.min_reg_size = P.min_reg_size; G.seg_cap = P.seg_cap;
-    G.lane_cap = 1024; G.pool_cap = 4 * P.npx; G.window = 8192;
-    if (const char* e = getenv("PLSLAM_LSD_GROW_WINDOW")) G.window = atoi(e);
-    G.prec = P.prec; G.prec_hi = P.prec_hi; G.density_th = P.density_th;
-    h->lane_warps = std::max<size_t>(std::min<size_t>(B * (size_t)h->grow_wpf_max, (size_t)h->grow_warps_target), B);
-    LN_TRY(dev_alloc(&h->d_st, npx * B)); LN_TRY(dev_alloc(&h->d_pool, (size_t)G.pool_cap * B)); LN_TRY(dev_alloc(&h->d_ctl, (size_t)lg::kCtlStride * B));
-    LN_TRY(dev_alloc(&h->d_lanebuf, h->lane_warps * 32 * (size_t)G.lane_cap));
+    // a region holds at most npx pixels; reduce_round's swap-remove scratch follows it (fill_off = npx)
+    h->region_stride = 2 * P.npx;
+    LN_TRY(dev_alloc(&h->d_region, (size_t)h->region_stride * B)); LN_TRY(dev_alloc(&h->d_far, npx * B));
     const int nw = 2 * kGradR * kGradR + 1;
     LN_TRY(dev_alloc(&h->d_wtab, (size_t)nw));
     k_lsd_wtab<<<(nw + 255) / 256, 256, 0, h->stream>>>(h->d_wtab, nw);
@@ -1133,7 +868,7 @@ extern "C" int pl_line_create(const PLLineConfig* cfg, PLLine** out) {
 
 extern "C" int pl_line_capacity(const PLLine* h) { return h ? h->P.capL : PL_ERR_ARG; }
 
-// Device timing of k_lsd_grow (the dominant kernel): enable, run, then read the duration of the LAST launch.
+// Device timing of k_lsd_grow_ordered (the dominant kernel): enable, run, then read the duration of the LAST launch.
 extern "C" int pl_line_set_timing(PLLine* h, int on) {
   PL_ARG(h);
   if (on && !h->ev0) { PL_CUDA(cudaEventCreate(&h->ev0)); PL_CUDA(cudaEventCreate(&h->ev1)); }
@@ -1146,7 +881,7 @@ extern "C" int pl_line_grow_ms(PLLine* h, float* ms) {
   PL_CUDA(cudaEventElapsedTime(ms, h->ev0, h->ev1));
   return PL_OK;
 }
-/* algorithmic bytes k_lsd_grow must move for one frame (DESIGN.md §6): per scaled pixel: record (16) + seed cos/sin (8)
+/* algorithmic bytes k_lsd_grow_ordered must move for one frame (DESIGN.md §6): per scaled pixel: record (16) + seed cos/sin (8)
  * + seed order entry (4); the USED map lives in shared memory */
 extern "C" long long pl_line_grow_bytes_per_frame(const PLLine* h) { return h ? (long long)h->P.npx * 28 : 0; }
 
@@ -1194,38 +929,21 @@ extern "C" int pl_line_extract_batch_dev(PLLine* h, const uint8_t* imgs, int str
     k_lsd_scatter<<<dim3((P.nchunk + 3) / 4, B), 128, 0, st>>>(P, h->d_sq, h->d_maxs, h->d_offsets, h->d_order);
     PL_LAUNCH_CHECK();
   }
-  if (B <= h->grow_spec_max_batch) {
-    // few frames: many regions of each frame in flight (ordered speculative execution, lsd_grow_core.cuh)
-    PL_CUDA(cudaMemsetAsync(h->d_st, 0, sizeof(unsigned) * (size_t)P.npx * B, st));
-    k_lsd_grow_init<<<(B + 127) / 128, 128, 0, st>>>(h->d_ctl, B);
-    PL_LAUNCH_CHECK();
-    if (h->timing) PL_CUDA(cudaEventRecord(h->ev0, st));
-    // warps per frame (one of them is the frame's committer when there is more than one)
-    const int wpf = std::max(1, std::min(h->grow_wpf_max, h->grow_warps_target / B));
-    k_lsd_grow<1><<<B * wpf, 32, 0, st>>>(P, h->GP, h->d_rec, h->d_seedcs, h->d_sq, h->d_order, h->d_ndef, h->d_st, h->d_pool, h->d_ctl,
-                                          h->d_lanebuf, h->d_wtab, h->d_segs, h->d_nseg, h->d_overflow, B, wpf);
-    PL_LAUNCH_CHECK();
-  } else {
-    // many frames: one warp per frame, the 32 lanes on one region at a time (lsd_grow_ordered.cuh); the list pool and the
-    // status words of the speculative kernel serve as region list and far-pixel mask
-    if (h->timing) PL_CUDA(cudaEventRecord(h->ev0, st));
-    static const int pre_maxb = getenv("PLSLAM_LSD_PRE_MAXB") ? atoi(getenv("PLSLAM_LSD_PRE_MAXB")) : 256;
-    // the kernel addresses the per-frame arrays with 32-bit element indices (frame * npx + pixel): at most 2^32 / npx frames per grid
-    const int chunk = (int)std::min<long long>(B, 0xffffffffLL / P.npx);
-    for (int b0 = 0; b0 < B; b0 += chunk) {
-      const int nb = std::min(chunk, B - b0);
-      const size_t po = (size_t)b0 * P.npx;
-      if (B <= pre_maxb)
-        k_lsd_grow_ordered<true><<<nb, 32, 0, st>>>(P, h->d_rec + po, h->d_sq + po, h->d_seedcs + po, h->d_order + po, h->d_ndef + b0,
-                                                    h->d_pool + (size_t)b0 * h->GP.pool_cap, h->GP.pool_cap, h->d_st + po, h->d_wtab,
-                                                    h->d_segs + (size_t)b0 * P.seg_cap, h->d_nseg + b0, h->d_overflow, nb);
-      else
-        k_lsd_grow_ordered<false><<<nb, 32, 0, st>>>(P, h->d_rec + po, h->d_sq + po, h->d_seedcs + po, h->d_order + po, h->d_ndef + b0,
-                                                     h->d_pool + (size_t)b0 * h->GP.pool_cap, h->GP.pool_cap, h->d_st + po, h->d_wtab,
-                                                     h->d_segs + (size_t)b0 * P.seg_cap, h->d_nseg + b0, h->d_overflow, nb);
-    }
-    PL_LAUNCH_CHECK();
+  // one warp per frame, the 32 lanes on one region at a time (lsd_grow_ordered.cuh).  Batches up to kPreMaxBatch frames do
+  // not fill the GPU with frames: there the kernel examines the neighbourhoods of 32 seeds at a time up front (kPre)
+  constexpr int kPreMaxBatch = 256;
+  const auto grow = B <= kPreMaxBatch ? k_lsd_grow_ordered<true> : k_lsd_grow_ordered<false>;
+  if (h->timing) PL_CUDA(cudaEventRecord(h->ev0, st));
+  // the kernel addresses the per-frame arrays with 32-bit element indices (frame * npx + pixel): at most 2^32 / npx frames per grid
+  const int chunk = (int)std::min<long long>(B, 0xffffffffLL / P.npx);
+  for (int b0 = 0; b0 < B; b0 += chunk) {
+    const int nb = std::min(chunk, B - b0);
+    const size_t po = (size_t)b0 * P.npx;
+    grow<<<nb, 32, 0, st>>>(P, h->d_rec + po, h->d_sq + po, h->d_seedcs + po, h->d_order + po, h->d_ndef + b0,
+                            h->d_region + (size_t)b0 * h->region_stride, h->region_stride, h->d_far + po, h->d_wtab,
+                            h->d_segs + (size_t)b0 * P.seg_cap, h->d_nseg + b0, h->d_overflow, nb);
   }
+  PL_LAUNCH_CHECK();
   if (h->timing) PL_CUDA(cudaEventRecord(h->ev1, st));
   k_keylines<<<B, 256, h->key_smem, st>>>(P, h->d_segs, h->d_nseg, mask, (PLKeyLineRec*)keylines, linefunc, n);
   PL_LAUNCH_CHECK();
@@ -1236,7 +954,7 @@ extern "C" int pl_line_extract_batch_dev(PLLine* h, const uint8_t* imgs, int str
   return PL_OK;
 }
 
-// capacity flags of the calls since the last check (segment_cap exceeded, or the region growing gave a frame up);
+// capacity flag of the calls since the last check (segment_cap exceeded);
 // the *_dev entry points are asynchronous and never look at them: their callers do, after synchronising
 extern "C" int pl_line_check_overflow(PLLine* h) {
   PL_ARG(h);
@@ -1244,8 +962,7 @@ extern "C" int pl_line_check_overflow(PLLine* h) {
   PL_CUDA(cudaMemcpy(&ov, h->d_overflow, sizeof(int), cudaMemcpyDeviceToHost));
   if (ov) {
     cudaMemset(h->d_overflow, 0, sizeof(int));
-    if (ov & 1) set_error("LSD produced more than segment_cap=%d segments", h->P.seg_cap);
-    else set_error("LSD region growing gave a frame up (list pool of %d words exhausted, or watchdog): see pl_line_debug_ctl", h->GP.pool_cap);
+    set_error("LSD produced more than segment_cap=%d segments", h->P.seg_cap);
     return PL_ERR_CAPACITY;
   }
   return PL_OK;
@@ -1312,12 +1029,6 @@ extern "C" int pl_line_debug_sobel(PLLine* h, int frame, short* dx, short* dy) {
   std::vector<short2> tmp(n);
   PL_CUDA(cudaMemcpy(tmp.data(), h->d_dxy + frame * n, n * sizeof(short2), cudaMemcpyDeviceToHost));
   for (size_t i = 0; i < n; i++) { dx[i] = tmp[i].x; dy[i] = tmp[i].y; }
-  return PL_OK;
-}
-extern "C" int pl_line_debug_ctl(PLLine* h, int frame, int* out, int nwords) {
-  PL_ARG(h && out && frame >= 0 && frame < h->cfg.max_batch && nwords > 0 && nwords <= lg::kCtlStride);
-  PL_CUDA(cudaStreamSynchronize(h->stream));
-  PL_CUDA(cudaMemcpy(out, h->d_ctl + (size_t)frame * lg::kCtlStride, sizeof(int) * nwords, cudaMemcpyDeviceToHost));
   return PL_OK;
 }
 // which sort built the seed order of the LAST call: 1 k_lsd_seed_order, 0 k_lsd_hist/scan/scatter

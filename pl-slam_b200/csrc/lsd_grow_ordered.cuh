@@ -1,10 +1,9 @@
-// LSD region growing, ORDERED variant: one warp walks one frame's seeds in order, the 32 lanes cooperate on ONE region.
-// This is the throughput form for batches that fill the GPU with frames (B >= ~resident warps): no speculation, no
-// atomics, no status words.  For small batches k_lsd_grow (speculative, lsd_grow_core.cuh) puts many regions of one
-// frame in flight instead.  Both produce the oracle's segment list bit for bit.
+// LSD region growing (k_lsd_grow_ordered): one warp walks one frame's seeds in order, the 32 lanes cooperate on ONE region.
+// Produces the oracle's segment list bit for bit.  Included by line.cu only, after LineParams and the shared helpers
+// (kFree / kNotDef, kPI / kDegToRads, fast_atan2_deg, angle_diff_signed, dist_d, dist_sq).
 //
-// Same pixel records as the speculative kernel ({own, angle, cos, sin}, 16 bytes); here the ownership word only says
-// free (lg::kFree) / undefined (lg::kNotDef) / used (0), and is written with plain stores by the lane that owns the pixel.
+// Pixel records {own, angle, cos, sin}, 16 bytes (k_lsd_grad): the ownership word says free (kFree) / undefined (kNotDef) /
+// used (0), and is written with plain stores by the lane that owns the pixel.
 //
 // Exactness of the fp64 parts (what round 1 did not have): LineSegmentDetectorImpl::region2rect / get_theta / refine sum over
 // the region IN LIST ORDER on the CPU.  The lanes load and form the per-pixel terms in parallel (32 pixels per batch), then
@@ -14,19 +13,13 @@
 // hole / survivor matching (hole r below the final size <- r-th survivor of the tail, counted from the end: what the CPU's
 // swap-with-last loop leaves behind), computed with warp prefix sums over the mask words.
 #pragma once
-#include "lsd_grow_core.cuh"
 
 namespace pl {
 namespace ord {
 
-using lg::kDegToRads;
-using lg::kPI;
 // recent queue entries in shared memory; older ones are re-read from the region list in global memory (L1 hits).  The L1 share matters
 // more than the ring: a small ring leaves more of the SM's shared memory / L1 split to L1
-#ifndef PL_GROW_RING
-#define PL_GROW_RING 64
-#endif
-constexpr int kORing = PL_GROW_RING;
+constexpr int kORing = 64;
 constexpr int kUsedO = 0;
 
 // Per-frame arrays are addressed as  kernel-parameter base + 32-bit element index (fb = frame * npx + pixel): one IMAD.WIDE per
@@ -90,7 +83,7 @@ __device__ __noinline__ double wmin_d(double v) {
   for (int o = 16; o > 0; o >>= 1) v = fmin(v, __shfl_xor_sync(0xffffffffu, v, o));
   return v;
 }
-__device__ __noinline__ float fast_atan2_cold(float y, float x) { return lg::fast_atan2_deg(y, x); }
+__device__ __noinline__ float fast_atan2_cold(float y, float x) { return fast_atan2_deg(y, x); }
 __device__ __forceinline__ bool is_aligned_generic(double a, double theta, double prec) {
   const double n1 = fabs(theta - a);
   const double n2 = fabs(n1 - 2 * kPI);
@@ -102,7 +95,8 @@ __device__ __forceinline__ bool is_aligned_generic(double a, double theta, doubl
 // then the candidates are committed in the reference's order (queue order, then row-major inside the 3x3): every
 // remaining candidate is tested against the CURRENT region angle at once, the first aligned one is added, which changes
 // the angle; a pixel added earlier in the same step invalidates its duplicates in the later neighbourhoods.
-// kFast: prec < pi/2, isAligned folded to  n <= prec || n >= prec_hi  (see lsd_grow_core.cuh aligned()).
+// kFast: prec < pi/2, isAligned folded to  n <= prec || n >= prec_hi  (prec_hi = smallest double with 2pi - n <= prec; 2pi - n
+// is exact for n in [pi, 4pi], so both forms agree bit for bit).
 // Alignment WITHOUT the arctangent for the clear cases (kFast only).  The exact test compares the candidate's angle a with
 // reg_angle = fastAtan2(sumdy, sumdx); the candidate's record also carries (cos a, sin a), so the TRUE angle D between the sum
 // vector and the candidate is known from one dot product: cos D = (sumdx*c + sumdy*s) / |sum|.  fastAtan2's polynomial is within
@@ -140,7 +134,7 @@ __device__ __forceinline__ int region_grow(const Ctx& C, unsigned seed, double p
         idx = yy * C.sw + xx;
         GSTAT_ALL(kFast ? 16 : 17, 1);
         const int4 v = ld_rec(C, idx);
-        if (v.x == lg::kFree) {                       // defined and not USED
+        if (v.x == kFree) {                           // defined and not USED
           valid = true; ab = v.y;
           csv = make_float2(__int_as_float(v.z), __int_as_float(v.w));
           pk = (unsigned)xx | ((unsigned)yy << 16);
@@ -174,7 +168,7 @@ __device__ __forceinline__ int region_grow(const Ctx& C, unsigned seed, double p
       }
       if (exact) {
         GSTAT(5, 1);
-        if (dirty) { reg_angle = (double)lg::fast_atan2_deg(sumdy, sumdx) * kDegToRads; dirty = false; }
+        if (dirty) { reg_angle = (double)fast_atan2_deg(sumdy, sumdx) * kDegToRads; dirty = false; }
         const double a = (double)__int_as_float(ab) * kDegToRads;
         bool al;
         if (kFast) { const double n1 = fabs(reg_angle - a); al = (n1 <= prec) || (n1 >= prec_hi); }
@@ -201,7 +195,7 @@ __device__ __forceinline__ int region_grow(const Ctx& C, unsigned seed, double p
     __syncwarp();
   }
   // most regions end below need_n and their angle is never read
-  if (dirty && cnt >= need_n) reg_angle = (double)lg::fast_atan2_deg(sumdy, sumdx) * kDegToRads;
+  if (dirty && cnt >= need_n) reg_angle = (double)fast_atan2_deg(sumdy, sumdx) * kDegToRads;
   reg_angle_out = reg_angle;
   return cnt;
 }
@@ -256,7 +250,7 @@ __device__ __noinline__ void region2rect(const Ctx& C, int n, double reg_angle, 
   double theta = (fabs(Ixx) > fabs(Iyy)) ? (double)fast_atan2_cold((float)(lambda - Ixx), (float)Ixy)
                                          : (double)fast_atan2_cold((float)Ixy, (float)(lambda - Iyy));
   theta *= kDegToRads;
-  if (fabs(lg::angle_diff_signed(theta, reg_angle)) > prec) theta += kPI;
+  if (fabs(angle_diff_signed(theta, reg_angle)) > prec) theta += kPI;
   double dx, dy;
   sincos(theta, &dy, &dx);              // one range reduction; same results as cos() / sin() (CUDA's sincos is the pair of them)
   double l_min = 0, l_max = 0, w_min = 0, w_max = 0;
@@ -290,7 +284,7 @@ __device__ __noinline__ int reduce_round(const Ctx& C, int n, double xc, double 
       const unsigned p = C.R[i];
       const double px = (double)(int)(p & 0xffffu), py = (double)(int)(p >> 16);
       far = (px - xc) * (px - xc) + (py - yc) * (py - yc) > radSq;
-      if (far) own_of(C, (int)(p >> 16) * C.sw + (int)(p & 0xffffu)) = lg::kFree;
+      if (far) own_of(C, (int)(p >> 16) * C.sw + (int)(p & 0xffffu)) = kFree;
     }
     const unsigned mw = __ballot_sync(0xffffffffu, far);
     if (lane == 0) C.mask[C.fb + (unsigned)(i0 >> 5)] = mw;
@@ -352,7 +346,7 @@ __device__ __noinline__ int reduce_round(const Ctx& C, int n, double xc, double 
 
 // LineSegmentDetectorImpl::refine + reduce_region_radius; n is updated; returns false if the region is rejected
 __device__ __noinline__ bool refine(const Ctx& C, int& n, double reg_angle, double prec, RectD& rec, double density_th, int lane, bool& released) {
-  double density = (double)n / (lg::dist_d(rec.x1, rec.y1, rec.x2, rec.y2) * rec.width);
+  double density = (double)n / (dist_d(rec.x1, rec.y1, rec.x2, rec.y2) * rec.width);
   if (density >= density_th) return true;
   released = true;              // from here on USED flags are cleared
   GSTAT(7, 1);
@@ -369,11 +363,11 @@ __device__ __noinline__ bool refine(const Ctx& C, int& n, double reg_angle, doub
     if (i < n) {
       const unsigned p = C.R[i];
       const int pidx = (int)(p >> 16) * C.sw + (int)(p & 0xffffu);
-      own_of(C, pidx) = lg::kFree;
+      own_of(C, pidx) = kFree;
       const double px = (double)(int)(p & 0xffffu), py = (double)(int)(p >> 16);
-      if (lg::dist_d(xc, yc, px, py) < rec.width) {
+      if (dist_d(xc, yc, px, py) < rec.width) {
         in = true;
-        ad = lg::angle_diff_signed((double)__int_as_float(angle_bits(C, pidx)) * kDegToRads, ang_c);
+        ad = angle_diff_signed((double)__int_as_float(angle_bits(C, pidx)) * kDegToRads, ang_c);
         ad2 = ad * ad;
       }
     }
@@ -396,16 +390,16 @@ __device__ __noinline__ bool refine(const Ctx& C, int& n, double reg_angle, doub
   n = region_grow_cold(C, p0, tau, reg_angle, lane);
   if (n < 2) return false;
   region2rect(C, n, reg_angle, prec, rec, lane);
-  density = (double)n / (lg::dist_d(rec.x1, rec.y1, rec.x2, rec.y2) * rec.width);
+  density = (double)n / (dist_d(rec.x1, rec.y1, rec.x2, rec.y2) * rec.width);
   if (density >= density_th) return true;
-  const double r1 = lg::dist_sq(xc, yc, rec.x1, rec.y1), r2 = lg::dist_sq(xc, yc, rec.x2, rec.y2);
+  const double r1 = dist_sq(xc, yc, rec.x1, rec.y1), r2 = dist_sq(xc, yc, rec.x2, rec.y2);
   double radSq = r1 > r2 ? r1 : r2;
   while (density < density_th) {
     radSq *= 0.75 * 0.75;
     n = reduce_round(C, n, xc, yc, radSq, lane);
     if (n < 2) return false;
     region2rect(C, n, reg_angle, prec, rec, lane);
-    density = (double)n / (lg::dist_d(rec.x1, rec.y1, rec.x2, rec.y2) * rec.width);
+    density = (double)n / (dist_d(rec.x1, rec.y1, rec.x2, rec.y2) * rec.width);
   }
   return true;
 }
@@ -433,7 +427,7 @@ __global__ void __launch_bounds__(32, 32) k_lsd_grow_ordered(LineParams P, int4*
       const unsigned pix = (i < n) ? O[i] : 0u;
       const int pidx = (int)(pix >> 16) * P.sw + (int)(pix & 0xffffu);
       const int4 me = (i < n) ? ld_rec(C, pidx) : make_int4(0, 0, 0, 0);
-      unsigned todo = __ballot_sync(0xffffffffu, i < n && me.x == lg::kFree);
+      unsigned todo = __ballot_sync(0xffffffffu, i < n && me.x == kFree);
       // Seeds of this batch whose region cannot get past the seed itself: no FREE neighbour is aligned with the seed's own angle
       // (the region angle of the first step).  Between two regions the set of free pixels only shrinks (a region releases only
       // pixels it took itself), so "no free aligned neighbour now" still holds when the seed's turn comes: the region is the
@@ -443,28 +437,26 @@ __global__ void __launch_bounds__(32, 32) k_lsd_grow_ordered(LineParams P, int4*
       bool single = false;
       if (kPre && ((todo >> lane) & 1u)) {
         const int sx = (int)(pix & 0xffffu), sy = (int)(pix >> 16);
-        const double a0 = (double)__int_as_float(me.y) * lg::kDegToRads;
+        const double a0 = (double)__int_as_float(me.y) * kDegToRads;
         bool any = false;
 #pragma unroll
         for (int q = 0; q < 8; q++) {
           const int kq = q + (q >= 4), xx = sx + kq % 3 - 1, yy = sy + kq / 3 - 1;
           if (xx >= 0 && yy >= 0 && xx < P.sw && yy < P.sh) {
             const int4 v = ld_rec(C, yy * P.sw + xx);
-            const double n1 = fabs(a0 - (double)__int_as_float(v.y) * lg::kDegToRads);
-            any |= (v.x == lg::kFree) && ((n1 <= P.prec) || (n1 >= P.prec_hi));
+            const double n1 = fabs(a0 - (double)__int_as_float(v.y) * kDegToRads);
+            any |= (v.x == kFree) && ((n1 <= P.prec) || (n1 >= P.prec_hi));
           }
         }
         single = !any;
         prefetch_l2(&C.S2[C.fb + (unsigned)pidx]);
       }
-#ifndef PL_GROW_NOPF                          // (PL_GROW_NOPF builds without these prefetches, for A/B timing)
       if (!kPre && ((todo >> lane) & 1u)) {   // this batch's seeds that will grow: their seed record and 3x3 rows into L2
         prefetch_l2(&C.S2[C.fb + (unsigned)pidx]);
         const int up = max(pidx - P.sw, 1), dn = min(pidx + P.sw, P.npx - 2);
         prefetch_l2(&C.REC[C.fb + (unsigned)(up - 1)]); prefetch_l2(&C.REC[C.fb + (unsigned)(up + 1)]); prefetch_l2(&C.REC[C.fb + (unsigned)(dn - 1)]); prefetch_l2(&C.REC[C.fb + (unsigned)(dn + 1)]);
         prefetch_l2(&C.REC[C.fb + (unsigned)(max(pidx, 1) - 1)]); prefetch_l2(&C.REC[C.fb + (unsigned)(min(pidx, P.npx - 2) + 1)]);
       }
-#endif
       const unsigned singles = __ballot_sync(0xffffffffu, single);
       if (i + 32 < n) { const unsigned pn = O[i + 32]; prefetch_l2(&C.REC[C.fb + (unsigned)((int)(pn >> 16) * P.sw + (int)(pn & 0xffffu))]); }
       while (todo) {
@@ -499,7 +491,7 @@ __global__ void __launch_bounds__(32, 32) k_lsd_grow_ordered(LineParams P, int4*
         // seeds later in this batch may have been consumed (or released by refine): re-read their words - unless the region was
         // the seed alone (36 % of the regions), which touched no other pixel
         if (cnt == 1) todo &= ~((2u << k) - 1u);
-        else todo = __ballot_sync(0xffffffffu, i < n && lane > k && own_of(C, pidx) == lg::kFree);
+        else todo = __ballot_sync(0xffffffffu, i < n && lane > k && own_of(C, pidx) == kFree);
       }
     }
     if (lane == 0) { nseg[f] = min(ns, P.seg_cap); if (ns > P.seg_cap) atomicOr(overflow, 1); }

@@ -19,10 +19,8 @@ def _segments_equal(a, b):
     assert a.tobytes() == b.tobytes(), "segment lists differ: first row %d" % int(np.nonzero((a != b).any(1))[0][0])
 
 
-@pytest.mark.parametrize("spec_maxb", [0, 4])
 @pytest.mark.parametrize("w,h,seed", [(640, 480, 1), (640, 480, 2), (752, 480, 5), (1241, 376, 4)])
-def test_stages_match_oracle(monkeypatch, w, h, seed, spec_maxb):
-    monkeypatch.setenv("PLSLAM_LSD_GROW_SPEC_MAXB", str(spec_maxb))     # 0: ordered kernel, 4: speculative kernel
+def test_stages_match_oracle(w, h, seed):
     img = synth.synth_frame(w, h, seed)
     ex = pl.LINEextractor(1, 1.2, 200, 0.0, width=w, height=h)
     kl, desc, lf = ex(img)
@@ -134,27 +132,8 @@ def _last_segments():
     return ex.debug_segments()
 
 
-@pytest.mark.parametrize("warps,wpf", [(1, 1), (4, 4), (64, 64), (2368, 64), (2368, 256)])
-def test_grow_warps_per_frame_do_not_change_the_result(monkeypatch, warps, wpf):
-    """The speculative region growing must give the sequential result whatever the number of warps (= regions in flight)
-    serving a frame: 1 warp (32 tasks in flight) ... 256 warps (8192 tasks in flight, heavy stealing / re-execution)."""
-    monkeypatch.setenv("PLSLAM_LSD_GROW_SPEC_MAXB", "64")        # the speculative kernel (the default is the ordered one)
-    monkeypatch.setenv("PLSLAM_LSD_GROW_WARPS", str(warps))
-    monkeypatch.setenv("PLSLAM_LSD_GROW_WPF", str(wpf))
-    K, D = synth.TUM1_K, synth.TUM1_DIST
-    img = oracle.undistort_remap(synth.synth_sequence(2, 640, 480, seed=1)[1], K, D)
-    ex = pl.LINEextractor(1, 1.2, 200, 0.0)
-    for rep in range(3):                     # the interleaving differs from run to run; the result must not
-        kl, desc, lf = ex(img)
-        _segments_equal(ex.debug_segments(), oracle.lsd_detect(img))
-    okl, odesc, olf = oracle.line_extract(img)
-    assert kl.tobytes() == okl.tobytes() and np.array_equal(desc, odesc)
-
-
-@pytest.mark.parametrize("spec_maxb", [0, 64])
-def test_grow_batches_of_odd_sizes(monkeypatch, spec_maxb):
-    """Batches that do not divide the warp budget: 3 and 37 frames, each frame against the oracle (both growing kernels)."""
-    monkeypatch.setenv("PLSLAM_LSD_GROW_SPEC_MAXB", str(spec_maxb))
+def test_grow_batches_of_odd_sizes():
+    """Batches of odd sizes: 3 and 37 frames, each frame against the oracle."""
     seq = synth.synth_sequence(37, 640, 480, seed=5)
     ex = pl.LINEextractor(1, 1.2, 200, 0.0, max_batch=37)
     for B in (3, 37):
@@ -164,11 +143,8 @@ def test_grow_batches_of_odd_sizes(monkeypatch, spec_maxb):
             assert nb[b] == len(okl) and klb[b, :nb[b]].tobytes() == okl.tobytes() and np.array_equal(descb[b, :nb[b]], odesc), (B, b)
 
 
-@pytest.mark.parametrize("spec_maxb", [0, 4])
-def test_grow_degenerate_frames(monkeypatch, spec_maxb):
-    """No gradient at all, pure noise (thousands of tiny regions), one long edge across the frame (one huge region);
-    through both region-growing kernels (0: ordered one-warp-per-frame kernel, 4: speculative kernel for a single frame)."""
-    monkeypatch.setenv("PLSLAM_LSD_GROW_SPEC_MAXB", str(spec_maxb))
+def test_grow_degenerate_frames():
+    """No gradient at all, pure noise (thousands of tiny regions), one long edge across the frame (one huge region)."""
     rng = np.random.Generator(np.random.PCG64(11))
     flat = np.full((480, 640), 128, np.uint8)
     noise = rng.integers(0, 256, (480, 640), dtype=np.uint8)

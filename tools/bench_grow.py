@@ -1,5 +1,5 @@
 """A/B timing of the LSD region-growing kernel across builds of the library: python tools/bench_grow.py lib1.so lib2.so ...
-Prints per library the k_lsd_grow time of one launch over B frames (CUDA events inside the library) and a checksum of the
+Prints per library the k_lsd_grow_ordered time of one launch over B frames (CUDA events inside the library) and a checksum of the
 line outputs (must be identical across builds)."""
 import ctypes as C, os, sys, zlib
 import numpy as np, torch
