@@ -381,6 +381,11 @@ int pl_undistort_remap_batch_dev(PLUndistort* h, const uint8_t* src, int sstride
 /* Frame::UndistortKeyPoints: only pt.x / pt.y change; k1 == 0 copies */
 int pl_undistort_keypoints(PLUndistort* h, const PLKeyPoint* kps, int n, PLKeyPoint* out);
 int pl_undistort_keypoints_dev(PLUndistort* h, const PLKeyPoint* kps, const int* n, int cap, int B, PLKeyPoint* out, void* stream);
+/* Line extraction on raw frames: every later pl_line_extract* call reads each frame through this map (what
+ * pl_undistort_remap would have stored) instead of taking the frames as already undistorted.  NULL unbinds it.  The map
+ * must have the line handle's size (else PL_ERR_ARG) and the caller keeps it alive while it is bound.  Batches below 32
+ * frames per SM are undistorted into a buffer of the handle first (W x H x max_batch bytes, made on first use). */
+int pl_line_set_undistort(PLLine* h, const PLUndistort* und);
 /* Frame::ComputeImageBounds -> {mnMinX, mnMinY, mnMaxX, mnMaxY} */
 int pl_frame_image_bounds(const float* K, const float* dist5, int width, int height, float* bounds);
 /* Frame::isInFrustum(MapPoint*, viewingCosLimit) for n map points: pos = GetWorldPos, normal = GetNormal,

@@ -321,6 +321,8 @@ class LINEextractor:
         L.pl_line_debug_order.argtypes = [vp, C.c_int, vp, C.c_int]
         L.pl_line_debug_seed_path.argtypes = [vp]
         L.pl_line_debug_fill_order.argtypes = [vp, C.c_int]
+        L.pl_line_set_undistort.argtypes = [vp, vp]
+        self._und = None
         check(L.pl_line_create(C.byref(self.cfg), C.byref(self._h)))
         self.capacity = check(L.pl_line_capacity(self._h))
 
@@ -328,6 +330,12 @@ class LINEextractor:
         if getattr(self, "_h", None) and self._h.value:
             lib().pl_line_destroy(self._h)
             self._h = vp()
+
+    def set_undistort(self, undistorter):
+        """Take raw frames from now on and undistort them with `undistorter` (an Undistorter of the same size) inside the
+        extraction, as Frame.cc:220-225 does before it calls the extractor; None takes undistorted frames again."""
+        check(lib().pl_line_set_undistort(self._h, undistorter.handle if undistorter is not None else None))
+        self._und = undistorter     # the map must outlive its use by this handle
 
     def __call__(self, image, mask=None):
         image = np.ascontiguousarray(image, np.uint8)

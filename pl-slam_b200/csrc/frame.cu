@@ -8,12 +8,11 @@
 // BORDER_CONSTANT 0; fp32 3x3 gemm as ((a0*b0 + a1*b1) + a2*b2) + c; cv::norm / dot with fp64 accumulation.
 #include "common.cuh"
 #include "frustum.cuh"
+#include "remap.cuh"
 #include <math.h>
 #include <vector>
 
 namespace pl {
-struct RemapEntry { short ix, iy; unsigned short tab; unsigned short pad; };   // 8 B per output pixel, shared by all frames
-
 // 4 consecutive output pixels per thread (uchar4 store); the 2x2 source taps are gathered through L1/L2
 __global__ void __launch_bounds__(256) k_remap(const uint8_t* __restrict__ src, int sstride, long long sframe, int w, int h,
                                                const RemapEntry* __restrict__ map, const int4* __restrict__ tab,
@@ -23,20 +22,12 @@ __global__ void __launch_bounds__(256) k_remap(const uint8_t* __restrict__ src, 
   const uint8_t* S = src + (long long)blockIdx.z * sframe;
   uint8_t o[4];
 #pragma unroll
-  for (int k = 0; k < 4; k++) {
-    const int x = min(x4 + k, w - 1);
-    const RemapEntry e = map[(long long)y * w + x];
-    const int4 t = __ldg(&tab[e.tab]);     // 16 KB table, L1-resident (per-lane index: not constant memory)
-    auto px = [&](int yy, int xx) { return (xx >= 0 && xx < w && yy >= 0 && yy < h) ? (int)S[(long long)yy * sstride + xx] : 0; };
-    const int acc = px(e.iy, e.ix) * t.x + px(e.iy, e.ix + 1) * t.y + px(e.iy + 1, e.ix) * t.z + px(e.iy + 1, e.ix + 1) * t.w;
-    o[k] = (uint8_t)((acc + (1 << 14)) >> 15);
-  }
+  for (int k = 0; k < 4; k++) o[k] = remap_px(S, sstride, w, h, map[(long long)y * w + min(x4 + k, w - 1)], tab);
   uint8_t* D = dst + (long long)blockIdx.z * dframe + (long long)y * dstride;
   if (x4 + 3 < w && ((dstride & 3) == 0)) *reinterpret_cast<uchar4*>(D + x4) = make_uchar4(o[0], o[1], o[2], o[3]);
   else for (int k = 0; k < 4 && x4 + k < w; k++) D[x4 + k] = o[k];
 }
 
-struct CamD { double fx, fy, cx, cy, k1, k2, p1, p2, k3; };
 __host__ __device__ inline void undistort_point(const CamD& c, float u, float v, float* ou, float* ov) {
   const double ifx = 1. / c.fx, ify = 1. / c.fy;
   double x = ((double)u - c.cx) * ifx, y = ((double)v - c.cy) * ify;
@@ -82,13 +73,6 @@ __global__ void k_frustum_lines(FrustumArgs A, const double* __restrict__ pos, c
 }  // namespace pl
 using namespace pl;
 
-struct PLUndistort {
-  int w, h; CamD cam; float K[4], D[5];
-  RemapEntry* d_map = nullptr;
-  int4* d_tab = nullptr;
-  uint8_t *d_src = nullptr, *d_dst = nullptr; int staged = 0;
-  cudaStream_t stream = nullptr;
-};
 static CamD make_cam(const float* K, const float* D) { return CamD{(double)K[0], (double)K[1], (double)K[2], (double)K[3], (double)D[0], (double)D[1], (double)D[2], (double)D[3], (double)D[4]}; }
 
 extern "C" void pl_undistort_destroy(PLUndistort* h) {

@@ -6,8 +6,9 @@
 //   BinaryDescriptor::compute     spec copy Thirdparty/line_descriptor/src/binary_descriptor_custom.cpp:350-398,539-687,1026-1372
 //
 // Kernel map (DESIGN.md §6)
-//   k_lsd_scale     7x7 sigma .75 Gaussian (8.8 fixed point) fused with the 0.8x INTER_LINEAR_EXACT resize, smem tiles
-//   k_lsd_grad      2x2 gradient -> one 16-byte record per pixel (angle, cos, sin, squared magnitude), per-frame max
+//   k_lsd_front     one tiled pass from the raw frame (undistorted on the fly when a camera map is bound): 7x7 sigma .75
+//                   Gaussian + 0.8x INTER_LINEAR_EXACT resize, 2x2 gradient -> one 16-byte record per pixel (angle, cos,
+//                   sin), squared magnitude, seed cos/sin, per-frame max; and the LBD Sobel pair (below)
 //   k_lsd_seed_order  stable counting sort of the defined pixels into 1024 magnitude bins (descending),
 //                   equal bins keep row-major order == OpenCV 4.13's seed order (pinned in the oracle tests); one
 //                   8-CTA cluster per frame, the order assembled in distributed shared memory.  k_lsd_hist/scan/scatter:
@@ -17,12 +18,13 @@
 //                   order; the 32 lanes test the 3x3 neighbourhood, evaluate angles and reduce the rectangle moments in parallel.
 //   k_keylines      KeyLine records, mask filter, response sort (bitonic, ties keep detection order), truncation
 //                   quirk of LineExtractor.cpp:44-67, normalised 2-D line equations
-//   k_lbd_sobel     5x5 sigma 1 Gaussian (8.8 fixed point) fused with the 3x3 Sobel pair -> int16 dx, dy
+//   (k_lsd_front)   5x5 sigma 1 Gaussian (8.8 fixed point) fused with the 3x3 Sobel pair -> int16 dx, dy
 //   k_lbd_describe  one CTA per line: 63 support rows in parallel (each row accumulates along the line in the
 //                   reference's order, fp32 without FMA), band statistics, 72-float LBD, 32-byte binarisation
 
 #include "common.cuh"
 #include "libm_glibc.cuh"
+#include "remap.cuh"
 #include <cooperative_groups.h>
 #include <math.h>
 #include <string.h>
@@ -85,53 +87,7 @@ __device__ __forceinline__ double angle_diff_signed(double a, double b) {
 __device__ __forceinline__ double dist_d(double x1, double y1, double x2, double y2) { return sqrt((x2 - x1) * (x2 - x1) + (y2 - y1) * (y2 - y1)); }
 __device__ __forceinline__ double dist_sq(double x1, double y1, double x2, double y2) { return (x2 - x1) * (x2 - x1) + (y2 - y1) * (y2 - y1); }
 
-// ---------------------------------------------------------------------------------------------- K_A scale
-// Output tile 32x32 of the 0.8x image <- 40x40 blurred pixels <- 44x44 raw pixels (taps at +-3 are zero).
-__global__ void __launch_bounds__(256) k_lsd_scale(LineParams P, const uint8_t* __restrict__ imgs, int stride,
-                                                   long long frame_stride, uint8_t* __restrict__ scaled) {
-  __shared__ uint8_t raw[44][48];
-  __shared__ uint16_t hp[44][40];
-  __shared__ uint8_t bl[40][40];
-  const int tid = threadIdx.x;
-  const int X0 = blockIdx.x * 32, Y0 = blockIdx.y * 32;
-  const int bx0 = (5 * X0) >> 2, by0 = (5 * Y0) >> 2;
-  const uint8_t* img = imgs + (long long)blockIdx.z * frame_stride;
-  for (int i = tid; i < 44 * 44; i += 256) {
-    int r = i / 44, c = i - r * 44;
-    int gy = reflect101(min(by0 - 2 + r, 2 * P.h - 2), P.h), gx = reflect101(min(bx0 - 2 + c, 2 * P.w - 2), P.w);
-    raw[r][c] = img[(long long)gy * stride + gx];
-  }
-  __syncthreads();
-  for (int i = tid; i < 44 * 40; i += 256) {
-    int r = i / 40, c = i - r * 40;
-    const uint8_t* p = &raw[r][c];
-    hp[r][c] = (uint16_t)(4 * (p[0] + p[4]) + 56 * (p[1] + p[3]) + 136 * p[2]);
-  }
-  __syncthreads();
-  for (int i = tid; i < 40 * 40; i += 256) {
-    int r = i / 40, c = i - r * 40;
-    uint32_t s = 4u * (hp[r][c] + hp[r + 4][c]) + 56u * (hp[r + 1][c] + hp[r + 3][c]) + 136u * hp[r + 2][c];
-    bl[r][c] = (uint8_t)((s + 32768u) >> 16);
-  }
-  __syncthreads();
-  uint8_t* out = scaled + (long long)blockIdx.z * P.npx;
-  for (int i = tid; i < 32 * 32; i += 256) {
-    int ty = i >> 5, tx = i & 31;
-    int x = X0 + tx, y = Y0 + ty;
-    if (x >= P.sw || y >= P.sh) continue;
-    int sx = (10 * x + 1) >> 3, xf = ((10 * x + 1) & 7) * 32;
-    int sy = (10 * y + 1) >> 3, yf = ((10 * y + 1) & 7) * 32;
-    if (sx >= P.w - 1) { sx = P.w - 1; xf = 0; }
-    if (sy >= P.h - 1) { sy = P.h - 1; yf = 0; }
-    int sx1 = min(sx + 1, P.w - 1), sy1 = min(sy + 1, P.h - 1);
-    int lx = sx - bx0, lx1 = sx1 - bx0, ly = sy - by0, ly1 = sy1 - by0;
-    int h0 = bl[ly][lx] * (256 - xf) + bl[ly][lx1] * xf;
-    int h1 = bl[ly1][lx] * (256 - xf) + bl[ly1][lx1] * xf;
-    out[(long long)y * P.sw + x] = (uint8_t)((h0 * (256 - yf) + h1 * yf + 32768) >> 16);
-  }
-}
-
-// ---------------------------------------------------------------------------------------------- K_B gradient
+// ---------------------------------------------------------------------------------------------- gradient records
 // Per scaled pixel, what region growing needs:
 //   REC = 16-byte record {own, angle, cos, sin}: own = ownership word of the region growing (kFree or kNotDef here),
 //         angle = level-line angle in degrees (cv::fastAtan2(gx, -gy)), cos/sin of float(angle_rad) rounded
@@ -162,73 +118,158 @@ __global__ void __launch_bounds__(256) k_lsd_grad_table(GradRec* __restrict__ T,
   grad_record(i / kGradN - kGradR, i % kGradN - kGradR, rec, scs);
   T[i] = rec; TS[i] = scs;
 }
-// One thread = 4 consecutive pixels of a row: two 8-byte row reads, four table lookups, 16-byte stores (the pass is bound by
-// the number of memory instructions, not by bytes).  kVec needs sw % 4 == 0 (rows of every output array 16-byte aligned).
-template <bool kVec>
-__global__ void __launch_bounds__(256) k_lsd_grad(LineParams P, const uint8_t* __restrict__ scaled, const float4* __restrict__ T,
-                                                  const float2* __restrict__ TS,
-                                                  int4* __restrict__ REC, int* __restrict__ S2, float2* __restrict__ seedcs, int* __restrict__ maxs) {
-  __shared__ int smax;
-  if (threadIdx.x == 0) smax = 0;
-  __syncthreads();
-  const int x0 = (blockIdx.x * 64 + (threadIdx.x & 63)) * 4, y = blockIdx.y * 4 + (threadIdx.x >> 6);
-  const int f = blockIdx.z;
-  int smx = 0;
-  if (x0 < P.sw && y < P.sh) {
-    const uint8_t* S = scaled + (long long)f * P.npx + (long long)y * P.sw + x0;
-    const bool lastrow = (y >= P.sh - 1);
-    int r0[5], r1[5];
-    if (kVec) {       // x0 % 4 == 0 and sw % 4 == 0: one aligned word + one byte per row
-      const unsigned w0 = *reinterpret_cast<const unsigned*>(S), w1 = lastrow ? 0u : *reinterpret_cast<const unsigned*>(S + P.sw);
-#pragma unroll
-      for (int k = 0; k < 4; k++) { r0[k] = (w0 >> (8 * k)) & 0xff; r1[k] = (w1 >> (8 * k)) & 0xff; }
-      const bool in4 = (x0 + 4 < P.sw);
-      r0[4] = in4 ? S[4] : 0; r1[4] = (in4 && !lastrow) ? S[P.sw + 4] : 0;
-    } else {
-#pragma unroll
-      for (int k = 0; k < 5; k++) {
-        const bool in = (x0 + k < P.sw);
-        r0[k] = in ? S[k] : 0;
-        r1[k] = (in && !lastrow) ? S[P.sw + k] : 0;
-      }
+// ---------------------------------------------------------------------------------------------- K_A front: image -> LSD + LBD inputs
+// One pass per (tile, frame) builds everything the later stages read from the frame, from the raw frame in HBM:
+//   source    the undistorted pixel (remap.cuh, when a camera map is bound) or the frame itself, at reflect-101 coordinates
+//   LSD       7x7 sigma .75 Gaussian (8.8 fixed point; its taps at +-3 are zero) + 0.8x INTER_LINEAR_EXACT resize -> scaled
+//             image; 2x2 gradient -> pixel record, gx^2+gy^2 and seed cos/sin (see grad_record), per-frame max of gx^2+gy^2
+//   LBD       5x5 sigma 1 Gaussian (8.8 fixed point) + 3x3 Sobel pair -> int16 dx, dy
+// Tile: 64x32 scaled pixels <-> 80x40 undistorted pixels.  Scaled x reads blurred (10x+1)>>3 and the pixel after it, so
+// scaled columns [64i, 64i+64) read blurred columns [80i, 80i+80), and the same 80 columns are the tile's Sobel outputs.
+// One source tile serves both: undistorted columns 80i-3 .. 80i+83, rows 40j-3 .. 40j+43 (the 5-tap blurs, one more scaled
+// column and row for the 2x2 gradient, the blurred ring of the Sobel).  Every source position is loaded at the
+// reflect-101 coordinate both kernels it restates used: the LBD blur is symmetric, so the blurred value of the reflected
+// image at -1 equals the one at +1, exactly Sobel's own BORDER_REFLECT_101 of the blurred image; no tap reflects again.
+// A CTA keeps its tile and walks kFrontFrames frames: the camera map of the tile (32 KB) is read from L2 once per CTA.
+// Every output row of a warp is contiguous (one thread per pixel): a warp stores 512 B of records, 256 B of seed cos/sin
+// and 128 B of gx^2+gy^2 in whole sectors.
+constexpr int kFrontSX = 64, kFrontSY = 32;                          // scaled pixels per tile
+constexpr int kFrontUX = 80, kFrontUY = 40;                          // undistorted (Sobel) pixels per tile
+constexpr int kFrontSrcW = kFrontUX + 7, kFrontSrcH = kFrontUY + 7;  // source tile: 3 before, 4 after
+constexpr int kFrontSrcP = kFrontSrcW + 1;
+constexpr int kFrontBW = kFrontUX + 2, kFrontBH = kFrontUY + 2;      // blurred tiles (LSD: +2 after; LBD: 1 before, 1 after)
+constexpr int kFrontSegRows = kFrontBH / 3;                          // blur: 3 row segments x 82 columns = 246 threads
+constexpr int kFrontFrames = 8;                                      // frames per CTA
+constexpr int kFrontThreads = 256;
+static_assert(kFrontBH % 3 == 0 && 3 * kFrontBW <= kFrontThreads, "blur thread layout");
+constexpr size_t kFrontMapSmem = (size_t)kFrontSrcH * kFrontSrcW * sizeof(RemapEntry);
+
+template <bool kMap>
+__global__ void __launch_bounds__(kFrontThreads) k_lsd_front(LineParams P, const uint8_t* __restrict__ imgs, int stride,
+                                                             long long frame_stride, int B, const RemapEntry* __restrict__ map,
+                                                             const int4* __restrict__ tab, const float4* __restrict__ T,
+                                                             const float2* __restrict__ TS, uint8_t* __restrict__ scaled,
+                                                             int4* __restrict__ REC, int* __restrict__ S2, float2* __restrict__ seedcs,
+                                                             int* __restrict__ maxs, short2* __restrict__ dxy) {
+  extern __shared__ __align__(16) unsigned char front_smem[];
+  RemapEntry* mp = reinterpret_cast<RemapEntry*>(front_smem);        // [kFrontSrcH * kFrontSrcW] (kMap only)
+  __shared__ uint8_t src[kFrontSrcH * kFrontSrcP];                   // undistorted (V0-3+r, U0-3+c)
+  __shared__ uint8_t bl[kFrontBH * kFrontBW];                        // LSD blur at (V0+r, U0+c)
+  __shared__ uint8_t bs[kFrontBH * kFrontBW];                        // LBD blur at (V0-1+r, U0-1+c)
+  __shared__ uint8_t sc[(kFrontSY + 1) * (kFrontSX + 1)];           // scaled (Y0+r, X0+c), 0 outside the image
+  __shared__ int smax[kFrontFrames];
+  const int tid = threadIdx.x, lane = tid & 31;
+  const int X0 = blockIdx.x * kFrontSX, Y0 = blockIdx.y * kFrontSY, U0 = blockIdx.x * kFrontUX, V0 = blockIdx.y * kFrontUY;
+  const int f0 = blockIdx.z * kFrontFrames, nf = min(kFrontFrames, B - f0);
+  auto srow = [&](int r) { return reflect101(min(V0 - 3 + r, 2 * P.h - 2), P.h); };
+  auto scol = [&](int c) { return reflect101(min(U0 - 3 + c, 2 * P.w - 2), P.w); };
+  if (tid < kFrontFrames) smax[tid] = 0;
+  if (kMap)
+    for (int i = tid; i < kFrontSrcH * kFrontSrcW; i += kFrontThreads) {
+      const int r = i / kFrontSrcW, c = i - r * kFrontSrcW;
+      mp[i] = map[(long long)srow(r) * P.w + scol(c)];
     }
-    int4 rec[4];
-    float se[4][2];
-    int sq[4];
+  __syncthreads();
+  for (int fi = 0; fi < nf; fi++) {
+    const int f = f0 + fi;
+    const uint8_t* img = imgs + (long long)f * frame_stride;
+    // 1. source tile
+    for (int i = tid; i < kFrontSrcH * kFrontSrcW; i += kFrontThreads) {
+      const int r = i / kFrontSrcW, c = i - r * kFrontSrcW;
+      src[r * kFrontSrcP + c] = kMap ? remap_px(img, stride, P.w, P.h, mp[i], tab) : img[(long long)srow(r) * stride + scol(c)];
+    }
+    __syncthreads();
+    // 2. both blurs: a thread walks down one blurred column of a row segment with the last five row sums of each in registers;
+    //    LBD column c reads source columns c..c+4, LSD column c source columns c+1..c+5
+    if (tid < 3 * kFrontBW) {
+      const int c = tid % kFrontBW, r0 = (tid / kFrontBW) * kFrontSegRows;
+      const uint8_t* p = src + r0 * kFrontSrcP + c;
+      int hs[5] = {0, 0, 0, 0, 0}, hl[5] = {0, 0, 0, 0, 0};
 #pragma unroll
-    for (int k = 0; k < 4; k++) {
-      rec[k] = make_int4(kNotDef, __float_as_int(kNotDefDeg), 0, 0); se[k][0] = se[k][1] = 0.f; sq[k] = 0;
-      if (x0 + k < P.sw - 1 && !lastrow) {
-        const int DA = r1[k + 1] - r0[k], BC = r0[k + 1] - r1[k];
-        const int gx = DA + BC, gy = DA - BC;
-        const int s = gx * gx + gy * gy;
-        sq[k] = s;
-        if (s > P.s_th) {
-          const int ti = (gx + kGradR) * kGradN + (gy + kGradR);
-          const float4 t = __ldg(&T[ti]);
-          const float2 scs = __ldg(&TS[ti]);
-          rec[k] = make_int4(kFree, __float_as_int(t.x), __float_as_int(t.y), __float_as_int(t.z));
-          se[k][0] = scs.x; se[k][1] = scs.y;
-          smx = max(smx, s);
+      for (int k = 0; k < kFrontSegRows + 5; k++, p += kFrontSrcP) {
+        const int q0 = p[0], q1 = p[1], q2 = p[2], q3 = p[3], q4 = p[4], q5 = p[5];
+#pragma unroll
+        for (int j = 0; j < 4; j++) { hs[j] = hs[j + 1]; hl[j] = hl[j + 1]; }
+        hs[4] = 14 * (q0 + q4) + 62 * (q1 + q3) + 104 * q2;
+        hl[4] = 4 * (q1 + q5) + 56 * (q2 + q4) + 136 * q3;
+        if (k >= 4 && k - 4 < kFrontSegRows) {       // LBD row r0+k-4 <- source rows r0+k-4 .. r0+k
+          const unsigned acc = 14u * (unsigned)(hs[0] + hs[4]) + 62u * (unsigned)(hs[1] + hs[3]) + 104u * (unsigned)hs[2];
+          bs[(r0 + k - 4) * kFrontBW + c] = (uint8_t)((acc + 32768u) >> 16);
+        }
+        if (k >= 5) {                                 // LSD row r0+k-5 <- source rows r0+k-4 .. r0+k
+          const unsigned s = 4u * (unsigned)(hl[0] + hl[4]) + 56u * (unsigned)(hl[1] + hl[3]) + 136u * (unsigned)hl[2];
+          bl[(r0 + k - 5) * kFrontBW + c] = (uint8_t)((s + 32768u) >> 16);
         }
       }
     }
-    const long long o = (long long)f * P.npx + (long long)y * P.sw + x0;
-    if (kVec) {
-#pragma unroll
-      for (int k = 0; k < 4; k++) REC[o + k] = rec[k];
-      *reinterpret_cast<int4*>(S2 + o) = make_int4(sq[0], sq[1], sq[2], sq[3]);
-      float4* e4 = reinterpret_cast<float4*>(seedcs + o);
-      e4[0] = make_float4(se[0][0], se[0][1], se[1][0], se[1][1]); e4[1] = make_float4(se[2][0], se[2][1], se[3][0], se[3][1]);
-    } else {
-      for (int k = 0; k < 4 && x0 + k < P.sw; k++) { REC[o + k] = rec[k]; S2[o + k] = sq[k]; seedcs[o + k] = make_float2(se[k][0], se[k][1]); }
+    __syncthreads();
+    // 3. 0.8x resize (INTER_LINEAR_EXACT, clamps at w-1 and h-1) of the tile and one more column and row
+    uint8_t* out = scaled + (long long)f * P.npx;
+    for (int i = tid; i < (kFrontSY + 1) * (kFrontSX + 1); i += kFrontThreads) {
+      const int ty = i / (kFrontSX + 1), tx = i - ty * (kFrontSX + 1);
+      const int x = X0 + tx, y = Y0 + ty;
+      uint8_t v = 0;
+      if (x < P.sw && y < P.sh) {
+        int sx = (10 * x + 1) >> 3, xf = ((10 * x + 1) & 7) * 32;
+        int sy = (10 * y + 1) >> 3, yf = ((10 * y + 1) & 7) * 32;
+        if (sx >= P.w - 1) { sx = P.w - 1; xf = 0; }
+        if (sy >= P.h - 1) { sy = P.h - 1; yf = 0; }
+        const int sx1 = min(sx + 1, P.w - 1), sy1 = min(sy + 1, P.h - 1);
+        const uint8_t* b0 = bl + (sy - V0) * kFrontBW;
+        const uint8_t* b1 = bl + (sy1 - V0) * kFrontBW;
+        const int h0 = b0[sx - U0] * (256 - xf) + b0[sx1 - U0] * xf;
+        const int h1 = b1[sx - U0] * (256 - xf) + b1[sx1 - U0] * xf;
+        v = (uint8_t)((h0 * (256 - yf) + h1 * yf + 32768) >> 16);
+        if (tx < kFrontSX && ty < kFrontSY) out[(long long)y * P.sw + x] = v;
+      }
+      sc[i] = v;
     }
-  }
+    __syncthreads();
+    // 4. gradient records: one pixel per thread, a warp on 32 consecutive pixels of a row
+    int smx = 0;
+    for (int i = tid; i < kFrontSY * kFrontSX; i += kFrontThreads) {
+      const int ty = i / kFrontSX, tx = i - ty * kFrontSX;
+      const int x = X0 + tx, y = Y0 + ty;
+      if (x >= P.sw || y >= P.sh) continue;
+      int4 rec = make_int4(kNotDef, __float_as_int(kNotDefDeg), 0, 0);
+      float2 se = make_float2(0.f, 0.f);
+      int sq = 0;
+      if (x < P.sw - 1 && y < P.sh - 1) {
+        const uint8_t* q = sc + ty * (kFrontSX + 1) + tx;
+        const int DA = q[kFrontSX + 2] - q[0], BC = q[1] - q[kFrontSX + 1];
+        const int gx = DA + BC, gy = DA - BC;
+        sq = gx * gx + gy * gy;
+        if (sq > P.s_th) {
+          const int ti = (gx + kGradR) * kGradN + (gy + kGradR);
+          const float4 t = __ldg(&T[ti]);
+          se = __ldg(&TS[ti]);
+          rec = make_int4(kFree, __float_as_int(t.x), __float_as_int(t.y), __float_as_int(t.z));
+          smx = max(smx, sq);
+        }
+      }
+      const long long o = (long long)f * P.npx + (long long)y * P.sw + x;
+      REC[o] = rec; S2[o] = sq; seedcs[o] = se;
+    }
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) smx = max(smx, __shfl_xor_sync(0xffffffffu, smx, o));
-  if ((threadIdx.x & 31) == 0 && smx > 0) atomicMax(&smax, smx);
+    for (int o = 16; o > 0; o >>= 1) smx = max(smx, __shfl_xor_sync(0xffffffffu, smx, o));
+    if (lane == 0 && smx > 0) atomicMax(&smax[fi], smx);
+    // 5. Sobel pair of the tile's undistorted pixels
+    short2* D = dxy + (long long)f * P.w * P.h;
+    for (int i = tid; i < kFrontUY * kFrontUX; i += kFrontThreads) {
+      const int ry = i / kFrontUX, rx = i - ry * kFrontUX;
+      const int x = U0 + rx, y = V0 + ry;
+      if (x >= P.w || y >= P.h) continue;
+      const uint8_t* b = bs + ry * kFrontBW + rx;
+      const int a00 = b[0], a01 = b[1], a02 = b[2];
+      const int a10 = b[kFrontBW], a12 = b[kFrontBW + 2];
+      const int a20 = b[2 * kFrontBW], a21 = b[2 * kFrontBW + 1], a22 = b[2 * kFrontBW + 2];
+      D[(long long)y * P.w + x] = make_short2((short)((a02 - a00) + 2 * (a12 - a10) + (a22 - a20)),
+                                              (short)((a20 - a00) + 2 * (a21 - a01) + (a22 - a02)));
+    }
+    // the next frame's stages 1-3 overwrite src, bl/bs and sc only after its first barrier: every read of this frame is done
+  }
   __syncthreads();
-  if (threadIdx.x == 0 && smax > 0) atomicMax(&maxs[f], smax);
+  if (tid < nf && smax[tid] > 0) atomicMax(&maxs[f0 + tid], smax[tid]);
 }
 __device__ __forceinline__ double s_norm(int s) { return sqrt((double)s / 4.0); }
 __device__ __forceinline__ int s_bin(int s, double bin_coef) { return (int)(s_norm(s) * bin_coef); }
@@ -553,63 +594,6 @@ __global__ void __launch_bounds__(256) k_keylines(LineParams P, const float4* __
   if (tid == 0) nl[f] = min(nout, P.capL);
 }
 
-// ---------------------------------------------------------------------------------------------- K_H LBD blur + Sobel
-// GaussianBlur 5x5 sigma 1 (8.8 fixed point rows [14 62 104 62 14]) fused with the Sobel pair (dx, dy as int16).
-// Tile: 64x64 blurred pixels <- 68x68 raw pixels in shared memory -> 62x62 outputs.  The raw tile is loaded at
-// reflect-101 coordinates; because the kernel is symmetric, the blur of the reflected image at column -1 equals the
-// blurred value at column +1, i.e. exactly what Sobel's own BORDER_REFLECT_101 of the BLURRED image needs, so no tap
-// ever reflects again.  One thread walks down one column: the last five horizontal sums live in registers (blur), then
-// a sliding 3x3 window of blurred bytes (Sobel).
-constexpr int kSobT = 64, kSobOut = kSobT - 2, kSobRawP = kSobT + 8, kSobSeg = kSobT / 4;
-__global__ void __launch_bounds__(256) k_lbd_sobel(LineParams P, const uint8_t* __restrict__ imgs, int stride,
-                                                   long long frame_stride, short2* __restrict__ dxy) {
-  __shared__ uint8_t raw[(kSobT + 4) * kSobRawP];
-  __shared__ uint8_t bl[kSobT * (kSobT + 4)];
-  const int tx = threadIdx.x & 63, ty = threadIdx.x >> 6;
-  const int X0 = blockIdx.x * kSobOut, Y0 = blockIdx.y * kSobOut;   // first output pixel of the tile
-  const uint8_t* img = imgs + (long long)blockIdx.z * frame_stride;
-  auto r101 = [](int p, int n) { if (p < 0) p = -p; if (p >= n) p = 2 * (n - 1) - p; return min(max(p, 0), n - 1); };
-  // raw rows Y0-3 .. Y0+64, columns X0-3 .. X0+64
-  for (int r = ty; r < kSobT + 4; r += 4) {
-    const uint8_t* row = img + (long long)r101(Y0 - 3 + r, P.h) * stride;
-    raw[r * kSobRawP + tx] = row[r101(X0 - 3 + tx, P.w)];
-    if (tx < 4) raw[r * kSobRawP + kSobT + tx] = row[r101(X0 - 3 + kSobT + tx, P.w)];
-  }
-  __syncthreads();
-  {  // blurred pixel (bx, by) of the tile = image pixel (X0-1+bx, Y0-1+by); thread: column tx, rows ty*16 .. +15
-    const uint8_t* p = raw + (ty * kSobSeg) * kSobRawP + tx;
-    auto hrow = [&](const uint8_t* q) { return 14 * (q[0] + q[4]) + 62 * (q[1] + q[3]) + 104 * q[2]; };
-    int w0 = hrow(p), w1 = hrow(p + kSobRawP), w2 = hrow(p + 2 * kSobRawP), w3 = hrow(p + 3 * kSobRawP);
-    p += 4 * kSobRawP;
-    uint8_t* o = bl + (ty * kSobSeg) * (kSobT + 4) + tx;
-#pragma unroll 4
-    for (int r = 0; r < kSobSeg; r++, p += kSobRawP, o += kSobT + 4) {
-      const int w4 = hrow(p);
-      const unsigned acc = 14u * (unsigned)(w0 + w4) + 62u * (unsigned)(w1 + w3) + 104u * (unsigned)w2;
-      *o = (uint8_t)((acc + 32768u) >> 16);
-      w0 = w1; w1 = w2; w2 = w3; w3 = w4;
-    }
-  }
-  __syncthreads();
-  const int x = X0 + tx - 1;                       // output column of blurred column tx (1..62 produce outputs)
-  if (tx < 1 || tx > kSobOut || x >= P.w) return;
-  const int rbeg = max(ty * kSobSeg, 1), rend = min(ty * kSobSeg + kSobSeg - 1, kSobOut);   // blurred rows of my outputs
-  const uint8_t* b = bl + (rbeg - 1) * (kSobT + 4) + tx;
-  int a00 = b[-1], a01 = b[0], a02 = b[1];
-  b += kSobT + 4;
-  int a10 = b[-1], a11 = b[0], a12 = b[1];
-  short2* D = dxy + (long long)blockIdx.z * P.w * P.h;
-  for (int r = rbeg; r <= rend; r++) {
-    b += kSobT + 4;
-    const int a20 = b[-1], a21 = b[0], a22 = b[1];
-    const int y = Y0 + r - 1;
-    if (y < P.h)
-      D[(long long)y * P.w + x] = make_short2((short)((a02 - a00) + 2 * (a12 - a10) + (a22 - a20)),
-                                              (short)((a20 - a00) + 2 * (a21 - a01) + (a22 - a02)));
-    a00 = a10; a01 = a11; a02 = a12; a10 = a20; a11 = a21; a12 = a22;
-  }
-}
-
 // ---------------------------------------------------------------------------------------------- K_I LBD describe
 __constant__ float c_gaussG[63];
 __constant__ float c_gaussL[21];
@@ -750,6 +734,8 @@ struct PLLine {
   // host-pointer API staging
   uint8_t* d_img = nullptr; PLKeyLineRec* d_kls = nullptr; uint8_t* d_desc = nullptr; double* d_lf = nullptr; int* d_nl = nullptr;
   uint8_t* d_mask = nullptr;
+  const PLUndistort* und = nullptr;     // pl_line_set_undistort: the frames are raw, k_lsd_front undistorts them (owned by the caller)
+  uint8_t* d_und = nullptr;             // undistorted frames of batches below 32 frames per SM (made on first use)
   size_t key_smem = 0;
   int last_B = 0;
   // optional device timing of the dominant kernel (bench.py roofline): events on the launching stream
@@ -764,7 +750,7 @@ extern "C" void pl_line_destroy(PLLine* h) {
   if (!h) return;
   cudaFree(h->d_gtab); cudaFree(h->d_gtab_seed); cudaFree(h->d_scaled); cudaFree(h->d_seedcs); cudaFree(h->d_rec); cudaFree(h->d_sq); cudaFree(h->d_region); cudaFree(h->d_far); cudaFree(h->d_wtab); cudaFree(h->d_counts); cudaFree(h->d_offsets);
   cudaFree(h->d_ndef); cudaFree(h->d_maxs); cudaFree(h->d_nseg); cudaFree(h->d_overflow); cudaFree(h->d_order);
-  cudaFree(h->d_segs); cudaFree(h->d_dxy); cudaFree(h->d_img); cudaFree(h->d_kls);
+  cudaFree(h->d_segs); cudaFree(h->d_dxy); cudaFree(h->d_und); cudaFree(h->d_img); cudaFree(h->d_kls);
   cudaFree(h->d_desc); cudaFree(h->d_lf); cudaFree(h->d_nl); cudaFree(h->d_mask);
   if (h->stream) cudaStreamDestroy(h->stream);
   delete h;
@@ -868,6 +854,16 @@ extern "C" int pl_line_create(const PLLineConfig* cfg, PLLine** out) {
 
 extern "C" int pl_line_capacity(const PLLine* h) { return h ? h->P.capL : PL_ERR_ARG; }
 
+extern "C" int pl_line_set_undistort(PLLine* h, const PLUndistort* und) {
+  PL_ARG(h);
+  if (und && (und->w != h->P.w || und->h != h->P.h)) {
+    set_error("pl_line_set_undistort: a %dx%d map for %dx%d frames", und->w, und->h, h->P.w, h->P.h);
+    return PL_ERR_ARG;
+  }
+  h->und = und;
+  return PL_OK;
+}
+
 // Device timing of k_lsd_grow_ordered (the dominant kernel): enable, run, then read the duration of the LAST launch.
 extern "C" int pl_line_set_timing(PLLine* h, int on) {
   PL_ARG(h);
@@ -907,14 +903,35 @@ extern "C" int pl_line_extract_batch_dev(PLLine* h, const uint8_t* imgs, int str
   h->last_B = B;
   h->last_seed_cluster = cluster;
   PL_CUDA(cudaMemsetAsync(h->d_maxs, 0, sizeof(int) * B, st));
-  k_lsd_scale<<<dim3((P.sw + 31) / 32, (P.sh + 31) / 32, B), 256, 0, st>>>(P, imgs, stride, (long long)frame_stride, h->d_scaled);
-  PL_LAUNCH_CHECK();
-  {
-    const dim3 grd((P.sw + 255) / 256, (P.sh + 3) / 4, B);
-    if (P.sw % 4 == 0)
-      k_lsd_grad<true><<<grd, 256, 0, st>>>(P, h->d_scaled, reinterpret_cast<const float4*>(h->d_gtab), h->d_gtab_seed, h->d_rec, h->d_sq, h->d_seedcs, h->d_maxs);
-    else
-      k_lsd_grad<false><<<grd, 256, 0, st>>>(P, h->d_scaled, reinterpret_cast<const float4*>(h->d_gtab), h->d_gtab_seed, h->d_rec, h->d_sq, h->d_seedcs, h->d_maxs);
+  {  // scaled image, pixel records, gx^2+gy^2, seed cos/sin, per-frame max and the LBD Sobel pair in one pass
+    // Below 32 frames per SM the front-end runs its chains on three streams (frontend.cu), and there the fused pass is placed
+    // beside the ORB chain's kernels.  Measured there (DESIGN.md §7), the grow that follows on the same SMs ran 10-20 % slower
+    // in two cases.  Case 1: the camera map read inside this pass (EuRoC configuration); so such batches undistort the frames
+    // first with k_remap, as before.  Case 2: this kernel's default shared-memory carve-out (KITTI configuration), which an SM
+    // keeps while other kernels stay resident; so such batches ask for the smallest carve-out, and the grow keeps its L1.
+    const bool serial = B >= h->seed_min_batch;
+    int rc = PL_OK;
+    const uint8_t* src = imgs; int sstride = stride; long long sframe = (long long)frame_stride;
+    if (h->und && !serial) {
+      const size_t fb = (size_t)P.w * P.h;
+      if (!h->d_und && (rc = dev_alloc(&h->d_und, fb * h->cfg.max_batch))) return rc;
+      // the remap only reads the map: the handle stays the caller's
+      if ((rc = pl_undistort_remap_batch_dev(const_cast<PLUndistort*>(h->und), imgs, stride, frame_stride, B, h->d_und, P.w, fb, st))) return rc;
+      src = h->d_und; sstride = P.w; sframe = (long long)fb;
+    }
+    const bool map = h->und && serial;
+    const dim3 grd(std::max((P.sw + kFrontSX - 1) / kFrontSX, (P.w + kFrontUX - 1) / kFrontUX),
+                   std::max((P.sh + kFrontSY - 1) / kFrontSY, (P.h + kFrontUY - 1) / kFrontUY), (B + kFrontFrames - 1) / kFrontFrames);
+    const float4* T = reinterpret_cast<const float4*>(h->d_gtab);
+    const RemapEntry* mp = map ? h->und->d_map : nullptr;
+    const int4* tab = map ? h->und->d_tab : nullptr;
+    cudaLaunchConfig_t lc = {};
+    lc.gridDim = grd; lc.blockDim = dim3(kFrontThreads); lc.dynamicSmemBytes = map ? kFrontMapSmem : 0; lc.stream = st;
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributePreferredSharedMemoryCarveout; at[0].val.sharedMemCarveout = 0;
+    if (!serial) { lc.attrs = at; lc.numAttrs = 1; }
+    PL_CUDA(cudaLaunchKernelEx(&lc, map ? k_lsd_front<true> : k_lsd_front<false>, P, src, sstride, sframe, B, mp, tab, T,
+                               (const float2*)h->d_gtab_seed, h->d_scaled, h->d_rec, h->d_sq, h->d_seedcs, h->d_maxs, h->d_dxy));
   }
   PL_LAUNCH_CHECK();
   if (cluster) {
@@ -946,8 +963,6 @@ extern "C" int pl_line_extract_batch_dev(PLLine* h, const uint8_t* imgs, int str
   PL_LAUNCH_CHECK();
   if (h->timing) PL_CUDA(cudaEventRecord(h->ev1, st));
   k_keylines<<<B, 256, h->key_smem, st>>>(P, h->d_segs, h->d_nseg, mask, (PLKeyLineRec*)keylines, linefunc, n);
-  PL_LAUNCH_CHECK();
-  k_lbd_sobel<<<dim3((P.w + kSobOut - 1) / kSobOut, (P.h + kSobOut - 1) / kSobOut, B), 256, 0, st>>>(P, imgs, stride, (long long)frame_stride, h->d_dxy);
   PL_LAUNCH_CHECK();
   k_lbd_describe<<<dim3(P.capL, B), 64, 0, st>>>(P, (const PLKeyLineRec*)keylines, n, h->d_dxy, desc);
   PL_LAUNCH_CHECK();

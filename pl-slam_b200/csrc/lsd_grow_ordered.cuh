@@ -2,7 +2,7 @@
 // Produces the oracle's segment list bit for bit.  Included by line.cu only, after LineParams and the shared helpers
 // (kFree / kNotDef, kPI / kDegToRads, fast_atan2_deg, angle_diff_signed, dist_d, dist_sq).
 //
-// Pixel records {own, angle, cos, sin}, 16 bytes (k_lsd_grad): the ownership word says free (kFree) / undefined (kNotDef) /
+// Pixel records {own, angle, cos, sin}, 16 bytes (k_lsd_front): the ownership word says free (kFree) / undefined (kNotDef) /
 // used (0), and is written with plain stores by the lane that owns the pixel.
 //
 // Exactness of the fp64 parts (what round 1 did not have): LineSegmentDetectorImpl::region2rect / get_theta / refine sum over
