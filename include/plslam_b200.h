@@ -39,6 +39,9 @@ typedef struct PLKeyPoint { /* byte-compatible with cv::KeyPoint (28 B) */
 typedef struct PLOrbConfig {
   int width, height;   /* frame size (fixed per handle)                               */
   int nfeatures;       /* ORBextractor.nFeatures                                      */
+                       /* each level's quota (mnFeaturesPerLevel) must fit one quadtree in shared memory: at most 4878
+                        * on a 4:3 frame with the H100's 232448 B per block; pl_orb_create refuses a larger quota with
+                        * PL_ERR_ARG and names the largest that fits */
   float scale_factor;  /* ORBextractor.scaleFactor                                    */
   int nlevels;         /* ORBextractor.nLevels (<= 12)                                */
   int ini_th_fast;     /* ORBextractor.iniThFAST                                      */

@@ -13,7 +13,8 @@
 #include <vector>
 
 namespace pl {
-// 4 consecutive output pixels per thread (uchar4 store); the 2x2 source taps are gathered through L1/L2
+// 4 consecutive output pixels per thread (uchar4 store where the row pointer is 4-byte aligned: a destination ROI may start
+// at any column and dframe may be any size); the 2x2 source taps are gathered through L1/L2
 __global__ void __launch_bounds__(256) k_remap(const uint8_t* __restrict__ src, int sstride, long long sframe, int w, int h,
                                                const RemapEntry* __restrict__ map, const int4* __restrict__ tab,
                                                uint8_t* __restrict__ dst, int dstride, long long dframe) {
@@ -24,7 +25,7 @@ __global__ void __launch_bounds__(256) k_remap(const uint8_t* __restrict__ src, 
 #pragma unroll
   for (int k = 0; k < 4; k++) o[k] = remap_px(S, sstride, w, h, map[(long long)y * w + min(x4 + k, w - 1)], tab);
   uint8_t* D = dst + (long long)blockIdx.z * dframe + (long long)y * dstride;
-  if (x4 + 3 < w && ((dstride & 3) == 0)) *reinterpret_cast<uchar4*>(D + x4) = make_uchar4(o[0], o[1], o[2], o[3]);
+  if (x4 + 3 < w && (((uintptr_t)D & 3) == 0)) *reinterpret_cast<uchar4*>(D + x4) = make_uchar4(o[0], o[1], o[2], o[3]);
   else for (int k = 0; k < 4 && x4 + k < w; k++) D[x4 + k] = o[k];
 }
 

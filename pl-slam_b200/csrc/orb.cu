@@ -871,13 +871,30 @@ extern "C" int pl_orb_create(const PLOrbConfig* cfg, PLOrb** out) {
   }
   P.ncells = (int)h->cells.size();
   P.pyr_frame = off; P.key_frame = keyoff; P.blur_frame = boff;
-  P.poolcap = (maxN + 4 * maxIni + 24 + 1) & ~1;
+  // k_quadtree holds one level's node pool, its bitonic sort region (a power of two) and free list in shared memory
+  auto poolcap_for = [&](int n) { return (n + 4 * maxIni + 24 + 1) & ~1; };
+  auto quad_smem_for = [&](int n) {
+    const int pc = poolcap_for(n);
+    int p2 = 1; while (p2 < pc) p2 <<= 1;
+    return (size_t)pc * sizeof(QNode) + (size_t)p2 * 8 + (size_t)pc * 6 + 64;
+  };
+  P.poolcap = poolcap_for(maxN);
   P.selcap = maxN + 4;
   P.cap = cfg->nfeatures + 4 * nl;
-  {  // bitonic sort needs a power-of-two region
-    int p2 = 1; while (p2 < P.poolcap) p2 <<= 1;
-    P.sortcap = p2;
-    h->quad_smem = (size_t)P.poolcap * sizeof(QNode) + (size_t)p2 * 8 + (size_t)P.poolcap * 6 + 64;
+  { int p2 = 1; while (p2 < P.poolcap) p2 <<= 1; P.sortcap = p2; }
+  h->quad_smem = quad_smem_for(maxN);
+  {
+    int dev = 0, smem_max = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&smem_max, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
+    if (h->quad_smem > (size_t)smem_max) {
+      int fit = maxN;
+      while (fit > 0 && quad_smem_for(fit) > (size_t)smem_max) fit--;
+      set_error("a per-level quota of %d features needs %zu B of quadtree shared memory, over the device's %d B; at most %d "
+                "features fit on one level (mnFeaturesPerLevel)", maxN, h->quad_smem, smem_max, fit);
+      delete h;
+      return PL_ERR_ARG;
+    }
   }
   const int B = cfg->max_batch;
 #define ORB_TRY(e) do { int _r = (e); if (_r) { pl_orb_destroy(h); return _r; } } while (0)
