@@ -6,7 +6,9 @@
  *
  * Conventions: plain pointers and sizes; `_dev` variants take DEVICE pointers (inputs resident
  * in HBM) plus a cudaStream_t passed as void* (NULL = the handle's own stream) and are
- * asynchronous; the plain variants take HOST pointers, copy in/out and synchronise.
+ * asynchronous; the plain variants take HOST pointers, copy in/out and synchronise.  A plain variant
+ * refuses a NULL array whose count is > 0 with PL_ERR_ARG, and reports a failed device allocation
+ * or copy while staging its arrays as PL_ERR_CUDA.
  * Return value: 0 = ok, <0 = error (pl_last_error() gives the text).  There is NO CPU fallback:
  * without a usable sm_90 (H100) device every compute entry point fails with PL_ERR_CUDA.
  */

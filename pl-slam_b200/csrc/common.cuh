@@ -5,6 +5,7 @@
 #include <stdio.h>
 #include <string>
 #include <atomic>
+#include <vector>
 #include "../../include/plslam_b200.h"
 
 namespace pl {
@@ -51,6 +52,70 @@ inline int dev_alloc(T** p, size_t n) {
   PL_CUDA(cudaMalloc((void**)p, n * sizeof(T)));
   return PL_OK;
 }
+
+// Device copies of one host-pointer call's arrays, freed when it goes out of scope.  What is not copied in is zero-filled; fills
+// and copies are synchronous cudaMemset / cudaMemcpy on the legacy default stream.  The first failure sticks and makes the later
+// calls no-ops that return NULL: PL_ERR_CUDA for a failed allocation or copy, PL_ERR_ARG for a NULL host array whose count is
+// > 0.  So a wrapper stages everything, then checks status() once before it launches.
+class Staging {
+ public:
+  Staging() = default;
+  Staging(const Staging&) = delete;
+  Staging& operator=(const Staging&) = delete;
+  ~Staging() { for (void* p : bufs_) cudaFree(p); }
+  int status() const { return rc_; }
+  // n elements of h in a buffer of max(room, n, 1) elements
+  template <typename T> T* in(const T* h, size_t n, size_t room = 0) {
+    if (!rc_ && n && !h) { rc_ = PL_ERR_ARG; set_error("host staging: NULL host array of %zu elements", n); }
+    T* d = alloc<T>(n > room ? n : room, n);
+    if (d && n) cuda(cudaMemcpy(d, h, n * sizeof(T), cudaMemcpyHostToDevice));
+    return rc_ ? nullptr : d;
+  }
+  // a buffer of max(n, 1) elements
+  template <typename T> T* out(size_t n) { return alloc<T>(n); }
+  // a buffer of max(room, n, 1) elements whose first n fetch() copies to h; none when h is NULL (an output not asked for)
+  template <typename T> T* out(T* h, size_t n, size_t room = 0) {
+    if (!h) return nullptr;
+    T* d = alloc<T>(n > room ? n : room);
+    if (d) outs_.push_back({h, d, n * sizeof(T)});
+    return d;
+  }
+  // waits for the fills and copies so far, before a launch on a stream that does not synchronise with the legacy one
+  int sync() { if (!rc_) cuda(cudaStreamSynchronize(cudaStreamLegacy)); return rc_; }
+  // n elements of d to h
+  template <typename T> int down(T* h, const T* d, size_t n) {
+    if (!rc_ && n) cuda(cudaMemcpy(h, d, n * sizeof(T), cudaMemcpyDeviceToHost));
+    return rc_;
+  }
+  // every out(h, n) buffer to its host array
+  int fetch() {
+    for (const Out& o : outs_) if (!rc_ && o.bytes) cuda(cudaMemcpy(o.host, o.dev, o.bytes, cudaMemcpyDeviceToHost));
+    return rc_;
+  }
+
+ private:
+  struct Out { void* host; const void* dev; size_t bytes; };
+  // max(n, 1) elements, zeroed from element `copied` on (the ones before it are the caller's to copy in)
+  template <typename T> T* alloc(size_t n, size_t copied = 0) {
+    if (rc_) return nullptr;
+    const size_t bytes = (n ? n : 1) * sizeof(T), head = copied * sizeof(T);
+    void* d = nullptr;
+    if (!cuda(cudaMalloc(&d, bytes))) return nullptr;
+    bufs_.push_back(d);
+    if (head < bytes && !cuda(cudaMemset((char*)d + head, 0, bytes - head))) return nullptr;
+    return (T*)d;
+  }
+  bool cuda(cudaError_t e) {   // only called while rc_ is PL_OK
+    if (e == cudaSuccess) return true;
+    cudaGetLastError();        // a failed call is not left for the next launch check to report
+    rc_ = PL_ERR_CUDA;
+    set_error("host staging: %s", cudaGetErrorString(e));
+    return false;
+  }
+  std::vector<void*> bufs_;
+  std::vector<Out> outs_;
+  int rc_ = PL_OK;
+};
 
 __device__ __forceinline__ int reflect101(int p, int n) {
   if (p < 0) p = -p;

@@ -163,16 +163,12 @@ extern "C" int pl_undistort_keypoints_dev(PLUndistort* h, const PLKeyPoint* kps,
 extern "C" int pl_undistort_keypoints(PLUndistort* h, const PLKeyPoint* kps, int n, PLKeyPoint* out) {
   PL_ARG(h && kps && out && n >= 0);
   if (n == 0) return PL_OK;
-  PLKeyPoint *di = nullptr, *dout = nullptr; int* dn = nullptr;
-  PL_CUDA(cudaMalloc((void**)&di, (size_t)n * 28)); PL_CUDA(cudaMalloc((void**)&dout, (size_t)n * 28)); PL_CUDA(cudaMalloc((void**)&dn, 4));
-  cudaMemcpy(di, kps, (size_t)n * 28, cudaMemcpyHostToDevice); cudaMemcpy(dn, &n, 4, cudaMemcpyHostToDevice);
-  int rc = pl_undistort_keypoints_dev(h, di, dn, n, 1, dout, h->stream);
-  cudaError_t e = cudaStreamSynchronize(h->stream);
-  if (rc == PL_OK && e == cudaSuccess) e = cudaMemcpy(out, dout, (size_t)n * 28, cudaMemcpyDeviceToHost);
-  cudaFree(di); cudaFree(dout); cudaFree(dn);
-  if (rc) return rc;
-  if (e != cudaSuccess) { set_error("pl_undistort_keypoints: %s", cudaGetErrorString(e)); return PL_ERR_CUDA; }
-  return PL_OK;
+  Staging s;
+  PLKeyPoint* di = s.in(kps, n); int* dn = s.in(&n, 1); PLKeyPoint* dout = s.out(out, n);
+  int rc;
+  if ((rc = s.status()) || (rc = s.sync()) || (rc = pl_undistort_keypoints_dev(h, di, dn, n, 1, dout, h->stream))) return rc;
+  PL_CUDA(cudaStreamSynchronize(h->stream));
+  return s.fetch();
 }
 // Frame::ComputeImageBounds: four corner points, host arithmetic (4 points)
 extern "C" int pl_frame_image_bounds(const float* K, const float* dist5, int width, int height, float* bounds) {
@@ -195,13 +191,6 @@ static int frustum_common(FrustumArgs& A, const float* Tcw, const float* Ow, con
   A.logScaleFactor = logSF; A.viewingCosLimit = cosLimit; A.nScaleLevels = nLevels; A.n = n;
   return require_device();
 }
-template <typename T> static T* upd(const T* h, size_t n, std::vector<void*>& fr) {
-  T* d = nullptr;
-  if (cudaMalloc((void**)&d, std::max<size_t>(n, 1) * sizeof(T)) != cudaSuccess) return nullptr;
-  fr.push_back(d);
-  if (h && n) cudaMemcpy(d, h, n * sizeof(T), cudaMemcpyHostToDevice);
-  return d;
-}
 extern "C" int pl_frame_is_in_frustum_points(const float* Tcw, const float* Ow, const float* K, const float* bounds,
                                              float log_scale_factor, int n_scale_levels, float viewing_cos_limit, int n,
                                              const float* pos, const float* normal, const float* min_dist, const float* max_dist,
@@ -209,22 +198,15 @@ extern "C" int pl_frame_is_in_frustum_points(const float* Tcw, const float* Ow, 
   FrustumArgs A;
   int rc = frustum_common(A, Tcw, Ow, K, bounds, log_scale_factor, n_scale_levels, viewing_cos_limit, n); if (rc) return rc;
   if (n == 0) return PL_OK;
-  std::vector<void*> fr;
-  float* dp = upd(pos, (size_t)n * 3, fr); float* dn = upd(normal, (size_t)n * 3, fr); float* dmin = upd(min_dist, n, fr); float* dmax = upd(max_dist, n, fr);
-  uint8_t* div = upd<uint8_t>(nullptr, n, fr); float* dpr = upd<float>(nullptr, (size_t)n * 2, fr); int* dl = upd<int>(nullptr, n, fr); float* dvc = upd<float>(nullptr, n, fr);
-  int ret = PL_ERR_CUDA;
-  if (dp && dn && dmin && dmax && div && dpr && dl && dvc) {
-    k_frustum_points<<<(n + 127) / 128, 128>>>(A, dp, dn, dmin, dmax, div, dpr, dl, dvc);
-    count_launch();
-    cudaError_t e = cudaDeviceSynchronize();
-    if (e == cudaSuccess) e = cudaMemcpy(inview, div, n, cudaMemcpyDeviceToHost);
-    if (e == cudaSuccess) e = cudaMemcpy(proj, dpr, (size_t)n * 8, cudaMemcpyDeviceToHost);
-    if (e == cudaSuccess) e = cudaMemcpy(level, dl, (size_t)n * 4, cudaMemcpyDeviceToHost);
-    if (e == cudaSuccess) e = cudaMemcpy(viewcos, dvc, (size_t)n * 4, cudaMemcpyDeviceToHost);
-    if (e == cudaSuccess) ret = PL_OK; else set_error("isInFrustum: %s", cudaGetErrorString(e));
-  } else set_error("isInFrustum: device allocation failed");
-  for (void* p : fr) cudaFree(p);
-  return ret;
+  PL_ARG(inview && proj && level && viewcos);
+  Staging s;
+  float* dp = s.in(pos, (size_t)n * 3); float* dn = s.in(normal, (size_t)n * 3); float* dmin = s.in(min_dist, n); float* dmax = s.in(max_dist, n);
+  uint8_t* div = s.out(inview, n); float* dpr = s.out(proj, (size_t)n * 2); int* dl = s.out(level, n); float* dvc = s.out(viewcos, n);
+  if ((rc = s.status())) return rc;
+  k_frustum_points<<<(n + 127) / 128, 128>>>(A, dp, dn, dmin, dmax, div, dpr, dl, dvc);
+  PL_LAUNCH_CHECK();
+  PL_CUDA(cudaDeviceSynchronize());
+  return s.fetch();
 }
 extern "C" int pl_frame_is_in_frustum_lines(const float* Tcw, const float* Ow, const float* K, const float* bounds,
                                             float log_scale_factor, float viewing_cos_limit, int n, const double* pos,
@@ -233,20 +215,13 @@ extern "C" int pl_frame_is_in_frustum_lines(const float* Tcw, const float* Ow, c
   FrustumArgs A;
   int rc = frustum_common(A, Tcw, Ow, K, bounds, log_scale_factor, 0, viewing_cos_limit, n); if (rc) return rc;
   if (n == 0) return PL_OK;
-  std::vector<void*> fr;
-  double* dp = upd(pos, (size_t)n * 6, fr); double* dn = upd(normal, (size_t)n * 3, fr); float* dmin = upd(min_dist, n, fr); float* dmax = upd(max_dist, n, fr);
-  uint8_t* div = upd<uint8_t>(nullptr, n, fr); float* dpr = upd<float>(nullptr, (size_t)n * 4, fr); int* dl = upd<int>(nullptr, n, fr); float* dvc = upd<float>(nullptr, n, fr);
-  int ret = PL_ERR_CUDA;
-  if (dp && dn && dmin && dmax && div && dpr && dl && dvc) {
-    k_frustum_lines<<<(n + 127) / 128, 128>>>(A, dp, dn, dmin, dmax, div, dpr, dl, dvc);
-    count_launch();
-    cudaError_t e = cudaDeviceSynchronize();
-    if (e == cudaSuccess) e = cudaMemcpy(inview, div, n, cudaMemcpyDeviceToHost);
-    if (e == cudaSuccess) e = cudaMemcpy(proj, dpr, (size_t)n * 16, cudaMemcpyDeviceToHost);
-    if (e == cudaSuccess) e = cudaMemcpy(level, dl, (size_t)n * 4, cudaMemcpyDeviceToHost);
-    if (e == cudaSuccess) e = cudaMemcpy(viewcos, dvc, (size_t)n * 4, cudaMemcpyDeviceToHost);
-    if (e == cudaSuccess) ret = PL_OK; else set_error("isInFrustum(lines): %s", cudaGetErrorString(e));
-  } else set_error("isInFrustum(lines): device allocation failed");
-  for (void* p : fr) cudaFree(p);
-  return ret;
+  PL_ARG(inview && proj && level && viewcos);
+  Staging s;
+  double* dp = s.in(pos, (size_t)n * 6); double* dn = s.in(normal, (size_t)n * 3); float* dmin = s.in(min_dist, n); float* dmax = s.in(max_dist, n);
+  uint8_t* div = s.out(inview, n); float* dpr = s.out(proj, (size_t)n * 4); int* dl = s.out(level, n); float* dvc = s.out(viewcos, n);
+  if ((rc = s.status())) return rc;
+  k_frustum_lines<<<(n + 127) / 128, 128>>>(A, dp, dn, dmin, dmax, div, dpr, dl, dvc);
+  PL_LAUNCH_CHECK();
+  PL_CUDA(cudaDeviceSynchronize());
+  return s.fetch();
 }

@@ -515,19 +515,16 @@ extern "C" int pl_global_ba(const PLBAProblem* p, int n_iterations, int robust, 
   blk_start.push_back((int)ent_a.size());
   std::vector<Ent>().swap(ents);
 
-  std::vector<void*> frees;
-  bool fail = false;
-  auto dalloc = [&](size_t bytes) -> void* { void* d = nullptr; if (cudaMalloc(&d, std::max<size_t>(bytes, 16)) != cudaSuccess) { fail = true; return nullptr; } frees.push_back(d); return d; };
-  auto up = [&](const void* h, size_t bytes) -> void* { void* d = dalloc(bytes); if (d && h && bytes) cudaMemcpy(d, h, bytes, cudaMemcpyHostToDevice); return d; };
-  auto upv = [&](const std::vector<int>& v) -> const int* { return (const int*)up(v.data(), 4 * v.size()); };
+  Staging s;
+  auto upv = [&](const std::vector<int>& v) { return s.in(v.data(), v.size()); };
   G A;
   A.n_kf = n_kf; A.n_pt = n_pt; A.n_ln = n_ln; A.n_pe = n_pe; A.n_le = std::max(n_le, 1); A.n_lm = n_lm; A.n_edges = n_edges;
   A.np = np; A.nl = nl; A.n = n; A.npad = npad; A.n_plb = n_plb; A.n_blk = n_blk;
-  A.kf_Tcw = (const float*)up(p->kf_Tcw, 64 * (size_t)n_kf); A.kf_K = (const float*)up(p->kf_K, 16 * (size_t)n_kf);
-  A.pt_Xw = (const float*)up(p->pt_Xw, 12 * (size_t)n_pt); A.ln_Xw = (const double*)up(p->ln_Xw, 48 * (size_t)n_ln);
+  A.kf_Tcw = s.in(p->kf_Tcw, 16 * (size_t)n_kf); A.kf_K = s.in(p->kf_K, 4 * (size_t)n_kf);
+  A.pt_Xw = s.in(p->pt_Xw, 3 * (size_t)n_pt); A.ln_Xw = s.in(p->ln_Xw, 6 * (size_t)n_ln);
   A.ed_kf = upv(ed_kf); A.ed_lm = upv(ed_lm);
-  A.pe_obs = (const float*)up(p->pe_obs, 8 * (size_t)n_pe); A.pe_w = (const float*)up(p->pe_inv_sigma2, 4 * (size_t)n_pe);
-  A.le_f = (const double*)up(p->le_func, 24 * (size_t)n_le);
+  A.pe_obs = s.in(p->pe_obs, 2 * (size_t)n_pe); A.pe_w = s.in(p->pe_inv_sigma2, (size_t)n_pe);
+  A.le_f = s.in(p->le_func, 3 * (size_t)n_le);
   A.lm_start = upv(lm_start); A.lm_edges = upv(lm_edges); A.kf_start = upv(kf_start); A.kf_edges = upv(kf_edges);
   A.pose_slot = upv(pose_slot); A.lm_slot = upv(lm_slot);
   if (plb_edges.empty()) plb_edges.push_back(0);
@@ -537,22 +534,24 @@ extern "C" int pl_global_ba(const PLBAProblem* p, int n_iterations, int robust, 
   A.plb_start = upv(plb_start); A.plb_edges = upv(plb_edges); A.plb_pose = upv(plb_pose); A.plb_lm = upv(plb_lm);
   A.lm_plb_start = upv(lm_plb_start); A.pose_plb_start = upv(pose_plb_start); A.pose_plb = upv(pose_plb);
   A.blk_start = upv(blk_start); A.blk_row = upv(blk_row); A.blk_col = upv(blk_col); A.ent_a = upv(ent_a); A.ent_b = upv(ent_b);
-  A.T = (SE3*)dalloc(sizeof(SE3) * n_kf); SE3* Tb = (SE3*)dalloc(sizeof(SE3) * n_kf);
-  A.Tp = (SE3*)dalloc(sizeof(SE3) * n_kf * 6); A.Tm = (SE3*)dalloc(sizeof(SE3) * n_kf * 6);
-  A.X = (double*)dalloc(24 * (size_t)n_lm); double* Xb = (double*)dalloc(24 * (size_t)n_lm);
-  A.err = (double*)dalloc(16 * (size_t)n_edges); A.JA = (double*)dalloc(48 * (size_t)n_edges); A.JB = (double*)dalloc(96 * (size_t)n_edges);
-  A.omr = (double*)dalloc(16 * (size_t)n_edges); A.wgt = (double*)dalloc(8 * (size_t)n_edges);
-  A.W = (double*)dalloc(144 * (size_t)std::max(n_plb, 1)); A.WD = (double*)dalloc(144 * (size_t)std::max(n_plb, 1));
-  A.Hpp = (double*)dalloc(288 * (size_t)std::max(np, 1)); A.bp = (double*)dalloc(48 * (size_t)std::max(np, 1));
-  A.Hll = (double*)dalloc(72 * (size_t)std::max(nl, 1)); A.bl = (double*)dalloc(24 * (size_t)std::max(nl, 1));
-  A.Dinv = (double*)dalloc(72 * (size_t)std::max(nl, 1)); A.Dinvb = (double*)dalloc(24 * (size_t)std::max(nl, 1));
-  A.Hs = (double*)dalloc(8 * (size_t)npad * npad); A.bs = (double*)dalloc(8 * (size_t)npad);
-  A.x = (double*)dalloc(8 * ((size_t)n + 3 * (size_t)nl + 8));
-  A.part = (double*)dalloc(8 * RED_BLOCKS); A.scal = (double*)dalloc(64); A.flag = (int*)dalloc(4);
-  float* d_kf_out = (float*)dalloc(64 * (size_t)n_kf); float* d_pt_out = (float*)dalloc(12 * (size_t)n_pt); double* d_ln_out = (double*)dalloc(48 * (size_t)n_ln);
+  A.T = s.out<SE3>(n_kf); SE3* Tb = s.out<SE3>(n_kf);
+  A.Tp = s.out<SE3>((size_t)n_kf * 6); A.Tm = s.out<SE3>((size_t)n_kf * 6);
+  A.X = s.out<double>(3 * (size_t)n_lm); double* Xb = s.out<double>(3 * (size_t)n_lm);
+  A.err = s.out<double>(2 * (size_t)n_edges); A.JA = s.out<double>(6 * (size_t)n_edges); A.JB = s.out<double>(12 * (size_t)n_edges);
+  A.omr = s.out<double>(2 * (size_t)n_edges); A.wgt = s.out<double>(n_edges);
+  A.W = s.out<double>(18 * (size_t)std::max(n_plb, 1)); A.WD = s.out<double>(18 * (size_t)std::max(n_plb, 1));
+  A.Hpp = s.out<double>(36 * (size_t)std::max(np, 1)); A.bp = s.out<double>(6 * (size_t)std::max(np, 1));
+  A.Hll = s.out<double>(9 * (size_t)std::max(nl, 1)); A.bl = s.out<double>(3 * (size_t)std::max(nl, 1));
+  A.Dinv = s.out<double>(9 * (size_t)std::max(nl, 1)); A.Dinvb = s.out<double>(3 * (size_t)std::max(nl, 1));
+  A.Hs = s.out<double>((size_t)npad * npad); A.bs = s.out<double>(npad);
+  A.x = s.out<double>((size_t)n + 3 * (size_t)nl + 8);
+  A.part = s.out<double>(RED_BLOCKS); A.scal = s.out<double>(8); A.flag = s.out<int>(1);
+  float* d_kf_out = s.out(kf_Tcw_out, 16 * (size_t)n_kf);
+  float* d_pt_out = pt_Xw_out ? s.out(pt_Xw_out, 3 * (size_t)n_pt) : s.out<float>(3 * (size_t)n_pt);
+  double* d_ln_out = ln_Xw_out ? s.out(ln_Xw_out, 6 * (size_t)n_ln) : s.out<double>(6 * (size_t)n_ln);
   A.robust = robust ? 1 : 0; A.info_line = 1.0;
   A.delta_p = (double)(float)std::sqrt(5.99); A.delta_l = (double)(float)std::sqrt(3.84);
-  int ret = PL_OK, done = 0;
+  int ret = s.status(), done = 0;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   auto terminate = [&]() { return stop_flag_host && *(volatile const int*)stop_flag_host; };
   auto sum_to = [&](int slot, int is_max) { k_gba_reduce<<<1, 1>>>(A, slot, is_max); count_launch(); };
@@ -560,8 +559,7 @@ extern "C" int pl_global_ba(const PLBAProblem* p, int n_iterations, int robust, 
     k_gba_errors<<<RED_BLOCKS, RED_THREADS>>>(A); sum_to(0, 0); count_launch();
     return cudaMemcpy(&out, A.scal, 8, cudaMemcpyDeviceToHost);
   };
-  if (fail) { set_error("global BA: device allocation failed (reduced system %d x %d)", npad, npad); ret = PL_ERR_CUDA; }
-  else {
+  if (ret == PL_OK) {
     cudaError_t e = cudaSuccess;
     cudaEventCreate(&ev0); cudaEventCreate(&ev1);
     cudaEventRecord(ev0, 0);
@@ -647,15 +645,12 @@ extern "C" int pl_global_ba(const PLBAProblem* p, int n_iterations, int robust, 
       e = cudaGetLastError();
     }
     if (e == cudaSuccess) e = cudaDeviceSynchronize();
-    if (e == cudaSuccess) e = cudaMemcpy(kf_Tcw_out, d_kf_out, 64 * (size_t)n_kf, cudaMemcpyDeviceToHost);
-    if (e == cudaSuccess && n_pt && pt_Xw_out) e = cudaMemcpy(pt_Xw_out, d_pt_out, 12 * (size_t)n_pt, cudaMemcpyDeviceToHost);
-    if (e == cudaSuccess && n_ln && ln_Xw_out) e = cudaMemcpy(ln_Xw_out, d_ln_out, 48 * (size_t)n_ln, cudaMemcpyDeviceToHost);
     if (e == cudaSuccess && solve_ms) cudaEventElapsedTime(solve_ms, ev0, ev1);
     if (e != cudaSuccess) { set_error("global BA: %s", cudaGetErrorString(e)); ret = PL_ERR_CUDA; }
+    else ret = s.fetch();
     if (ev0) cudaEventDestroy(ev0);
     if (ev1) cudaEventDestroy(ev1);
   }
   if (iterations) *iterations = done;
-  for (void* d : frees) cudaFree(d);
   return ret;
 }

@@ -342,41 +342,21 @@ extern "C" int pl_pose_optimization(int mode, const float* Tcw_in, const float* 
   PL_ARG(Tcw_in && K && Tcw_out && n_points >= 0 && n_lines >= 0);
   int rc = require_device(); if (rc) return rc;
   const int cp = std::max(n_points, 1), cl = std::max(n_lines, 1);
-  std::vector<void*> frees;
-  auto up = [&](const void* h, size_t bytes, size_t alloc_bytes) -> void* {
-    void* d = nullptr;
-    if (cudaMalloc(&d, std::max<size_t>(alloc_bytes, 8)) != cudaSuccess) return nullptr;
-    frees.push_back(d);
-    if (h && bytes) cudaMemcpy(d, h, bytes, cudaMemcpyHostToDevice);
-    return d;
-  };
-  float* dT = (float*)up(Tcw_in, 64, 64); float* dK = (float*)up(K, 16, 16);
-  int* dnp = (int*)up(&n_points, 4, 4); int* dnl = (int*)up(&n_lines, 4, 4);
-  float* dobs = (float*)up(pt_obs, (size_t)n_points * 8, (size_t)cp * 8);
-  float* dw = (float*)up(pt_inv_sigma2, (size_t)n_points * 4, (size_t)cp * 4);
-  float* dX = (float*)up(pt_Xw, (size_t)n_points * 12, (size_t)cp * 12);
-  double* dlf = (double*)up(line_func, (size_t)n_lines * 24, (size_t)cl * 24);
-  double* dlX = (double*)up(line_Xw, (size_t)n_lines * 48, (size_t)cl * 48);
-  float* dTo = (float*)up(nullptr, 0, 64);
-  uint8_t* dpo = (uint8_t*)up(nullptr, 0, cp); uint8_t* dlo = (uint8_t*)up(nullptr, 0, cl);
-  int* dinl = (int*)up(nullptr, 0, 4); int* dits = (int*)up(nullptr, 0, 4);
-  double* scr = (double*)up(nullptr, 0, pl_pose_optimization_scratch_doubles(1, cp, cl) * 8);
-  int ret = PL_ERR_CUDA;
-  if (dT && dK && dnp && dnl && dobs && dw && dX && dlf && dlX && dTo && dpo && dlo && dinl && dits && scr) {
-    ret = pl_pose_optimization_dev(mode, 1, dT, dK, dnp, cp, dobs, dw, dX, dnl, cl, dlf, dlX, dTo, dpo, dlo, dinl, dits, scr, nullptr);
-    if (ret == PL_OK) {
-      int inl = 0, its = 0;
-      cudaError_t e = cudaMemcpy(Tcw_out, dTo, 64, cudaMemcpyDeviceToHost);
-      // the kernel writes only the masks of the edges the mode optimises (mode 1: points, mode 2: lines); the other one is the
-      // caller's and stays untouched, as the reference leaves mvbLineOutlier / mvbOutlier alone in those modes
-      if (e == cudaSuccess && mode != 2 && n_points && pt_outlier) e = cudaMemcpy(pt_outlier, dpo, n_points, cudaMemcpyDeviceToHost);
-      if (e == cudaSuccess && mode != 1 && n_lines && line_outlier) e = cudaMemcpy(line_outlier, dlo, n_lines, cudaMemcpyDeviceToHost);
-      if (e == cudaSuccess) e = cudaMemcpy(&inl, dinl, 4, cudaMemcpyDeviceToHost);
-      if (e == cudaSuccess) e = cudaMemcpy(&its, dits, 4, cudaMemcpyDeviceToHost);
-      if (e != cudaSuccess) { set_error("pose optimisation: %s", cudaGetErrorString(e)); ret = PL_ERR_CUDA; }
-      else { ret = inl; if (iterations) *iterations = its; }
-    }
-  } else set_error("pose optimisation: device allocation failed");
-  for (void* p : frees) cudaFree(p);
-  return ret;
+  Staging s;
+  float* dT = s.in(Tcw_in, 16); float* dK = s.in(K, 4); int* dnp = s.in(&n_points, 1); int* dnl = s.in(&n_lines, 1);
+  float* dobs = s.in(pt_obs, (size_t)n_points * 2); float* dw = s.in(pt_inv_sigma2, n_points); float* dX = s.in(pt_Xw, (size_t)n_points * 3);
+  double* dlf = s.in(line_func, (size_t)n_lines * 3); double* dlX = s.in(line_Xw, (size_t)n_lines * 6);
+  int inl = 0, its = 0;
+  float* dTo = s.out(Tcw_out, 16); int* dinl = s.out(&inl, 1); int* dits = s.out(&its, 1);
+  // the kernel writes only the masks of the edges the mode optimises (mode 1: points, mode 2: lines); the other one is the
+  // caller's and stays untouched, as the reference leaves mvbLineOutlier / mvbOutlier alone in those modes
+  uint8_t* dpo = mode != 2 && pt_outlier ? s.out(pt_outlier, n_points, cp) : s.out<uint8_t>(cp);
+  uint8_t* dlo = mode != 1 && line_outlier ? s.out(line_outlier, n_lines, cl) : s.out<uint8_t>(cl);
+  double* scr = s.out<double>(pl_pose_optimization_scratch_doubles(1, cp, cl));
+  if ((rc = s.status()) ||
+      (rc = pl_pose_optimization_dev(mode, 1, dT, dK, dnp, cp, dobs, dw, dX, dnl, cl, dlf, dlX, dTo, dpo, dlo, dinl, dits, scr, nullptr)) ||
+      (rc = s.fetch()))
+    return rc;
+  if (iterations) *iterations = its;
+  return inl;
 }

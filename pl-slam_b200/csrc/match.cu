@@ -1036,41 +1036,19 @@ __global__ void __launch_bounds__(128) k_lsd_fuse_search(LineFuseArgs A) {
   A.best_idx[i] = bestIdx; A.best_dist[i] = bestDist;
 }
 
-namespace {
-struct Stage {  // tiny RAII helper for the host-pointer wrappers
-  std::vector<void*> ptrs;
-  ~Stage() { for (void* p : ptrs) cudaFree(p); }
-  template <typename T> T* up(const T* h, size_t n) {
-    T* d = nullptr;
-    if (cudaMalloc((void**)&d, std::max<size_t>(n, 1) * sizeof(T)) != cudaSuccess) return nullptr;
-    ptrs.push_back(d);
-    if (h && n) cudaMemcpy(d, h, n * sizeof(T), cudaMemcpyHostToDevice);
-    return d;
-  }
-  template <typename T> T* alloc(size_t n) { return up<T>(nullptr, n); }
-};
-template <typename T> int down(T* h, const T* d, size_t n) {
-  PL_CUDA(cudaMemcpy(h, d, n * sizeof(T), cudaMemcpyDeviceToHost));
-  return PL_OK;
-}
-}  // namespace
-
 extern "C" int pl_descriptor_distance_batch(const uint8_t* a, const uint8_t* b, int n, int* out) {
   // convenience for tests: n independent 32-byte pairs, host pointers
   PL_ARG(a && b && out && n >= 0);
   int rc = require_device(); if (rc) return rc;
-  Stage s;
-  uint8_t* da = s.up(a, (size_t)n * 32); uint8_t* db = s.up(b, (size_t)n * 32);
-  int one = 1; (void)one;
-  std::vector<int> n1(1, n);
+  Staging s;
+  uint8_t* da = s.in(a, (size_t)n * 32); uint8_t* db = s.in(b, (size_t)n * 32);
   // reuse k_bf_knn2 with cap2 = 1 per pair would be wasteful; do pairs as n batches of 1x1
-  std::vector<int> ones(n, 1);
-  int* dn = s.up(ones.data(), (size_t)n);
-  int* idx = s.alloc<int>((size_t)n * 2); int* dist = s.alloc<int>((size_t)n * 2);
-  PL_ARG(da && db && dn && idx && dist);
+  std::vector<int> ones(n, 1), hd((size_t)n * 2);
+  int* dn = s.in(ones.data(), (size_t)n);
+  int* idx = s.out<int>((size_t)n * 2); int* dist = s.out(hd.data(), (size_t)n * 2);
+  if ((rc = s.status())) return rc;
   if (n) { k_bf_knn2<<<dim3(1, n), 128>>>(da, dn, db, dn, 1, 1, idx, dist); PL_LAUNCH_CHECK(); }
-  std::vector<int> hd((size_t)n * 2);
-  rc = down(hd.data(), dist, (size_t)n * 2); if (rc) return rc;
+  if ((rc = s.fetch())) return rc;
   for (int i = 0; i < n; i++) out[i] = hd[2 * i];
   return PL_OK;
 }
@@ -1086,14 +1064,12 @@ extern "C" int pl_frame_assign_grid(const PLKeyPoint* keys, int n, const float* 
                                     int* cell_items) {
   PL_ARG(keys && bounds && cell_start && cell_items && n >= 0 && n < 65535);
   int rc = require_device(); if (rc) return rc;
-  Stage s;
+  Staging s;
   int cap = std::max(n, 1);
-  PLKeyPoint* dk = s.up(keys, (size_t)n); int* dn = s.up(&n, 1); float* db = s.up(bounds, 4);
-  int* ds = s.alloc<int>(NCELL + 1); int* di = s.alloc<int>(cap);
-  PL_ARG(dk && dn && db && ds && di);
-  rc = pl_frame_assign_grid_dev(dk, dn, cap, 1, db, ds, di, nullptr); if (rc) return rc;
-  rc = down(cell_start, ds, NCELL + 1); if (rc) return rc;
-  return down(cell_items, di, (size_t)n);
+  PLKeyPoint* dk = s.in(keys, (size_t)n); int* dn = s.in(&n, 1); float* db = s.in(bounds, 4);
+  int* ds = s.out(cell_start, NCELL + 1); int* di = s.out(cell_items, (size_t)n, cap);
+  if ((rc = s.status()) || (rc = pl_frame_assign_grid_dev(dk, dn, cap, 1, db, ds, di, nullptr))) return rc;
+  return s.fetch();
 }
 
 extern "C" int pl_orb_search_for_initialization_dev(const PLKeyPoint* keys1, const uint8_t* desc1, const int* n1,
@@ -1118,24 +1094,19 @@ extern "C" int pl_orb_search_for_initialization(const PLKeyPoint* keys1, const u
                                                 int window_size, float nnratio, int check_orientation) {
   PL_ARG(keys1 && desc1 && keys2 && desc2 && bounds && prev_matched && matches12 && n1 >= 0 && n2 >= 0);
   int rc = require_device(); if (rc) return rc;
-  Stage s;
-  int cap = std::max(std::max(n1, n2), 1);
-  std::vector<PLKeyPoint> k1(cap), k2(cap);
-  std::vector<uint8_t> d1((size_t)cap * 32), d2((size_t)cap * 32);
-  std::vector<float> pm((size_t)cap * 2, 0.f);
-  if (n1) { memcpy(k1.data(), keys1, n1 * sizeof(PLKeyPoint)); memcpy(d1.data(), desc1, (size_t)n1 * 32); memcpy(pm.data(), prev_matched, (size_t)n1 * 8); }
-  if (n2) { memcpy(k2.data(), keys2, n2 * sizeof(PLKeyPoint)); memcpy(d2.data(), desc2, (size_t)n2 * 32); }
-  PLKeyPoint* dk1 = s.up(k1.data(), cap); PLKeyPoint* dk2 = s.up(k2.data(), cap);
-  uint8_t* dd1 = s.up(d1.data(), d1.size()); uint8_t* dd2 = s.up(d2.data(), d2.size());
-  int* dn1 = s.up(&n1, 1); int* dn2 = s.up(&n2, 1); float* db = s.up(bounds, 4); float* dpm = s.up(pm.data(), pm.size());
-  int* dm = s.alloc<int>(cap); int* dnm = s.alloc<int>(1); int* scr = s.alloc<int>((size_t)2 * cap);
-  PL_ARG(dk1 && dk2 && dd1 && dd2 && dn1 && dn2 && db && dpm && dm && dnm && scr);
-  rc = pl_orb_search_for_initialization_dev(dk1, dd1, dn1, dk2, dd2, dn2, cap, 1, db, dpm, dm, dnm, window_size, nnratio,
-                                            check_orientation, scr, nullptr);
-  if (rc) return rc;
+  Staging s;
+  const size_t cap = std::max(std::max(n1, n2), 1);
+  PLKeyPoint* dk1 = s.in(keys1, n1, cap); PLKeyPoint* dk2 = s.in(keys2, n2, cap);
+  uint8_t* dd1 = s.in(desc1, (size_t)n1 * 32, cap * 32); uint8_t* dd2 = s.in(desc2, (size_t)n2 * 32, cap * 32);
+  int* dn1 = s.in(&n1, 1); int* dn2 = s.in(&n2, 1); float* db = s.in(bounds, 4);
+  float* dpm = s.in(prev_matched, (size_t)n1 * 2, cap * 2);
   int nm = 0;
-  rc = down(&nm, dnm, 1); if (rc) return rc;
-  if (n1) { rc = down(matches12, dm, (size_t)n1); if (rc) return rc; rc = down(prev_matched, dpm, (size_t)n1 * 2); if (rc) return rc; }
+  int* dm = s.out(matches12, n1, cap); int* dnm = s.out(&nm, 1); int* scr = s.out<int>(2 * cap);
+  if ((rc = s.status()) ||
+      (rc = pl_orb_search_for_initialization_dev(dk1, dd1, dn1, dk2, dd2, dn2, (int)cap, 1, db, dpm, dm, dnm, window_size, nnratio,
+                                                 check_orientation, scr, nullptr)) ||
+      (rc = s.fetch()) || (rc = s.down(prev_matched, dpm, (size_t)n1 * 2)))
+    return rc;
   return nm;
 }
 
@@ -1148,26 +1119,20 @@ extern "C" int pl_orb_search_by_projection_last(const PLKeyPoint* keys_cur, cons
                                                 const uint8_t* cur_preassigned, int* cur_match) {
   PL_ARG(keys_cur && desc_cur && bounds && Tcw && K && scale_factors && cur_match && n_cur >= 0 && n_cur <= 6144 && n_last >= 0);
   int rc = require_device(); if (rc) return rc;
-  Stage s;
+  Staging s;
   const int cap = std::max(n_cur, 1), capl = std::max(n_last, 1);
-  ProjLastArgs A;
-  A.keys = s.up(keys_cur, n_cur); A.desc = s.up(desc_cur, (size_t)n_cur * 32); A.n = s.up(&n_cur, 1); A.cap = cap;
-  A.bounds = s.up(bounds, 4); A.Tcw = s.up(Tcw, 16); A.K = s.up(K, 4); A.scaleFactors = s.up(scale_factors, nlevels);
-  A.nlevels = nlevels; A.n_last = s.up(&n_last, 1); A.cap_last = capl;
-  A.last_valid = s.up(last_valid, n_last); A.last_pos = s.up(last_pos, (size_t)n_last * 3);
-  A.last_desc = s.up(last_desc, (size_t)n_last * 32); A.last_octave = s.up(last_octave, n_last);
-  A.last_angle = s.up(last_angle, n_last);
-  A.th = th; A.checkOri = check_orientation;
-  A.preassigned = cur_preassigned ? s.up(cur_preassigned, n_cur) : nullptr;
-  A.match = s.alloc<int>(cap); A.nmatches = s.alloc<int>(1);
-  PL_ARG(A.keys && A.desc && A.match && A.nmatches && A.last_pos && A.last_desc);
-  size_t sm = grid_smem_bytes(cap);
-  PL_CUDA(cudaFuncSetAttribute(k_search_proj_last, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
-  k_search_proj_last<<<1, 32, sm>>>(A);
-  PL_LAUNCH_CHECK();
+  PLKeyPoint* dk = s.in(keys_cur, n_cur); uint8_t* dd = s.in(desc_cur, (size_t)n_cur * 32); int* dn = s.in(&n_cur, 1);
+  float* db = s.in(bounds, 4); float* dT = s.in(Tcw, 16); float* dK = s.in(K, 4); float* dsf = s.in(scale_factors, nlevels);
+  int* dnl = s.in(&n_last, 1); uint8_t* dv = s.in(last_valid, n_last); float* dp = s.in(last_pos, (size_t)n_last * 3);
+  uint8_t* dld = s.in(last_desc, (size_t)n_last * 32); int* dlo = s.in(last_octave, n_last); float* dla = s.in(last_angle, n_last);
+  uint8_t* dpre = cur_preassigned ? s.in(cur_preassigned, n_cur) : nullptr;
   int nm = 0;
-  rc = down(&nm, A.nmatches, 1); if (rc) return rc;
-  if (n_cur) { rc = down(cur_match, A.match, (size_t)n_cur); if (rc) return rc; }
+  int* dm = s.out(cur_match, n_cur, cap); int* dnm = s.out(&nm, 1);
+  if ((rc = s.status()) ||
+      (rc = search_by_projection_last_launch(dk, dd, dn, cap, 1, db, dT, dK, dsf, nlevels, dnl, capl, dv, dp, dld, nullptr, dlo, dla, th,
+                                             check_orientation, dpre, nullptr, 0, dm, dnm, nullptr)) ||
+      (rc = s.fetch()))
+    return rc;
   return nm;
 }
 
@@ -1178,23 +1143,20 @@ extern "C" int pl_orb_search_by_projection_points(const PLKeyPoint* keys, const 
                                                   float th, float nnratio, const uint8_t* preassigned, int* match) {
   PL_ARG(keys && desc && bounds && scale_factors && match && n >= 0 && n_mp >= 0);
   int rc = require_device(); if (rc) return rc;
-  Stage s;
+  Staging s;
   const int cap = std::max(n, 1), capm = std::max(n_mp, 1);
-  ProjPointsArgs A{};
-  A.keys = s.up(keys, n); A.desc = s.up(desc, (size_t)n * 32); A.n = s.up(&n, 1); A.cap = cap;
-  A.bounds = s.up(bounds, 4); A.scaleFactors = s.up(scale_factors, nlevels);
-  A.n_mp = s.up(&n_mp, 1); A.cap_mp = capm; A.in_view = s.up(in_view, n_mp); A.proj = s.up(proj, (size_t)n_mp * 2);
-  A.level = s.up(level, n_mp); A.view_cos = s.up(view_cos, n_mp); A.mp_desc = s.up(mp_desc, (size_t)n_mp * 32);
-  A.th = th; A.nnratio = nnratio; A.preassigned = preassigned ? s.up(preassigned, n) : nullptr;
-  A.match = s.alloc<int>(cap); A.nmatches = s.alloc<int>(1);
-  PL_ARG(A.keys && A.desc && A.match && A.nmatches);
-  size_t sm = grid_smem_bytes(cap);
-  PL_CUDA(cudaFuncSetAttribute(k_search_proj_points, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
-  k_search_proj_points<<<1, 32, sm>>>(A);
-  PL_LAUNCH_CHECK();
+  PLKeyPoint* dk = s.in(keys, n); uint8_t* dd = s.in(desc, (size_t)n * 32); int* dn = s.in(&n, 1);
+  float* db = s.in(bounds, 4); float* dsf = s.in(scale_factors, nlevels);
+  int* dnm_in = s.in(&n_mp, 1); uint8_t* dv = s.in(in_view, n_mp); float* dp = s.in(proj, (size_t)n_mp * 2);
+  int* dl = s.in(level, n_mp); float* dvc = s.in(view_cos, n_mp); uint8_t* dmd = s.in(mp_desc, (size_t)n_mp * 32);
+  uint8_t* dpre = preassigned ? s.in(preassigned, n) : nullptr;
   int nm = 0;
-  rc = down(&nm, A.nmatches, 1); if (rc) return rc;
-  if (n) { rc = down(match, A.match, (size_t)n); if (rc) return rc; }
+  int* dm = s.out(match, n, cap); int* dnm = s.out(&nm, 1);
+  if ((rc = s.status()) ||
+      (rc = search_by_projection_points_launch(dk, dd, dn, cap, 1, db, dsf, dnm_in, capm, dv, dp, dl, dvc, dmd, th, nullptr, nullptr,
+                                               nnratio, dpre, dm, dnm, nullptr)) ||
+      (rc = s.fetch()))
+    return rc;
   return nm;
 }
 
@@ -1262,15 +1224,14 @@ extern "C" int pl_match_bf_knn2(const uint8_t* d1, int n1, const uint8_t* d2, in
   PL_ARG(d1 && d2 && idx && dist && n1 >= 0 && n2 >= 0);
   int rc = require_device(); if (rc) return rc;
   if (n1 == 0) return PL_OK;
-  Stage s;
-  uint8_t* a = s.up(d1, (size_t)n1 * 32); uint8_t* b = s.up(d2, (size_t)std::max(n2, 1) * 32);
-  int* dn1 = s.up(&n1, 1); int* dn2 = s.up(&n2, 1);
-  int* di = s.alloc<int>((size_t)n1 * 2); int* dd = s.alloc<int>((size_t)n1 * 2);
-  PL_ARG(a && b && dn1 && dn2 && di && dd);
+  Staging s;
+  uint8_t* a = s.in(d1, (size_t)n1 * 32); uint8_t* b = s.in(d2, (size_t)n2 * 32, 32);
+  int* dn1 = s.in(&n1, 1); int* dn2 = s.in(&n2, 1);
+  int* di = s.out(idx, (size_t)n1 * 2); int* dd = s.out(dist, (size_t)n1 * 2);
+  if ((rc = s.status())) return rc;
   k_bf_knn2<<<dim3((n1 + 3) / 4, 1), 128>>>(a, dn1, b, dn2, n1, std::max(n2, 1), di, dd);
   PL_LAUNCH_CHECK();
-  rc = down(idx, di, (size_t)n1 * 2); if (rc) return rc;
-  return down(dist, dd, (size_t)n1 * 2);
+  return s.fetch();
 }
 
 extern "C" int pl_lsd_search_double_dev(const uint8_t* d1, const int* n1, const uint8_t* d2, const int* n2, int cap1,
@@ -1289,18 +1250,15 @@ static int search_double_host(const uint8_t* d1, int n1, const uint8_t* d2, int 
                               int* matches) {
   PL_ARG(d1 && d2 && matches && n1 >= 0 && n2 >= 0);
   int rc = require_device(); if (rc) return rc;
-  Stage s;
+  Staging s;
   const int c1 = std::max(n1, 1), c2 = std::max(n2, 1);
-  uint8_t* a = s.up(d1, (size_t)n1 * 32); uint8_t* b = s.up(d2, (size_t)n2 * 32);
-  if (n1 == 0) a = s.alloc<uint8_t>(32);
-  if (n2 == 0) b = s.alloc<uint8_t>(32);
-  int* dn1 = s.up(&n1, 1); int* dn2 = s.up(&n2, 1);
-  int* dm = s.alloc<int>(c1); int* dnm = s.alloc<int>(1);
-  PL_ARG(a && b && dn1 && dn2 && dm && dnm);
-  rc = pl_lsd_search_double_dev(a, dn1, b, dn2, c1, c2, 1, th, nnratio, mutual, dm, dnm, nullptr); if (rc) return rc;
+  uint8_t* a = s.in(d1, (size_t)n1 * 32, 32); uint8_t* b = s.in(d2, (size_t)n2 * 32, 32);
+  int* dn1 = s.in(&n1, 1); int* dn2 = s.in(&n2, 1);
   int nm = 0;
-  rc = down(&nm, dnm, 1); if (rc) return rc;
-  if (n1) { rc = down(matches, dm, (size_t)n1); if (rc) return rc; }
+  int* dm = s.out(matches, n1, c1); int* dnm = s.out(&nm, 1);
+  if ((rc = s.status()) || (rc = pl_lsd_search_double_dev(a, dn1, b, dn2, c1, c2, 1, th, nnratio, mutual, dm, dnm, nullptr)) ||
+      (rc = s.fetch()))
+    return rc;
   return nm;
 }
 extern "C" int pl_lsd_frame_bf_match(const uint8_t* d1, int n1, const uint8_t* d2, int n2, float th, float nnratio,
@@ -1346,47 +1304,43 @@ __global__ void __launch_bounds__(32) k_line_grid(const KeyLine68* kl, int n, co
 extern "C" int pl_frame_assign_grid_lines(const void* keylines_un, int n, const float* bounds, int* cell_start, int* cell_items, int cap_items) {
   PL_ARG(keylines_un && bounds && cell_start && cell_items && n >= 0 && n < 60000);
   int rc = require_device(); if (rc) return rc;
-  Stage s;
+  Staging s;
   const int cap = std::max(n, 1);
-  KeyLine68* dk = (KeyLine68*)s.up((const uint8_t*)keylines_un, (size_t)n * 68);
-  float* db = s.up(bounds, 4);
-  int* ds = s.alloc<int>(NCELL + 1); unsigned short* di = s.alloc<unsigned short>((size_t)cap * kMaxPath);
-  unsigned short* dp = s.alloc<unsigned short>((size_t)cap * kMaxPath); unsigned short* dl = s.alloc<unsigned short>(cap);
-  PL_ARG(dk && db && ds && di && dp && dl);
+  KeyLine68* dk = (KeyLine68*)s.in((const uint8_t*)keylines_un, (size_t)n * 68);
+  float* db = s.in(bounds, 4);
+  int* ds = s.out(cell_start, NCELL + 1); unsigned short* di = s.out<unsigned short>((size_t)cap * kMaxPath);
+  unsigned short* dp = s.out<unsigned short>((size_t)cap * kMaxPath); unsigned short* dl = s.out<unsigned short>(cap);
+  if ((rc = s.status())) return rc;
   k_line_grid<<<1, 32>>>(dk, n, db, ds, di, dp, dl);
   PL_LAUNCH_CHECK();
-  rc = down(cell_start, ds, NCELL + 1); if (rc) return rc;
+  if ((rc = s.fetch())) return rc;
   const int tot = cell_start[NCELL];
   std::vector<unsigned short> tmp(std::max(tot, 1));
-  rc = down(tmp.data(), di, (size_t)tot); if (rc) return rc;
+  if ((rc = s.down(tmp.data(), di, (size_t)tot))) return rc;
   for (int i = 0; i < tot && i < cap_items; i++) cell_items[i] = tmp[i];
   return tot;
 }
 
 static int line_search_host(int variant, const void* kls, const double* lfunc, const uint8_t* desc, int n, const float* bounds,
-                            int n_q, const uint8_t* q_valid, const float* q_proj, const uint8_t* q_desc, const float* q_length,
-                            const float* q_view_cos, float th, float nnratio, const uint8_t* preassigned, int* match) {
+                            int n_q, const uint8_t* q_valid, const float* q_proj, const uint8_t* q_desc,
+                            const float* q_length_or_view_cos, float th, float nnratio, const uint8_t* preassigned, int* match) {
   PL_ARG(kls && lfunc && desc && bounds && match && n >= 0 && n < 60000 && n_q >= 0);
   int rc = require_device(); if (rc) return rc;
-  Stage s;
+  Staging s;
   const int cap = std::max(n, 1), capq = std::max(n_q, 1);
-  LineSearchArgs A{};
-  A.kl = (const KeyLine68*)s.up((const uint8_t*)kls, (size_t)n * 68); A.lfunc = s.up(lfunc, (size_t)n * 3); A.desc = s.up(desc, (size_t)n * 32);
-  A.n = s.up(&n, 1); A.cap = cap; A.bounds = s.up(bounds, 4);
-  A.n_q = s.up(&n_q, 1); A.cap_q = capq; A.q_valid = s.up(q_valid, n_q); A.q_proj = s.up(q_proj, (size_t)n_q * 4);
-  A.q_desc = s.up(q_desc, (size_t)n_q * 32);
-  A.q_length = q_length ? s.up(q_length, n_q) : nullptr; A.q_view_cos = q_view_cos ? s.up(q_view_cos, n_q) : nullptr;
-  A.th = th; A.nnratio = nnratio; A.variant = variant;
-  A.preassigned = preassigned ? s.up(preassigned, n) : nullptr;
-  A.match = s.alloc<int>(cap); A.nmatches = s.alloc<int>(1);
-  A.g_start = s.alloc<int>(NCELL + 1); A.g_items = s.alloc<unsigned short>((size_t)cap * kMaxPath);
-  A.g_path = s.alloc<unsigned short>((size_t)cap * kMaxPath); A.g_plen = s.alloc<unsigned short>(cap); A.g_first = s.alloc<int>(cap);
-  PL_ARG(A.kl && A.lfunc && A.desc && A.match && A.nmatches && A.g_start && A.g_items && A.g_path && A.g_plen && A.g_first);
-  k_line_search<<<1, 32>>>(A);
-  PL_LAUNCH_CHECK();
+  uint8_t* dk = s.in((const uint8_t*)kls, (size_t)n * 68); double* dlf = s.in(lfunc, (size_t)n * 3);
+  uint8_t* dd = s.in(desc, (size_t)n * 32); int* dn = s.in(&n, 1); float* db = s.in(bounds, 4);
+  int* dnq = s.in(&n_q, 1); uint8_t* dv = s.in(q_valid, n_q); float* dp = s.in(q_proj, (size_t)n_q * 4);
+  uint8_t* dqd = s.in(q_desc, (size_t)n_q * 32); float* dlv = s.in(q_length_or_view_cos, n_q);
+  uint8_t* dpre = preassigned ? s.in(preassigned, n) : nullptr;
   int nm = 0;
-  rc = down(&nm, A.nmatches, 1); if (rc) return rc;
-  if (n) { rc = down(match, A.match, (size_t)n); if (rc) return rc; }
+  int* dm = s.out(match, n, cap); int* dnm = s.out(&nm, 1);
+  uint8_t* scratch = s.out<uint8_t>(pl_lsd_search_scratch_bytes(cap, 1));
+  if ((rc = s.status()) ||
+      (rc = lsd_search_by_projection_launch(variant, dk, dlf, dd, dn, cap, 1, db, dnq, capq, dv, dp, dqd, dlv, th, nullptr, nullptr,
+                                            nnratio, dpre, dm, dnm, scratch, nullptr)) ||
+      (rc = s.fetch()))
+    return rc;
   return nm;
 }
 
@@ -1395,14 +1349,14 @@ extern "C" int pl_lsd_search_by_projection_last(const void* keylines_cur, const 
                                                 const float* last_proj, const uint8_t* last_desc, const float* last_length,
                                                 float th, const uint8_t* cur_preassigned, int* cur_match) {
   return line_search_host(0, keylines_cur, linefunc_cur, desc_cur, n_cur, bounds, n_last, last_valid, last_proj, last_desc,
-                          last_length, nullptr, th, 0.f, cur_preassigned, cur_match);
+                          last_length, th, 0.f, cur_preassigned, cur_match);
 }
 extern "C" int pl_lsd_search_by_projection_lines(const void* keylines, const double* linefunc, const uint8_t* desc, int n,
                                                  const float* bounds, int n_ml, const uint8_t* in_view, const float* proj,
                                                  const float* view_cos, const uint8_t* ml_desc, float th, float nnratio,
                                                  const uint8_t* preassigned, int* match) {
-  return line_search_host(1, keylines, linefunc, desc, n, bounds, n_ml, in_view, proj, ml_desc, nullptr, view_cos, th, nnratio,
-                          preassigned, match);
+  return line_search_host(1, keylines, linefunc, desc, n, bounds, n_ml, in_view, proj, ml_desc, view_cos, th, nnratio, preassigned,
+                          match);
 }
 
 extern "C" size_t pl_lsd_search_scratch_bytes(int cap, int B) {
@@ -1470,12 +1424,12 @@ extern "C" int pl_orb_search_for_triangulation(const PLKeyPoint* keys1_un, const
   if (q_idx1.empty() || n1 == 0 || n2 == 0) return 0;
   const int nitems2 = fv2_start[nn2];
   for (int i = 0; i < nitems2; i++) PL_ARG(fv2_items[i] >= 0 && fv2_items[i] < n2);
-  Stage s;
+  Staging s;
   TriArgs A;
-  A.k1 = s.up(keys1_un, n1); A.k2 = s.up(keys2_un, n2); A.d1 = s.up(desc1, (size_t)n1 * 32); A.d2 = s.up(desc2, (size_t)n2 * 32);
-  A.mp1 = s.up(has_mp1, n1); A.mp2 = s.up(has_mp2, n2);
-  A.q_idx1 = s.up(q_idx1.data(), q_idx1.size()); A.q_s = s.up(q_s.data(), q_s.size()); A.q_e = s.up(q_e.data(), q_e.size());
-  A.fv2_items = s.up(fv2_items, nitems2); A.nq = (int)q_idx1.size(); A.n1 = n1;
+  A.k1 = s.in(keys1_un, n1); A.k2 = s.in(keys2_un, n2); A.d1 = s.in(desc1, (size_t)n1 * 32); A.d2 = s.in(desc2, (size_t)n2 * 32);
+  A.mp1 = s.in(has_mp1, n1); A.mp2 = s.in(has_mp2, n2);
+  A.q_idx1 = s.in(q_idx1.data(), q_idx1.size()); A.q_s = s.in(q_s.data(), q_s.size()); A.q_e = s.in(q_e.data(), q_e.size());
+  A.fv2_items = s.in(fv2_items, nitems2); A.nq = (int)q_idx1.size(); A.n1 = n1;
   memcpy(A.F, F12, sizeof(A.F));
   {  // epipole of camera 1 in image 2 (:729-737): C2 = R2w*Cw + t2w in cv::gemm's fp32 order
     float C2[3];
@@ -1483,15 +1437,13 @@ extern "C" int pl_orb_search_for_triangulation(const PLKeyPoint* keys1_un, const
     const float invz = 1.0f / C2[2];
     A.ex = K2[0] * C2[0] * invz + K2[2]; A.ey = K2[1] * C2[1] * invz + K2[3];
   }
-  A.scale2 = s.up(scale_factors2, nlevels); A.sigma2_2 = s.up(level_sigma2_2, nlevels); A.checkOri = check_orientation;
-  A.matches12 = s.alloc<int>(n1); A.nmatches = s.alloc<int>(1); A.bins = s.alloc<unsigned char>(n1);
-  PL_ARG(A.k1 && A.k2 && A.d1 && A.d2 && A.mp1 && A.mp2 && A.q_idx1 && A.q_s && A.q_e && A.fv2_items && A.scale2 && A.sigma2_2 &&
-         A.matches12 && A.nmatches && A.bins);
+  A.scale2 = s.in(scale_factors2, nlevels); A.sigma2_2 = s.in(level_sigma2_2, nlevels); A.checkOri = check_orientation;
+  int nm = 0;
+  A.matches12 = s.out(matches12, n1); A.nmatches = s.out(&nm, 1); A.bins = s.out<unsigned char>(n1);
+  if ((rc = s.status())) return rc;
   k_search_triangulation<<<1, 256>>>(A);
   PL_LAUNCH_CHECK();
-  int nm = 0;
-  rc = down(&nm, A.nmatches, 1); if (rc) return rc;
-  rc = down(matches12, A.matches12, (size_t)n1); if (rc) return rc;
+  if ((rc = s.fetch())) return rc;
   return nm;
 }
 
@@ -1505,23 +1457,21 @@ extern "C" int pl_orb_fuse_search(const PLKeyPoint* keys_un, const uint8_t* desc
   PL_ARG(n_mp == 0 || (pos && normal && min_dist && max_dist && mp_desc));
   int rc = require_device(); if (rc) return rc;
   if (n_mp == 0) return PL_OK;
-  Stage s;
+  Staging s;
   FuseArgs A;
-  A.keys = s.up(keys_un, n); A.desc = s.up(desc, (size_t)n * 32); A.n = n;
+  A.keys = s.in(keys_un, n); A.desc = s.in(desc, (size_t)n * 32); A.n = n;
   memcpy(A.bounds, bounds, 16); memcpy(A.T, Tcw, 64); memcpy(A.Ow, Ow, 12); memcpy(A.K, K, 16);
-  A.scaleFactors = s.up(scale_factors, nlevels); A.invSigma2 = s.up(inv_level_sigma2, nlevels);
+  A.scaleFactors = s.in(scale_factors, nlevels); A.invSigma2 = s.in(inv_level_sigma2, nlevels);
   A.logScaleFactor = log_scale_factor; A.nLevels = nlevels; A.n_mp = n_mp;
-  A.skip = skip ? s.up(skip, n_mp) : nullptr; A.pos = s.up(pos, (size_t)n_mp * 3); A.normal = s.up(normal, (size_t)n_mp * 3);
-  A.minDist = s.up(min_dist, n_mp); A.maxDist = s.up(max_dist, n_mp); A.mp_desc = s.up(mp_desc, (size_t)n_mp * 32); A.th = th;
-  A.best_idx = s.alloc<int>(n_mp); A.best_dist = s.alloc<int>(n_mp);
-  PL_ARG(A.keys && A.desc && A.scaleFactors && A.invSigma2 && A.pos && A.normal && A.minDist && A.maxDist && A.mp_desc && A.best_idx &&
-         A.best_dist);
+  A.skip = skip ? s.in(skip, n_mp) : nullptr; A.pos = s.in(pos, (size_t)n_mp * 3); A.normal = s.in(normal, (size_t)n_mp * 3);
+  A.minDist = s.in(min_dist, n_mp); A.maxDist = s.in(max_dist, n_mp); A.mp_desc = s.in(mp_desc, (size_t)n_mp * 32); A.th = th;
+  A.best_idx = s.out(best_idx, n_mp); A.best_dist = s.out(best_dist, n_mp);
+  if ((rc = s.status())) return rc;
   const size_t sm = grid_smem_bytes(std::max(n, 1));
   PL_CUDA(cudaFuncSetAttribute(k_fuse_search, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
   k_fuse_search<<<1, 32 * kFuseWarps, sm>>>(A);
   PL_LAUNCH_CHECK();
-  rc = down(best_idx, A.best_idx, (size_t)n_mp); if (rc) return rc;
-  return down(best_dist, A.best_dist, (size_t)n_mp);
+  return s.fetch();
 }
 
 static int search_by_bow_host(const PLKeyPoint* keysKF_un, const uint8_t* descKF, const uint8_t* has_mp_kf, int nKF,
@@ -1544,21 +1494,20 @@ static int search_by_bow_host(const PLKeyPoint* keysKF_un, const uint8_t* descKF
   for (int i = 0; i < nitK; i++) PL_ARG(fvK_items[i] >= 0 && fvK_items[i] < nKF);
   for (int i = 0; i < nitF; i++) PL_ARG(fvF_items[i] >= 0 && fvF_items[i] < nF);
   PL_ARG(nF < (1 << 20));
-  Stage s;
+  Staging s;
   BowArgs A;
-  A.kK = s.up(keysKF_un, nKF); A.kF = s.up(keysF, nF); A.dK = s.up(descKF, (size_t)nKF * 32); A.dF = s.up(descF, (size_t)nF * 32);
-  A.mpK = s.up(has_mp_kf, nKF);
-  A.pairK_s = s.up(ks.data(), ks.size()); A.pairK_e = s.up(ke.data(), ke.size()); A.pairF_s = s.up(fs.data(), fs.size()); A.pairF_e = s.up(fe.data(), fe.size());
-  A.itK = s.up(fvK_items, nitK); A.itF = s.up(fvF_items, nitF); A.npairs = (int)ks.size(); A.nF = nF;
+  A.kK = s.in(keysKF_un, nKF); A.kF = s.in(keysF, nF); A.dK = s.in(descKF, (size_t)nKF * 32); A.dF = s.in(descF, (size_t)nF * 32);
+  A.mpK = s.in(has_mp_kf, nKF);
+  A.pairK_s = s.in(ks.data(), ks.size()); A.pairK_e = s.in(ke.data(), ke.size()); A.pairF_s = s.in(fs.data(), fs.size()); A.pairF_e = s.in(fe.data(), fe.size());
+  A.itK = s.in(fvK_items, nitK); A.itF = s.in(fvF_items, nitF); A.npairs = (int)ks.size(); A.nF = nF;
   A.nnratio = nnratio; A.checkOri = check_orientation;
-  A.mpF = has_mp_f ? s.up(has_mp_f, nF) : nullptr; A.strict = strict;
-  A.matchesF = s.alloc<int>(nF); A.bins = s.alloc<unsigned char>(nF); A.nmatches = s.alloc<int>(1);
-  PL_ARG(A.kK && A.kF && A.dK && A.dF && A.mpK && A.pairK_s && A.pairK_e && A.pairF_s && A.pairF_e && A.itK && A.itF && A.matchesF && A.bins && A.nmatches);
+  A.mpF = has_mp_f ? s.in(has_mp_f, nF) : nullptr; A.strict = strict;
+  int nm = 0;
+  A.matchesF = s.out(matchesF, nF); A.bins = s.out<unsigned char>(nF); A.nmatches = s.out(&nm, 1);
+  if ((rc = s.status())) return rc;
   k_search_by_bow<<<1, 32 * kBowWarps>>>(A);
   PL_LAUNCH_CHECK();
-  int nm = 0;
-  rc = down(&nm, A.nmatches, 1); if (rc) return rc;
-  rc = down(matchesF, A.matchesF, (size_t)nF); if (rc) return rc;
+  if ((rc = s.fetch())) return rc;
   return nm;
 }
 
@@ -1595,27 +1544,26 @@ extern "C" int pl_orb_search_by_projection_keyframe(const PLKeyPoint* keys_cur, 
   PL_ARG(keys_cur && desc_cur && bounds && Tcw && Ow && K && scale_factors && cur_match && n_cur >= 0 && n_cur <= 6144 && n_kf >= 0 && nlevels > 0);
   PL_ARG(n_kf == 0 || (kf_valid && pos && mp_desc && min_dist && max_dist && kf_angle));
   int rc = require_device(); if (rc) return rc;
-  Stage s;
+  Staging s;
   const int cap = std::max(n_cur, 1), capl = std::max(n_kf, 1);
   ProjLastArgs A;
-  A.keys = s.up(keys_cur, n_cur); A.desc = s.up(desc_cur, (size_t)n_cur * 32); A.n = s.up(&n_cur, 1); A.cap = cap;
-  A.bounds = s.up(bounds, 4); A.Tcw = s.up(Tcw, 16); A.K = s.up(K, 4); A.scaleFactors = s.up(scale_factors, nlevels);
-  A.nlevels = nlevels; A.n_last = s.up(&n_kf, 1); A.cap_last = capl;
-  A.last_valid = s.up(kf_valid, n_kf); A.last_pos = s.up(pos, (size_t)n_kf * 3); A.last_desc = s.up(mp_desc, (size_t)n_kf * 32);
-  A.last_octave = nullptr; A.last_angle = s.up(kf_angle, n_kf);
+  A.keys = s.in(keys_cur, n_cur); A.desc = s.in(desc_cur, (size_t)n_cur * 32); A.n = s.in(&n_cur, 1); A.cap = cap;
+  A.bounds = s.in(bounds, 4); A.Tcw = s.in(Tcw, 16); A.K = s.in(K, 4); A.scaleFactors = s.in(scale_factors, nlevels);
+  A.nlevels = nlevels; A.n_last = s.in(&n_kf, 1); A.cap_last = capl;
+  A.last_valid = s.in(kf_valid, n_kf); A.last_pos = s.in(pos, (size_t)n_kf * 3); A.last_desc = s.in(mp_desc, (size_t)n_kf * 32);
+  A.last_octave = nullptr; A.last_angle = s.in(kf_angle, n_kf);
   A.th = th; A.checkOri = check_orientation;
-  A.preassigned = cur_preassigned ? s.up(cur_preassigned, n_cur) : nullptr;
-  A.match = s.alloc<int>(cap); A.nmatches = s.alloc<int>(1);
-  A.kfMode = 1; A.maxDist = orb_dist; A.min_dist = s.up(min_dist, n_kf); A.max_dist = s.up(max_dist, n_kf);
+  A.preassigned = cur_preassigned ? s.in(cur_preassigned, n_cur) : nullptr;
+  int nm = 0;
+  A.match = s.out(cur_match, n_cur, cap); A.nmatches = s.out(&nm, 1);
+  A.kfMode = 1; A.maxDist = orb_dist; A.min_dist = s.in(min_dist, n_kf); A.max_dist = s.in(max_dist, n_kf);
   memcpy(A.Ow, Ow, 12); A.logSF = log_scale_factor;
-  PL_ARG(A.keys && A.desc && A.match && A.nmatches && A.last_pos && A.last_desc && A.min_dist && A.max_dist && A.last_angle);
+  if ((rc = s.status())) return rc;
   size_t sm = grid_smem_bytes(cap);
   PL_CUDA(cudaFuncSetAttribute(k_search_proj_last, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
   k_search_proj_last<<<1, 32, sm>>>(A);
   PL_LAUNCH_CHECK();
-  int nm = 0;
-  rc = down(&nm, A.nmatches, 1); if (rc) return rc;
-  if (n_cur) { rc = down(cur_match, A.match, (size_t)n_cur); if (rc) return rc; }
+  if ((rc = s.fetch())) return rc;
   return nm;
 }
 
@@ -1625,15 +1573,13 @@ extern "C" int pl_mappoint_distinctive_descriptors(const uint8_t* desc, const in
   if (n_mp == 0) return PL_OK;
   const int total = offsets[n_mp];
   PL_ARG(total >= 0);
-  Stage s;
-  const uint8_t* dd = s.up(desc, (size_t)total * 32); const int* doff = s.up(offsets, (size_t)n_mp + 1);
-  int* db = s.alloc<int>(n_mp); uint8_t* dout = out_desc ? s.alloc<uint8_t>((size_t)n_mp * 32) : nullptr;
-  PL_ARG(dd && doff && db);
+  Staging s;
+  const uint8_t* dd = s.in(desc, (size_t)total * 32); const int* doff = s.in(offsets, (size_t)n_mp + 1);
+  int* db = s.out(best_idx, n_mp); uint8_t* dout = s.out(out_desc, (size_t)n_mp * 32);
+  if ((rc = s.status())) return rc;
   k_distinctive<<<(n_mp + kDistWarps - 1) / kDistWarps, 32 * kDistWarps>>>(dd, doff, n_mp, db, dout);
   PL_LAUNCH_CHECK();
-  rc = down(best_idx, db, (size_t)n_mp); if (rc) return rc;
-  if (out_desc) { rc = down(out_desc, dout, (size_t)n_mp * 32); if (rc) return rc; }
-  return PL_OK;
+  return s.fetch();
 }
 
 extern "C" int pl_lsd_fuse_search(const void* keylines, int nl, const uint8_t* kf_point_desc, int n_pdesc, const float* bounds, const float* Tcw,
@@ -1645,21 +1591,19 @@ extern "C" int pl_lsd_fuse_search(const void* keylines, int nl, const uint8_t* k
   int rc = require_device(); if (rc) return rc;
   *stop_at = n_ml;
   if (n_ml == 0) return PL_OK;
-  Stage s;
+  Staging s;
   LineFuseArgs A;
-  A.kl = reinterpret_cast<const KeyLine68*>(s.up(static_cast<const uint8_t*>(keylines), (size_t)nl * 68)); A.nl = nl;
-  A.pdesc = s.up(kf_point_desc, (size_t)n_pdesc * 32); A.n_pdesc = n_pdesc;
+  A.kl = reinterpret_cast<const KeyLine68*>(s.in(static_cast<const uint8_t*>(keylines), (size_t)nl * 68)); A.nl = nl;
+  A.pdesc = s.in(kf_point_desc, (size_t)n_pdesc * 32); A.n_pdesc = n_pdesc;
   memcpy(A.bounds, bounds, 16); memcpy(A.T, Tcw, 64); memcpy(A.Ow, Ow, 12); memcpy(A.K, K, 16);
   A.scale_line = scale_line; A.logScaleFactorLine = log_scale_factor_line; A.n_ml = n_ml;
-  A.skip = s.up(skip, n_ml); A.pos = s.up(pos, (size_t)n_ml * 6); A.normal = s.up(normal, (size_t)n_ml * 3);
-  A.minDist = s.up(min_dist, n_ml); A.maxDist = s.up(max_dist, n_ml); A.ml_desc = s.up(ml_desc, (size_t)n_ml * 32); A.th = th;
-  A.best_idx = s.alloc<int>(n_ml); A.best_dist = s.alloc<int>(n_ml); A.stop_at = s.up(stop_at, 1);
-  PL_ARG(A.kl && A.pdesc && A.skip && A.pos && A.normal && A.minDist && A.maxDist && A.ml_desc && A.best_idx && A.best_dist && A.stop_at);
+  A.skip = s.in(skip, n_ml); A.pos = s.in(pos, (size_t)n_ml * 6); A.normal = s.in(normal, (size_t)n_ml * 3);
+  A.minDist = s.in(min_dist, n_ml); A.maxDist = s.in(max_dist, n_ml); A.ml_desc = s.in(ml_desc, (size_t)n_ml * 32); A.th = th;
+  A.best_idx = s.out(best_idx, n_ml); A.best_dist = s.out(best_dist, n_ml); A.stop_at = s.in(stop_at, 1);
+  if ((rc = s.status())) return rc;
   k_lsd_fuse_search<<<(n_ml + 127) / 128, 128>>>(A);
   PL_LAUNCH_CHECK();
-  rc = down(best_idx, A.best_idx, (size_t)n_ml); if (rc) return rc;
-  rc = down(best_dist, A.best_dist, (size_t)n_ml); if (rc) return rc;
-  rc = down(stop_at, A.stop_at, 1); if (rc) return rc;
+  if ((rc = s.fetch()) || (rc = s.down(stop_at, A.stop_at, 1))) return rc;
   for (int i = *stop_at; i < n_ml; i++) { best_idx[i] = -1; best_dist[i] = 256; }     // never reached by the reference's loop
   return PL_OK;
 }

@@ -481,73 +481,42 @@ extern "C" int pl_track_local_map(PLMap* map, const PLTrackFrames* F, const PLTr
   const int cap = std::max(n, 1), capL = std::max(nl, 1);
   const size_t lp = (size_t)L->pt_count[0], ll = (size_t)L->ln_count[0];
   const int cLP = std::max((int)lp, 1), cLL = std::max((int)ll, 1);
-  std::vector<void*> fr;
-  cudaError_t e = cudaSuccess;
-  auto dal = [&](size_t bytes) -> void* {
-    void* p = nullptr;
-    if (e == cudaSuccess) e = cudaMalloc(&p, std::max<size_t>(bytes, 16));
-    if (e == cudaSuccess) { fr.push_back(p); e = cudaMemset(p, 0, std::max<size_t>(bytes, 16)); }
-    return e == cudaSuccess ? p : nullptr;
-  };
-  auto dup = [&](const void* h, size_t bytes) -> void* {
-    void* p = dal(bytes);
-    if (p && h && bytes) e = cudaMemcpy(p, h, bytes, cudaMemcpyHostToDevice);
-    return e == cudaSuccess ? p : nullptr;
-  };
+  Staging s;
   PLTrackFrames D = *F;
   D.cap_points = cap; D.cap_lines = capL;
-  D.keys_un = (const PLKeyPoint*)dup(F->keys_un, (size_t)n * sizeof(PLKeyPoint)); D.desc = (const uint8_t*)dup(F->desc, (size_t)n * 32);
-  D.n = (const int*)dup(&n, 4);
-  D.keylines = dup(F->keylines, (size_t)nl * 68); D.line_func = (const double*)dup(F->line_func, (size_t)nl * 24);
-  D.line_desc = (const uint8_t*)dup(F->line_desc, (size_t)nl * 32); D.nl = (const int*)dup(&nl, 4);
-  D.bounds = (const float*)dup(F->bounds, 16); D.scale_factors = (const float*)dup(F->scale_factors, (size_t)F->nlevels * 4);
-  D.inv_level_sigma2 = (const float*)dup(F->inv_level_sigma2, (size_t)F->nlevels * 4);
-  D.Tcw0 = (const float*)dup(F->Tcw0, 64); D.K = (const float*)dup(F->K, 16);
-  D.point_map_in = F->point_map_in ? (const int*)dup(F->point_map_in, (size_t)n * 4) : nullptr;
-  D.line_map_in = F->line_map_in ? (const int*)dup(F->line_map_in, (size_t)nl * 4) : nullptr;
+  D.keys_un = s.in(F->keys_un, n); D.desc = s.in(F->desc, (size_t)n * 32); D.n = s.in(&n, 1);
+  D.keylines = s.in((const uint8_t*)F->keylines, (size_t)nl * 68); D.line_func = s.in(F->line_func, (size_t)nl * 3);
+  D.line_desc = s.in(F->line_desc, (size_t)nl * 32); D.nl = s.in(&nl, 1);
+  D.bounds = s.in(F->bounds, 4); D.scale_factors = s.in(F->scale_factors, F->nlevels);
+  D.inv_level_sigma2 = s.in(F->inv_level_sigma2, F->nlevels); D.Tcw0 = s.in(F->Tcw0, 16); D.K = s.in(F->K, 4);
+  D.point_map_in = F->point_map_in ? s.in(F->point_map_in, n) : nullptr;
+  D.line_map_in = F->line_map_in ? s.in(F->line_map_in, nl) : nullptr;
   const int zero = 0;
   PLTrackLocal DL = *L;
   DL.pt_offset = &zero; DL.ln_offset = &zero; DL.cap_local_points = cLP; DL.cap_local_lines = cLL;
   DL.n_pt_index = (int)lp; DL.n_ln_index = (int)ll;
-  DL.pt_index = lp ? (const int*)dup(L->pt_index + L->pt_offset[0], lp * 4) : nullptr;
-  DL.ln_index = ll ? (const int*)dup(L->ln_index + L->ln_offset[0], ll * 4) : nullptr;
-  struct Field { void* host; size_t bytes; void* dev; };
-  std::vector<Field> outs;
+  DL.pt_index = lp ? s.in(L->pt_index + L->pt_offset[0], lp) : nullptr;
+  DL.ln_index = ll ? s.in(L->ln_index + L->ln_offset[0], ll) : nullptr;
   // required outputs always get a device array; optional ones only when asked for
-  auto dout = [&](void* h, size_t bytes, size_t alloc) -> void* {
-    if (!h) return nullptr;
-    void* d = dal(alloc); outs.push_back({h, bytes, d}); return d;
-  };
   int ok_h = 0;
   PLTrackOut DO;
-  DO.Tcw = (float*)dout(O->Tcw, 64, 64); DO.ok = (int*)dout(&ok_h, 4, 4); DO.inliers = (int*)dout(O->inliers, 8, 8);
-  DO.point_map = (int*)dout(O->point_map, (size_t)n * 4, (size_t)cap * 4); DO.point_outlier = (uint8_t*)dout(O->point_outlier, n, cap);
-  DO.line_map = (int*)dout(O->line_map, (size_t)nl * 4, (size_t)capL * 4); DO.line_outlier = (uint8_t*)dout(O->line_outlier, nl, capL);
-  DO.pt_in_view = (uint8_t*)dout(O->pt_in_view, lp, cLP); DO.pt_proj = (float*)dout(O->pt_proj, lp * 8, (size_t)cLP * 8);
-  DO.pt_level = (int*)dout(O->pt_level, lp * 4, (size_t)cLP * 4); DO.pt_view_cos = (float*)dout(O->pt_view_cos, lp * 4, (size_t)cLP * 4);
-  DO.ln_in_view = (uint8_t*)dout(O->ln_in_view, ll, cLL); DO.ln_proj = (float*)dout(O->ln_proj, ll * 16, (size_t)cLL * 16);
-  DO.ln_level = (int*)dout(O->ln_level, ll * 4, (size_t)cLL * 4); DO.ln_view_cos = (float*)dout(O->ln_view_cos, ll * 4, (size_t)cLL * 4);
-  DO.pt_match = (int*)dout(O->pt_match, (size_t)n * 4, (size_t)cap * 4); DO.ln_match = (int*)dout(O->ln_match, (size_t)nl * 4, (size_t)capL * 4);
-  DO.prob_n_points = (int*)dout(O->prob_n_points, 4, 4); DO.prob_n_lines = (int*)dout(O->prob_n_lines, 4, 4);
-  DO.prob_pt_obs = (float*)dout(O->prob_pt_obs, (size_t)n * 8, (size_t)cap * 8);
-  DO.prob_pt_inv_sigma2 = (float*)dout(O->prob_pt_inv_sigma2, (size_t)n * 4, (size_t)cap * 4);
-  DO.prob_pt_Xw = (float*)dout(O->prob_pt_Xw, (size_t)n * 12, (size_t)cap * 12);
-  DO.prob_line_func = (double*)dout(O->prob_line_func, (size_t)nl * 24, (size_t)capL * 24);
-  DO.prob_line_Xw = (double*)dout(O->prob_line_Xw, (size_t)nl * 48, (size_t)capL * 48);
-  void* scr = dal(pl_track_local_map_scratch_bytes(1, cap, capL, cLP, cLL));
-  int ret = PL_ERR_CUDA;
-  if (e != cudaSuccess || !scr) set_error("track_local_map: %s", cudaGetErrorString(e));
-  else {
-    ret = pl_track_local_map_dev(map, &D, &DL, &DO, scr, map->stream);
-    if (ret == PL_OK) {
-      e = cudaStreamSynchronize(map->stream);
-      for (const Field& f : outs) if (e == cudaSuccess && f.bytes) e = cudaMemcpy(f.host, f.dev, f.bytes, cudaMemcpyDeviceToHost);
-      if (e != cudaSuccess) { set_error("track_local_map: %s", cudaGetErrorString(e)); ret = PL_ERR_CUDA; }
-    }
-  }
-  for (void* p : fr) cudaFree(p);
-  if (ret != PL_OK) return ret;
-  if ((rc = pl_map_check_indices(map))) return rc;
+  DO.Tcw = s.out(O->Tcw, 16); DO.ok = s.out(&ok_h, 1); DO.inliers = s.out(O->inliers, 2);
+  DO.point_map = s.out(O->point_map, n, cap); DO.point_outlier = s.out(O->point_outlier, n, cap);
+  DO.line_map = s.out(O->line_map, nl, capL); DO.line_outlier = s.out(O->line_outlier, nl, capL);
+  DO.pt_in_view = s.out(O->pt_in_view, lp, cLP); DO.pt_proj = s.out(O->pt_proj, lp * 2, (size_t)cLP * 2);
+  DO.pt_level = s.out(O->pt_level, lp, cLP); DO.pt_view_cos = s.out(O->pt_view_cos, lp, cLP);
+  DO.ln_in_view = s.out(O->ln_in_view, ll, cLL); DO.ln_proj = s.out(O->ln_proj, ll * 4, (size_t)cLL * 4);
+  DO.ln_level = s.out(O->ln_level, ll, cLL); DO.ln_view_cos = s.out(O->ln_view_cos, ll, cLL);
+  DO.pt_match = s.out(O->pt_match, n, cap); DO.ln_match = s.out(O->ln_match, nl, capL);
+  DO.prob_n_points = s.out(O->prob_n_points, 1); DO.prob_n_lines = s.out(O->prob_n_lines, 1);
+  DO.prob_pt_obs = s.out(O->prob_pt_obs, (size_t)n * 2, (size_t)cap * 2); DO.prob_pt_inv_sigma2 = s.out(O->prob_pt_inv_sigma2, n, cap);
+  DO.prob_pt_Xw = s.out(O->prob_pt_Xw, (size_t)n * 3, (size_t)cap * 3);
+  DO.prob_line_func = s.out(O->prob_line_func, (size_t)nl * 3, (size_t)capL * 3);
+  DO.prob_line_Xw = s.out(O->prob_line_Xw, (size_t)nl * 6, (size_t)capL * 6);
+  void* scr = s.out<uint8_t>(pl_track_local_map_scratch_bytes(1, cap, capL, cLP, cLL));
+  if ((rc = s.status()) || (rc = s.sync()) || (rc = pl_track_local_map_dev(map, &D, &DL, &DO, scr, map->stream))) return rc;
+  PL_CUDA(cudaStreamSynchronize(map->stream));
+  if ((rc = s.fetch()) || (rc = pl_map_check_indices(map))) return rc;
   return ok_h;
 }
 
@@ -803,75 +772,40 @@ extern "C" int pl_track_motion_model(PLMap* map, const PLTrackFrames* F, const P
          nl0 <= F->cap_lines);
   int rc = require_device(); if (rc) return rc;
   const int cap = std::max(std::max(n, n0), 1), capL = std::max(std::max(nl, nl0), 1);
-  std::vector<void*> fr;
-  cudaError_t e = cudaSuccess;
-  auto dal = [&](size_t bytes) -> void* {
-    void* p = nullptr;
-    if (e == cudaSuccess) e = cudaMalloc(&p, std::max<size_t>(bytes, 16));
-    if (e == cudaSuccess) { fr.push_back(p); e = cudaMemset(p, 0, std::max<size_t>(bytes, 16)); }
-    return e == cudaSuccess ? p : nullptr;
-  };
-  auto dup = [&](const void* h, size_t bytes) -> void* {
-    void* p = dal(bytes);
-    if (p && h && bytes) e = cudaMemcpy(p, h, bytes, cudaMemcpyHostToDevice);
-    return e == cudaSuccess ? p : nullptr;
-  };
+  Staging s;
   PLTrackFrames D = *F;
   D.cap_points = cap; D.cap_lines = capL;
-  D.keys_un = (const PLKeyPoint*)dup(F->keys_un, (size_t)n * sizeof(PLKeyPoint)); D.desc = (const uint8_t*)dup(F->desc, (size_t)n * 32);
-  D.n = (const int*)dup(&n, 4);
-  D.keylines = dup(F->keylines, (size_t)nl * 68); D.line_func = (const double*)dup(F->line_func, (size_t)nl * 24);
-  D.line_desc = (const uint8_t*)dup(F->line_desc, (size_t)nl * 32); D.nl = (const int*)dup(&nl, 4);
-  D.bounds = (const float*)dup(F->bounds, 16); D.scale_factors = (const float*)dup(F->scale_factors, (size_t)F->nlevels * 4);
-  D.inv_level_sigma2 = (const float*)dup(F->inv_level_sigma2, (size_t)F->nlevels * 4);
-  D.K = (const float*)dup(F->K, 16);
+  D.keys_un = s.in(F->keys_un, n); D.desc = s.in(F->desc, (size_t)n * 32); D.n = s.in(&n, 1);
+  D.keylines = s.in((const uint8_t*)F->keylines, (size_t)nl * 68); D.line_func = s.in(F->line_func, (size_t)nl * 3);
+  D.line_desc = s.in(F->line_desc, (size_t)nl * 32); D.nl = s.in(&nl, 1);
+  D.bounds = s.in(F->bounds, 4); D.scale_factors = s.in(F->scale_factors, F->nlevels);
+  D.inv_level_sigma2 = s.in(F->inv_level_sigma2, F->nlevels); D.K = s.in(F->K, 4);
   PLTrackLast DL;
-  DL.keys_un = (const PLKeyPoint*)dup(Ls->keys_un, (size_t)n0 * sizeof(PLKeyPoint)); DL.n = (const int*)dup(&n0, 4);
-  DL.keylines = dup(Ls->keylines, (size_t)nl0 * 68); DL.nl = (const int*)dup(&nl0, 4);
-  DL.point_map = (const int*)dup(Ls->point_map, (size_t)n0 * 4); DL.point_outlier = (const uint8_t*)dup(Ls->point_outlier, (size_t)n0);
-  DL.line_map = (const int*)dup(Ls->line_map, (size_t)nl0 * 4); DL.line_outlier = (const uint8_t*)dup(Ls->line_outlier, (size_t)nl0);
-  DL.Tcw = (const float*)dup(Ls->Tcw, 64); DL.velocity = (const float*)dup(Ls->velocity, 64);
-  struct Field { void* host; size_t bytes; void* dev; };
-  std::vector<Field> outs;
-  auto dout = [&](void* h, size_t bytes, size_t alloc) -> void* {
-    if (!h) return nullptr;
-    void* d = dal(alloc); outs.push_back({h, bytes, d}); return d;
-  };
+  DL.keys_un = s.in(Ls->keys_un, n0); DL.n = s.in(&n0, 1);
+  DL.keylines = s.in((const uint8_t*)Ls->keylines, (size_t)nl0 * 68); DL.nl = s.in(&nl0, 1);
+  DL.point_map = s.in(Ls->point_map, n0); DL.point_outlier = s.in(Ls->point_outlier, n0);
+  DL.line_map = s.in(Ls->line_map, nl0); DL.line_outlier = s.in(Ls->line_outlier, nl0);
+  DL.Tcw = s.in(Ls->Tcw, 16); DL.velocity = s.in(Ls->velocity, 16);
   int ok_h = 0;
   PLTrackMotionOut DO;
-  DO.Tcw = (float*)dout(O->Tcw, 64, 64); DO.ok = (int*)dout(&ok_h, 4, 4); DO.nmatches = (int*)dout(O->nmatches, 8, 8);
-  DO.vo = (int*)dout(O->vo, 4, 4);
-  if (DO.vo && e == cudaSuccess) e = cudaMemcpy(DO.vo, O->vo, 4, cudaMemcpyHostToDevice);   // in / out
-  DO.point_map = (int*)dout(O->point_map, (size_t)n * 4, (size_t)cap * 4); DO.line_map = (int*)dout(O->line_map, (size_t)nl * 4, (size_t)capL * 4);
-  DO.point_seen = (int*)dout(O->point_seen, (size_t)n * 4, (size_t)cap * 4);
-  DO.line_seen = (int*)dout(O->line_seen, (size_t)nl * 4, (size_t)capL * 4);
-  DO.guess = (float*)dout(O->guess, 64, 64);
-  DO.pt_match = (int*)dout(O->pt_match, (size_t)n * 4, (size_t)cap * 4);
-  DO.pt_match_retry = (int*)dout(O->pt_match_retry, (size_t)n * 4, (size_t)cap * 4);
-  DO.retried = (uint8_t*)dout(O->retried, 1, 1); DO.ln_match = (int*)dout(O->ln_match, (size_t)nl * 4, (size_t)capL * 4);
-  DO.ln_in_view = (uint8_t*)dout(O->ln_in_view, nl0, capL); DO.ln_proj = (float*)dout(O->ln_proj, (size_t)nl0 * 16, (size_t)capL * 16);
-  DO.ln_level = (int*)dout(O->ln_level, (size_t)nl0 * 4, (size_t)capL * 4);
-  DO.ln_view_cos = (float*)dout(O->ln_view_cos, (size_t)nl0 * 4, (size_t)capL * 4);
-  DO.prob_n_points = (int*)dout(O->prob_n_points, 4, 4); DO.prob_n_lines = (int*)dout(O->prob_n_lines, 4, 4);
-  DO.prob_pt_obs = (float*)dout(O->prob_pt_obs, (size_t)n * 8, (size_t)cap * 8);
-  DO.prob_pt_inv_sigma2 = (float*)dout(O->prob_pt_inv_sigma2, (size_t)n * 4, (size_t)cap * 4);
-  DO.prob_pt_Xw = (float*)dout(O->prob_pt_Xw, (size_t)n * 12, (size_t)cap * 12);
-  DO.prob_line_func = (double*)dout(O->prob_line_func, (size_t)nl * 24, (size_t)capL * 24);
-  DO.prob_line_Xw = (double*)dout(O->prob_line_Xw, (size_t)nl * 48, (size_t)capL * 48);
-  void* scr = dal(pl_track_motion_model_scratch_bytes(1, cap, capL));
-  int ret = PL_ERR_CUDA;
-  if (e != cudaSuccess || !scr) set_error("track_motion_model: %s", cudaGetErrorString(e));
-  else {
-    ret = pl_track_motion_model_dev(map, &D, &DL, &DO, scr, map->stream);
-    if (ret == PL_OK) {
-      e = cudaStreamSynchronize(map->stream);
-      for (const Field& f : outs) if (e == cudaSuccess && f.bytes) e = cudaMemcpy(f.host, f.dev, f.bytes, cudaMemcpyDeviceToHost);
-      if (e != cudaSuccess) { set_error("track_motion_model: %s", cudaGetErrorString(e)); ret = PL_ERR_CUDA; }
-    }
-  }
-  for (void* p : fr) cudaFree(p);
-  if (ret != PL_OK) return ret;
-  if ((rc = pl_map_check_indices(map))) return rc;
+  DO.Tcw = s.out(O->Tcw, 16); DO.ok = s.out(&ok_h, 1); DO.nmatches = s.out(O->nmatches, 2);
+  DO.vo = s.in(O->vo, 1);   // in / out
+  DO.point_map = s.out(O->point_map, n, cap); DO.line_map = s.out(O->line_map, nl, capL);
+  DO.point_seen = s.out(O->point_seen, n, cap); DO.line_seen = s.out(O->line_seen, nl, capL);
+  DO.guess = s.out(O->guess, 16);
+  DO.pt_match = s.out(O->pt_match, n, cap); DO.pt_match_retry = s.out(O->pt_match_retry, n, cap);
+  DO.retried = s.out(O->retried, 1); DO.ln_match = s.out(O->ln_match, nl, capL);
+  DO.ln_in_view = s.out(O->ln_in_view, nl0, capL); DO.ln_proj = s.out(O->ln_proj, (size_t)nl0 * 4, (size_t)capL * 4);
+  DO.ln_level = s.out(O->ln_level, nl0, capL); DO.ln_view_cos = s.out(O->ln_view_cos, nl0, capL);
+  DO.prob_n_points = s.out(O->prob_n_points, 1); DO.prob_n_lines = s.out(O->prob_n_lines, 1);
+  DO.prob_pt_obs = s.out(O->prob_pt_obs, (size_t)n * 2, (size_t)cap * 2); DO.prob_pt_inv_sigma2 = s.out(O->prob_pt_inv_sigma2, n, cap);
+  DO.prob_pt_Xw = s.out(O->prob_pt_Xw, (size_t)n * 3, (size_t)cap * 3);
+  DO.prob_line_func = s.out(O->prob_line_func, (size_t)nl * 3, (size_t)capL * 3);
+  DO.prob_line_Xw = s.out(O->prob_line_Xw, (size_t)nl * 6, (size_t)capL * 6);
+  void* scr = s.out<uint8_t>(pl_track_motion_model_scratch_bytes(1, cap, capL));
+  if ((rc = s.status()) || (rc = s.sync()) || (rc = pl_track_motion_model_dev(map, &D, &DL, &DO, scr, map->stream))) return rc;
+  PL_CUDA(cudaStreamSynchronize(map->stream));
+  if ((rc = s.fetch()) || (rc = s.down(O->vo, DO.vo, 1)) || (rc = pl_map_check_indices(map))) return rc;
   return ok_h;
 }
 

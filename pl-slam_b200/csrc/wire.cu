@@ -59,15 +59,12 @@ static int pose_records_host(const float* poses, int n, std::vector<float>& rec)
   if (rc) return rc;
   rec.assign((size_t)std::max(n, 1) * 16, 0.f);
   if (n == 0) return PL_OK;
-  float *d_T = nullptr, *d_r = nullptr;
-  PL_CUDA(cudaMalloc(&d_T, (size_t)n * 64));
-  if (cudaMalloc(&d_r, (size_t)n * 64) != cudaSuccess) { cudaFree(d_T); set_error("pose records: device allocation failed"); return PL_ERR_CUDA; }
-  cudaError_t e = cudaMemcpy(d_T, poses, (size_t)n * 64, cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) { k_pose_records<<<(n + 127) / 128, 128>>>(d_T, n, d_r); count_launch(); e = cudaGetLastError(); }
-  if (e == cudaSuccess) e = cudaMemcpy(rec.data(), d_r, (size_t)n * 64, cudaMemcpyDeviceToHost);
-  cudaFree(d_T); cudaFree(d_r);
-  if (e != cudaSuccess) { set_error("pose records: %s", cudaGetErrorString(e)); return PL_ERR_CUDA; }
-  return PL_OK;
+  Staging s;
+  float* d_T = s.in(poses, (size_t)n * 16); float* d_r = s.out(rec.data(), (size_t)n * 16);
+  if ((rc = s.status())) return rc;
+  k_pose_records<<<(n + 127) / 128, 128>>>(d_T, n, d_r);
+  PL_LAUNCH_CHECK();
+  return s.fetch();
 }
 
 static long long emit(const std::string& s, char* out, size_t cap) {
