@@ -29,6 +29,8 @@ const char* pl_last_error(void);
 int pl_version(void);
 /* number of kernels this library has launched since load (bench.py's gpu_launches claim) */
 unsigned long long pl_launch_count(void);
+/* device bytes currently held through the library's owner type: every handle's buffers, not per-call staging */
+unsigned long long pl_device_bytes(void);
 
 /* ------------------------------------------------------------------ ORB extraction
  * replaces ORB_SLAM2::ORBextractor (reference include/ORBextractor.h:45-111,

@@ -37,6 +37,7 @@ def lib():
         L = C.CDLL(LIB_PATH)
         L.pl_last_error.restype = C.c_char_p
         L.pl_launch_count.restype = C.c_ulonglong
+        L.pl_device_bytes.restype = C.c_ulonglong
         L.pl_orb_create.argtypes = [C.POINTER(PLOrbConfig), C.POINTER(vp)]
         L.pl_orb_destroy.argtypes = [vp]
         L.pl_orb_capacity.argtypes = [vp]
@@ -62,6 +63,11 @@ def _p(a):
 
 def launch_count():
     return int(lib().pl_launch_count())
+
+
+def device_bytes():
+    """Device bytes the library's handles hold now (pl_device_bytes)."""
+    return int(lib().pl_device_bytes())
 
 
 class ORBextractor:

@@ -6,6 +6,7 @@
 namespace pl {
 static thread_local char g_err[512] = "";
 std::atomic<unsigned long long> g_launches{0};
+std::atomic<unsigned long long> g_dev_bytes{0};
 
 void set_error(const char* fmt, ...) {
   va_list ap;
@@ -46,3 +47,4 @@ int require_device() {
 extern "C" const char* pl_last_error(void) { return pl::g_err; }
 extern "C" int pl_version(void) { return 100; }
 extern "C" unsigned long long pl_launch_count(void) { return pl::g_launches.load(); }
+extern "C" unsigned long long pl_device_bytes(void) { return pl::g_dev_bytes.load(); }

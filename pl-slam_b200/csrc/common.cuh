@@ -5,6 +5,8 @@
 #include <stdio.h>
 #include <string>
 #include <atomic>
+#include <memory>
+#include <utility>
 #include <vector>
 #include "../../include/plslam_b200.h"
 
@@ -44,14 +46,55 @@ constexpr int kSerialFramesPerSM = 32;
     }                                                                                       \
   } while (0)
 
+#define PL_TRY(expr) do { const int _r = (expr); if (_r) return _r; } while (0)
+
 // Fails loudly when no Blackwell device is usable: there is no CPU fallback in this library.
 int require_device();
 
-template <typename T>
-inline int dev_alloc(T** p, size_t n) {
-  PL_CUDA(cudaMalloc((void**)p, n * sizeof(T)));
-  return PL_OK;
-}
+// Owners of the device memory, streams and events a handle holds: move-only, released by their destructor, and converted to
+// the raw pointer or handle wherever one is passed, so a handle is freed by deleting it.  A group of buffers made on first use
+// is built in a local and moved into its handle only once every allocation succeeded.
+extern std::atomic<unsigned long long> g_dev_bytes;   // bytes held by DevBufs (pl_device_bytes)
+template <typename T> class DevBuf {
+ public:
+  DevBuf() = default;
+  DevBuf(DevBuf&& o) noexcept { *this = std::move(o); }
+  DevBuf& operator=(DevBuf&& o) noexcept { std::swap(p_, o.p_); std::swap(n_, o.n_); return *this; }
+  ~DevBuf() { if (p_) { cudaFree(p_); g_dev_bytes -= n_ * sizeof(T); } }
+  int alloc(size_t n) {   // n elements, in place of what it held
+    void* p = nullptr;
+    PL_CUDA(cudaMalloc(&p, n * sizeof(T)));
+    *this = DevBuf();
+    p_ = (T*)p; n_ = p ? n : 0; g_dev_bytes += n_ * sizeof(T);
+    return PL_OK;
+  }
+  T* get() const { return p_; }
+  operator T*() const { return p_; }
+ private:
+  T* p_ = nullptr;
+  size_t n_ = 0;
+};
+template <typename H, cudaError_t (*Create)(H*, unsigned), cudaError_t (*Destroy)(H)> class CudaOwner {
+ public:
+  CudaOwner() = default;
+  CudaOwner(CudaOwner&& o) noexcept { std::swap(h_, o.h_); }
+  CudaOwner& operator=(CudaOwner&& o) noexcept { std::swap(h_, o.h_); return *this; }
+  ~CudaOwner() { if (h_) Destroy(h_); }
+  int create(unsigned flags) {
+    H h = nullptr;
+    PL_CUDA(Create(&h, flags));
+    *this = CudaOwner(); h_ = h;
+    return PL_OK;
+  }
+  operator H() const { return h_; }
+ private:
+  H h_ = nullptr;
+};
+using Stream = CudaOwner<cudaStream_t, cudaStreamCreateWithFlags, cudaStreamDestroy>;
+using Event = CudaOwner<cudaEvent_t, cudaEventCreateWithFlags, cudaEventDestroy>;
+// std::unique_ptr deleter for a handle another handle holds: Owned<PLOrb, pl_orb_destroy>
+template <auto Destroy> struct HandleDeleter { template <typename P> void operator()(P* p) const { Destroy(p); } };
+template <typename P, auto Destroy> using Owned = std::unique_ptr<P, HandleDeleter<Destroy>>;
 
 // Device copies of one host-pointer call's arrays, freed when it goes out of scope.  What is not copied in is zero-filled; fills
 // and copies are synchronous cudaMemset / cudaMemcpy on the legacy default stream.  The first failure sticks and makes the later

@@ -78,14 +78,12 @@ static CamD make_cam(const float* K, const float* D) { return CamD{(double)K[0],
 
 extern "C" void pl_undistort_destroy(PLUndistort* h) {
   if (!h) return;
-  cudaFree(h->d_map); cudaFree(h->d_tab); cudaFree(h->d_src); cudaFree(h->d_dst);
-  if (h->stream) cudaStreamDestroy(h->stream);
   delete h;
 }
 extern "C" int pl_undistort_create(const float* K, const float* dist5, int width, int height, PLUndistort** out) {
   PL_ARG(K && dist5 && out && width > 0 && height > 0 && width < 32000 && height < 32000);
   int rc = require_device(); if (rc) return rc;
-  PLUndistort* h = new PLUndistort;
+  std::unique_ptr<PLUndistort> h(new PLUndistort);
   h->w = width; h->h = height; h->cam = make_cam(K, dist5);
   memcpy(h->K, K, 16); memcpy(h->D, dist5, 20);
   const CamD& c = h->cam;
@@ -124,13 +122,12 @@ extern "C" int pl_undistort_create(const float* K, const float* dist5, int width
         for (int k = 0; k < 4; k++) tab[(i * 32 + j) * 4 + k] = iw[k];
       }
   }
-  cudaError_t e = cudaMalloc((void**)&h->d_map, map.size() * sizeof(RemapEntry));
-  if (e == cudaSuccess) e = cudaMemcpy(h->d_map, map.data(), map.size() * sizeof(RemapEntry), cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) e = cudaMalloc((void**)&h->d_tab, sizeof(tab));
-  if (e == cudaSuccess) e = cudaMemcpy(h->d_tab, tab, sizeof(tab), cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking);
-  if (e != cudaSuccess) { set_error("pl_undistort_create: %s", cudaGetErrorString(e)); pl_undistort_destroy(h); return PL_ERR_CUDA; }
-  *out = h;
+  PL_TRY(h->d_map.alloc(map.size()));
+  PL_CUDA(cudaMemcpy(h->d_map, map.data(), map.size() * sizeof(RemapEntry), cudaMemcpyHostToDevice));
+  PL_TRY(h->d_tab.alloc(sizeof(tab) / sizeof(int4)));
+  PL_CUDA(cudaMemcpy(h->d_tab, tab, sizeof(tab), cudaMemcpyHostToDevice));
+  PL_TRY(h->stream.create(cudaStreamNonBlocking));
+  *out = h.release();
   return PL_OK;
 }
 extern "C" int pl_undistort_remap_batch_dev(PLUndistort* h, const uint8_t* src, int sstride, size_t sframe, int B, uint8_t* dst,
@@ -144,11 +141,16 @@ extern "C" int pl_undistort_remap_batch_dev(PLUndistort* h, const uint8_t* src, 
 extern "C" int pl_undistort_remap(PLUndistort* h, const uint8_t* src, int sstride, uint8_t* dst, int dstride) {
   PL_ARG(h && src && dst && sstride >= h->w && dstride >= h->w);
   const size_t n = (size_t)h->w * h->h;
-  if (!h->staged) { PL_CUDA(cudaMalloc((void**)&h->d_src, n)); PL_CUDA(cudaMalloc((void**)&h->d_dst, n)); h->staged = 1; }
-  PL_CUDA(cudaMemcpy2DAsync(h->d_src, h->w, src, sstride, h->w, h->h, cudaMemcpyHostToDevice, h->stream));
-  int rc = pl_undistort_remap_batch_dev(h, h->d_src, h->w, n, 1, h->d_dst, h->w, n, h->stream);
+  if (!h->io) {
+    auto io = std::make_unique<PLUndistort::HostStaging>();
+    PL_TRY(io->d_src.alloc(n));
+    PL_TRY(io->d_dst.alloc(n));
+    h->io = std::move(io);
+  }
+  PL_CUDA(cudaMemcpy2DAsync(h->io->d_src, h->w, src, sstride, h->w, h->h, cudaMemcpyHostToDevice, h->stream));
+  int rc = pl_undistort_remap_batch_dev(h, h->io->d_src, h->w, n, 1, h->io->d_dst, h->w, n, h->stream);
   if (rc) return rc;
-  PL_CUDA(cudaMemcpy2DAsync(dst, dstride, h->d_dst, h->w, h->w, h->h, cudaMemcpyDeviceToHost, h->stream));
+  PL_CUDA(cudaMemcpy2DAsync(dst, dstride, h->io->d_dst, h->w, h->w, h->h, cudaMemcpyDeviceToHost, h->stream));
   PL_CUDA(cudaStreamSynchronize(h->stream));
   return PL_OK;
 }

@@ -85,77 +85,62 @@ using namespace pl;
 
 struct PLFrontend {
   PLFrontendConfig cfg;
-  PLOrb* orb = nullptr;
-  PLLine* line = nullptr;
-  cudaStream_t stream = nullptr;
-  cudaStream_t sLine = nullptr, sLm = nullptr;      // side streams: LSD/LBD chain and the LM run beside the ORB chain
-  cudaEvent_t evStart = nullptr, evLine = nullptr, evLm = nullptr;
+  Owned<PLOrb, pl_orb_destroy> orb;
+  Owned<PLLine, pl_line_destroy> line;
+  Stream stream;
+  Stream sLine, sLm;      // side streams: LSD/LBD chain and the LM run beside the ORB chain
+  Event evStart, evLine, evLm;
   int overlap = 0;
   int serial_batch = 0;          // batches of at least this many frames run the three chains on one stream (see pl_frontend_create)
   int B = 0, capK = 0, capL = 0;
   // device-resident per-batch state
-  uint8_t* d_img = nullptr;
+  DevBuf<uint8_t> d_img;
   PLKeyPoint* d_kps = nullptr; uint8_t* d_desc = nullptr; int* d_n = nullptr;
-  void* d_kl = nullptr; uint8_t* d_ldesc = nullptr; double* d_lf = nullptr; int* d_nl = nullptr;
-  float* d_bounds = nullptr; float* d_pm = nullptr; int* d_m12 = nullptr; int* d_nm = nullptr; int* d_scr = nullptr;
-  int* d_lm = nullptr; int* d_nlm = nullptr;
+  void* d_kl = nullptr; uint8_t* d_ldesc = nullptr; DevBuf<double> d_lf; int* d_nl = nullptr;
+  DevBuf<float> d_bounds, d_pm; DevBuf<int> d_m12, d_nm, d_scr;
+  DevBuf<int> d_lm, d_nlm;
   // rotated views so that "previous frame" is a plain pointer offset: copies of frame B-1 placed before frame 0
-  PLKeyPoint* d_kps_prev = nullptr; uint8_t* d_desc_prev = nullptr; int* d_n_prev = nullptr;
-  uint8_t* d_ldesc_prev = nullptr; int* d_nl_prev = nullptr;
-  uint8_t* d_kl_prev = nullptr;          // keylines hold B+1 slots like the descriptors (d_kl = slot 1)
+  DevBuf<PLKeyPoint> d_kps_prev; DevBuf<uint8_t> d_desc_prev; DevBuf<int> d_n_prev;
+  DevBuf<uint8_t> d_ldesc_prev; DevBuf<int> d_nl_prev;
+  DevBuf<uint8_t> d_kl_prev;             // keylines hold B+1 slots like the descriptors (d_kl = slot 1)
   char order[4] = {'L', 'O', 'M', 0};
   // steady-state tracking stage (pl_frontend_set_tracking): the map seen from frame b is frame b-1's features (see k_track_points)
   int tracking = 0;
-  float* d_sf = nullptr;
-  float *d_tpos = nullptr, *d_tang = nullptr, *d_tproj = nullptr, *d_tvcos = nullptr;
-  int *d_toct = nullptr, *d_tm1 = nullptr, *d_tnm1 = nullptr, *d_tm2 = nullptr, *d_tnm2 = nullptr;
-  uint8_t *d_tvalid = nullptr, *d_tview = nullptr, *d_tpre = nullptr;
-  float *d_lqproj = nullptr, *d_lqlen = nullptr, *d_lqvcos = nullptr;
-  int *d_lm1 = nullptr, *d_lnm1 = nullptr, *d_lm2 = nullptr, *d_lnm2 = nullptr;
-  uint8_t *d_lqvalid = nullptr, *d_lqview = nullptr, *d_lpre = nullptr, *d_lscratch = nullptr;
+  struct Tracking {
+    DevBuf<float> d_sf, d_tpos, d_tang, d_tproj, d_tvcos;
+    DevBuf<int> d_toct, d_tm1, d_tnm1, d_tm2, d_tnm2;
+    DevBuf<uint8_t> d_tvalid, d_tview, d_tpre;
+    DevBuf<float> d_lqproj, d_lqlen, d_lqvcos;
+    DevBuf<int> d_lm1, d_lnm1, d_lm2, d_lnm2;
+    DevBuf<uint8_t> d_lqvalid, d_lqview, d_lpre, d_lscratch;
+  };
+  std::unique_ptr<Tracking> tr;          // made on the first pl_frontend_set_tracking(h, 1)
   // LM problems
-  float *d_T0 = nullptr, *d_K = nullptr, *d_pobs = nullptr, *d_pw = nullptr, *d_pX = nullptr, *d_Tout = nullptr;
-  double *d_lfun = nullptr, *d_lX = nullptr, *d_scratch = nullptr;
-  int *d_np = nullptr, *d_nl_lm = nullptr, *d_inl = nullptr, *d_its = nullptr;
-  uint8_t *d_pout = nullptr, *d_lout = nullptr;
+  DevBuf<float> d_T0, d_K, d_pobs, d_pw, d_pX, d_Tout;
+  DevBuf<double> d_lfun, d_lX, d_scratch;
+  DevBuf<int> d_np, d_nl_lm, d_inl, d_its;
+  DevBuf<uint8_t> d_pout, d_lout;
   // camera (pl_frontend_set_camera): undistortion map (bound to the line handle), undistorted keypoints (B+1 slots like d_kps)
-  PLUndistort* und = nullptr;
-  PLKeyPoint* d_kpsu_prev = nullptr;
-  // streaming (pl_frontend_submit / pl_frontend_wait): two input buffers, one output snapshot, copy streams
-  uint8_t* d_in[2] = {nullptr, nullptr};
-  uint8_t* d_stage = nullptr;
-  cudaStream_t sUp = nullptr, sDown = nullptr;
-  cudaEvent_t evUp[2] = {nullptr, nullptr}, evFree[2] = {nullptr, nullptr}, evSnap = nullptr, evOut = nullptr;
-  cudaEvent_t evStep[2] = {nullptr, nullptr};   // host outputs of submit #c are complete when evStep[c & 1] fires
+  Owned<PLUndistort, pl_undistort_destroy> und;
+  DevBuf<PLKeyPoint> d_kpsu_prev;
+  // streaming (pl_frontend_submit / pl_frontend_wait): two input buffers, one output snapshot, copy streams; made on first use
+  struct Streaming {
+    DevBuf<uint8_t> d_in[2], d_stage;
+    Stream sUp, sDown;
+    Event evUp[2], evFree[2], evSnap, evOut;
+    Event evStep[2];   // host outputs of submit #c are complete when evStep[c & 1] fires
+  };
+  std::unique_ptr<Streaming> io;
   int slot = 0;
   long long submitted = 0, completed = 0;
   int wrap = 0;       // 1: frame 0 is matched against the LAST frame of the same batch (closed loop); 0: against the last frame of the previous step
-  float* d_orb_tab = nullptr;
+  DevBuf<float> d_orb_tab;
   int last_B = 0;                       // frames of the last step (0: none yet) and where its mvKeysUn are
   const PLKeyPoint* last_ku = nullptr;   // mvScaleFactors, mvInvLevelSigma2 for pl_frontend_track_local_map_dev (made on first use)
 };
 
 extern "C" void pl_frontend_destroy(PLFrontend* h) {
   if (!h) return;
-  pl_orb_destroy(h->orb); pl_line_destroy(h->line); pl_undistort_destroy(h->und);
-  cudaFree(h->d_kpsu_prev); cudaFree(h->d_orb_tab);
-  cudaFree(h->d_in[0]); cudaFree(h->d_in[1]); cudaFree(h->d_stage);
-  if (h->sUp) cudaStreamDestroy(h->sUp);
-  if (h->sDown) cudaStreamDestroy(h->sDown);
-  for (cudaEvent_t e : {h->evUp[0], h->evUp[1], h->evFree[0], h->evFree[1], h->evSnap, h->evOut, h->evStep[0], h->evStep[1]}) if (e) cudaEventDestroy(e);
-  void* ptrs[] = {h->d_img, h->d_kl_prev, h->d_sf, h->d_tpos, h->d_tang, h->d_tproj, h->d_tvcos, h->d_toct, h->d_tm1, h->d_tnm1, h->d_tm2, h->d_tnm2,
-                  h->d_tvalid, h->d_tview, h->d_tpre, h->d_lqproj, h->d_lqlen, h->d_lqvcos, h->d_lm1, h->d_lnm1, h->d_lm2, h->d_lnm2,
-                  h->d_lqvalid, h->d_lqview, h->d_lpre, h->d_lscratch, h->d_lf, h->d_bounds, h->d_pm, h->d_m12,
-                  h->d_nm, h->d_scr, h->d_lm, h->d_nlm, h->d_kps_prev, h->d_desc_prev, h->d_n_prev, h->d_ldesc_prev, h->d_nl_prev,
-                  h->d_T0, h->d_K, h->d_pobs, h->d_pw, h->d_pX, h->d_Tout, h->d_lfun, h->d_lX, h->d_scratch, h->d_np, h->d_nl_lm,
-                  h->d_inl, h->d_its, h->d_pout, h->d_lout};
-  for (void* p : ptrs) cudaFree(p);
-  if (h->stream) cudaStreamDestroy(h->stream);
-  if (h->sLine) cudaStreamDestroy(h->sLine);
-  if (h->sLm) cudaStreamDestroy(h->sLm);
-  if (h->evStart) cudaEventDestroy(h->evStart);
-  if (h->evLine) cudaEventDestroy(h->evLine);
-  if (h->evLm) cudaEventDestroy(h->evLm);
   delete h;
 }
 
@@ -163,22 +148,20 @@ extern "C" int pl_frontend_create(const PLFrontendConfig* cfg, PLFrontend** out)
   PL_ARG(cfg && out && cfg->max_batch >= 1 && cfg->lm_cap_points >= 1 && cfg->lm_cap_lines >= 1);
   int rc = require_device();
   if (rc) return rc;
-  PLFrontend* h = new PLFrontend;
+  std::unique_ptr<PLFrontend> h(new PLFrontend);
   h->cfg = *cfg;
   h->B = cfg->max_batch;
-#define FE_TRY(e) do { int _r = (e); if (_r) { pl_frontend_destroy(h); return _r; } } while (0)
-#define FE_CUDA(e) do { cudaError_t _e = (e); if (_e != cudaSuccess) { set_error("%s -> %s", #e, cudaGetErrorString(_e)); pl_frontend_destroy(h); return PL_ERR_CUDA; } } while (0)
   PLOrbConfig oc = {cfg->width, cfg->height, cfg->orb_nfeatures, cfg->orb_scale_factor, cfg->orb_nlevels, cfg->orb_ini_th, cfg->orb_min_th, cfg->max_batch, 0};
-  FE_TRY(pl_orb_create(&oc, &h->orb));
+  PLOrb* orb = nullptr;
+  PL_TRY(pl_orb_create(&oc, &orb));
+  h->orb.reset(orb);
   PLLineConfig lc = {cfg->width, cfg->height, cfg->line_nfeatures, cfg->line_min_length, cfg->max_batch, 0, 0};
-  FE_TRY(pl_line_create(&lc, &h->line));
-  h->capK = pl_orb_capacity(h->orb); h->capL = pl_line_capacity(h->line);
-  FE_CUDA(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
-  FE_CUDA(cudaStreamCreateWithFlags(&h->sLine, cudaStreamNonBlocking));
-  FE_CUDA(cudaStreamCreateWithFlags(&h->sLm, cudaStreamNonBlocking));
-  FE_CUDA(cudaEventCreateWithFlags(&h->evStart, cudaEventDisableTiming));
-  FE_CUDA(cudaEventCreateWithFlags(&h->evLine, cudaEventDisableTiming));
-  FE_CUDA(cudaEventCreateWithFlags(&h->evLm, cudaEventDisableTiming));
+  PLLine* line = nullptr;
+  PL_TRY(pl_line_create(&lc, &line));
+  h->line.reset(line);
+  h->capK = pl_orb_capacity(orb); h->capL = pl_line_capacity(line);
+  for (Stream* s : {&h->stream, &h->sLine, &h->sLm}) PL_TRY(s->create(cudaStreamNonBlocking));
+  for (Event* e : {&h->evStart, &h->evLine, &h->evLm}) PL_TRY(e->create(cudaEventDisableTiming));
   // The three chains run on separate streams (PLSLAM_FRONTEND_OVERLAP=0: one stream): the low-occupancy kernels (matchers,
   // quadtree, pose optimisation) fill the tails of the others.  Not from 32 frames per SM on: there k_lsd_grow_ordered is one
   // wave of one-warp CTAs that holds all 32 block slots and the whole register file of every SM, so the other chains are only
@@ -187,8 +170,8 @@ extern "C" int pl_frontend_create(const PLFrontendConfig* cfg, PLFrontend** out)
   { const char* e = getenv("PLSLAM_FRONTEND_OVERLAP"); h->overlap = !(e && e[0] == '0'); }
   {
     int dev = 0, sms = 132;
-    FE_CUDA(cudaGetDevice(&dev));
-    FE_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    PL_CUDA(cudaGetDevice(&dev));
+    PL_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
     h->serial_batch = pl::kSerialFramesPerSM * sms;
   }
   if (const char* e = getenv("PLSLAM_FRONTEND_ORDER")) {
@@ -196,28 +179,28 @@ extern "C" int pl_frontend_create(const PLFrontendConfig* cfg, PLFrontend** out)
     if (o.size() == 3 && o.find('L') != std::string::npos && o.find('O') != std::string::npos && o.find('M') != std::string::npos) memcpy(h->order, o.data(), 3);
   }
   const size_t B = h->B, cK = h->capK, cL = h->capL, cp = cfg->lm_cap_points, cl = cfg->lm_cap_lines;
-  FE_TRY(dev_alloc(&h->d_img, (size_t)cfg->width * cfg->height * B));
+  PL_TRY(h->d_img.alloc((size_t)cfg->width * cfg->height * B));
   // feature arrays hold B+1 frames: slot 0 = copy of the batch's last frame ("previous" of frame 0), slots 1..B = frames
-  FE_TRY(dev_alloc(&h->d_kps_prev, cK * (B + 1))); h->d_kps = h->d_kps_prev + cK;
-  FE_TRY(dev_alloc(&h->d_desc_prev, cK * 32 * (B + 1))); h->d_desc = h->d_desc_prev + cK * 32;
-  FE_TRY(dev_alloc(&h->d_n_prev, B + 1)); h->d_n = h->d_n_prev + 1;
-  FE_CUDA(cudaMemset(h->d_n_prev, 0, sizeof(int) * (B + 1)));      // before the first step frame 0 has no predecessor
-  FE_TRY(dev_alloc(&h->d_ldesc_prev, cL * 32 * (B + 1))); h->d_ldesc = h->d_ldesc_prev + cL * 32;
-  FE_TRY(dev_alloc(&h->d_nl_prev, B + 1)); h->d_nl = h->d_nl_prev + 1;
-  FE_CUDA(cudaMemset(h->d_nl_prev, 0, sizeof(int) * (B + 1)));
-  FE_TRY(dev_alloc(&h->d_kl_prev, cL * 68 * (B + 1))); h->d_kl = h->d_kl_prev + cL * 68;
-  FE_TRY(dev_alloc(&h->d_lf, cL * 3 * B));
-  FE_TRY(dev_alloc(&h->d_bounds, 4)); FE_TRY(dev_alloc(&h->d_pm, cK * 2 * B)); FE_TRY(dev_alloc(&h->d_m12, cK * B));
-  FE_TRY(dev_alloc(&h->d_nm, B)); FE_TRY(dev_alloc(&h->d_scr, cK * 2 * B)); FE_TRY(dev_alloc(&h->d_lm, cL * B)); FE_TRY(dev_alloc(&h->d_nlm, B));
+  PL_TRY(h->d_kps_prev.alloc(cK * (B + 1))); h->d_kps = h->d_kps_prev + cK;
+  PL_TRY(h->d_desc_prev.alloc(cK * 32 * (B + 1))); h->d_desc = h->d_desc_prev + cK * 32;
+  PL_TRY(h->d_n_prev.alloc(B + 1)); h->d_n = h->d_n_prev + 1;
+  PL_CUDA(cudaMemset(h->d_n_prev, 0, sizeof(int) * (B + 1)));      // before the first step frame 0 has no predecessor
+  PL_TRY(h->d_ldesc_prev.alloc(cL * 32 * (B + 1))); h->d_ldesc = h->d_ldesc_prev + cL * 32;
+  PL_TRY(h->d_nl_prev.alloc(B + 1)); h->d_nl = h->d_nl_prev + 1;
+  PL_CUDA(cudaMemset(h->d_nl_prev, 0, sizeof(int) * (B + 1)));
+  PL_TRY(h->d_kl_prev.alloc(cL * 68 * (B + 1))); h->d_kl = h->d_kl_prev + cL * 68;
+  PL_TRY(h->d_lf.alloc(cL * 3 * B));
+  PL_TRY(h->d_bounds.alloc(4)); PL_TRY(h->d_pm.alloc(cK * 2 * B)); PL_TRY(h->d_m12.alloc(cK * B));
+  PL_TRY(h->d_nm.alloc(B)); PL_TRY(h->d_scr.alloc(cK * 2 * B)); PL_TRY(h->d_lm.alloc(cL * B)); PL_TRY(h->d_nlm.alloc(B));
   float bounds[4] = {0.f, 0.f, (float)cfg->width, (float)cfg->height};   // Frame::ComputeImageBounds without distortion
-  FE_CUDA(cudaMemcpy(h->d_bounds, bounds, sizeof(bounds), cudaMemcpyHostToDevice));
-  FE_TRY(dev_alloc(&h->d_T0, 16 * B)); FE_TRY(dev_alloc(&h->d_K, 4 * B)); FE_TRY(dev_alloc(&h->d_pobs, cp * 2 * B));
-  FE_TRY(dev_alloc(&h->d_pw, cp * B)); FE_TRY(dev_alloc(&h->d_pX, cp * 3 * B)); FE_TRY(dev_alloc(&h->d_Tout, 16 * B * 2));
-  FE_TRY(dev_alloc(&h->d_lfun, cl * 3 * B)); FE_TRY(dev_alloc(&h->d_lX, cl * 6 * B));
-  FE_TRY(dev_alloc(&h->d_scratch, pl_pose_optimization_scratch_doubles((int)B, (int)cp, (int)cl)));
-  FE_TRY(dev_alloc(&h->d_np, B)); FE_TRY(dev_alloc(&h->d_nl_lm, B)); FE_TRY(dev_alloc(&h->d_inl, B * 2)); FE_TRY(dev_alloc(&h->d_its, B * 2));
-  FE_TRY(dev_alloc(&h->d_pout, cp * B * 2)); FE_TRY(dev_alloc(&h->d_lout, cl * B * 2));
-  *out = h;
+  PL_CUDA(cudaMemcpy(h->d_bounds, bounds, sizeof(bounds), cudaMemcpyHostToDevice));
+  PL_TRY(h->d_T0.alloc(16 * B)); PL_TRY(h->d_K.alloc(4 * B)); PL_TRY(h->d_pobs.alloc(cp * 2 * B));
+  PL_TRY(h->d_pw.alloc(cp * B)); PL_TRY(h->d_pX.alloc(cp * 3 * B)); PL_TRY(h->d_Tout.alloc(16 * B * 2));
+  PL_TRY(h->d_lfun.alloc(cl * 3 * B)); PL_TRY(h->d_lX.alloc(cl * 6 * B));
+  PL_TRY(h->d_scratch.alloc(pl_pose_optimization_scratch_doubles((int)B, (int)cp, (int)cl)));
+  PL_TRY(h->d_np.alloc(B)); PL_TRY(h->d_nl_lm.alloc(B)); PL_TRY(h->d_inl.alloc(B * 2)); PL_TRY(h->d_its.alloc(B * 2));
+  PL_TRY(h->d_pout.alloc(cp * B * 2)); PL_TRY(h->d_lout.alloc(cl * B * 2));
+  *out = h.release();
   return PL_OK;
 }
 
@@ -280,23 +263,22 @@ extern "C" long long pl_frontend_set_pose_problems_async(PLFrontend* h, int B, c
 // Steady-state tracking stage on / off (default off).  Allocates its arrays on first use.
 extern "C" int pl_frontend_set_tracking(PLFrontend* h, int on) {
   PL_ARG(h);
-  if (on && !h->d_sf) {
+  if (on && !h->tr) {
     const size_t B = h->B, cK = h->capK, cL = h->capL;
     std::vector<float> sf(std::max(h->cfg.orb_nlevels, 1), 1.0f);
     for (size_t i = 1; i < sf.size(); i++) sf[i] = sf[i - 1] * h->cfg.orb_scale_factor;     // ORBextractor.cc:419-426
-    int rc;
-#define TR_TRY(e) do { if ((rc = (e))) return rc; } while (0)
-    TR_TRY(dev_alloc(&h->d_sf, sf.size()));
-    PL_CUDA(cudaMemcpy(h->d_sf, sf.data(), sf.size() * sizeof(float), cudaMemcpyHostToDevice));
-    TR_TRY(dev_alloc(&h->d_tpos, cK * 3 * B)); TR_TRY(dev_alloc(&h->d_tang, cK * B)); TR_TRY(dev_alloc(&h->d_tproj, cK * 2 * B));
-    TR_TRY(dev_alloc(&h->d_tvcos, cK * B)); TR_TRY(dev_alloc(&h->d_toct, cK * B)); TR_TRY(dev_alloc(&h->d_tm1, cK * B)); TR_TRY(dev_alloc(&h->d_tnm1, B));
-    TR_TRY(dev_alloc(&h->d_tm2, cK * B)); TR_TRY(dev_alloc(&h->d_tnm2, B)); TR_TRY(dev_alloc(&h->d_tvalid, cK * B)); TR_TRY(dev_alloc(&h->d_tview, cK * B));
-    TR_TRY(dev_alloc(&h->d_tpre, cK * B));
-    TR_TRY(dev_alloc(&h->d_lqproj, cL * 4 * B)); TR_TRY(dev_alloc(&h->d_lqlen, cL * B)); TR_TRY(dev_alloc(&h->d_lqvcos, cL * B));
-    TR_TRY(dev_alloc(&h->d_lm1, cL * B)); TR_TRY(dev_alloc(&h->d_lnm1, B)); TR_TRY(dev_alloc(&h->d_lm2, cL * B)); TR_TRY(dev_alloc(&h->d_lnm2, B));
-    TR_TRY(dev_alloc(&h->d_lqvalid, cL * B)); TR_TRY(dev_alloc(&h->d_lqview, cL * B)); TR_TRY(dev_alloc(&h->d_lpre, cL * B));
-    TR_TRY(dev_alloc(&h->d_lscratch, pl_lsd_search_scratch_bytes((int)cL, (int)B)));
-#undef TR_TRY
+    auto t = std::make_unique<PLFrontend::Tracking>();
+    PL_TRY(t->d_sf.alloc(sf.size()));
+    PL_CUDA(cudaMemcpy(t->d_sf, sf.data(), sf.size() * sizeof(float), cudaMemcpyHostToDevice));
+    PL_TRY(t->d_tpos.alloc(cK * 3 * B)); PL_TRY(t->d_tang.alloc(cK * B)); PL_TRY(t->d_tproj.alloc(cK * 2 * B));
+    PL_TRY(t->d_tvcos.alloc(cK * B)); PL_TRY(t->d_toct.alloc(cK * B)); PL_TRY(t->d_tm1.alloc(cK * B)); PL_TRY(t->d_tnm1.alloc(B));
+    PL_TRY(t->d_tm2.alloc(cK * B)); PL_TRY(t->d_tnm2.alloc(B)); PL_TRY(t->d_tvalid.alloc(cK * B)); PL_TRY(t->d_tview.alloc(cK * B));
+    PL_TRY(t->d_tpre.alloc(cK * B));
+    PL_TRY(t->d_lqproj.alloc(cL * 4 * B)); PL_TRY(t->d_lqlen.alloc(cL * B)); PL_TRY(t->d_lqvcos.alloc(cL * B));
+    PL_TRY(t->d_lm1.alloc(cL * B)); PL_TRY(t->d_lnm1.alloc(B)); PL_TRY(t->d_lm2.alloc(cL * B)); PL_TRY(t->d_lnm2.alloc(B));
+    PL_TRY(t->d_lqvalid.alloc(cL * B)); PL_TRY(t->d_lqview.alloc(cL * B)); PL_TRY(t->d_lpre.alloc(cL * B));
+    PL_TRY(t->d_lscratch.alloc(pl_lsd_search_scratch_bytes((int)cL, (int)B)));
+    h->tr = std::move(t);
   }
   h->tracking = on ? 1 : 0;
   return PL_OK;
@@ -305,23 +287,24 @@ extern "C" int pl_frontend_set_tracking(PLFrontend* h, int on) {
 // of the previous frame's feature (-1 none); which: 0 = motion-model search, 1 = local-map search.
 extern "C" int pl_frontend_fetch_tracking(PLFrontend* h, int B, int which, int* point_match, int* n_point_matches, int* line_match,
                                           int* n_line_matches, float* map_pos, uint8_t* point_in_view, uint8_t* line_in_view) {
-  PL_ARG(h && h->tracking && h->d_sf && B >= 1 && B <= h->B && (which == 0 || which == 1));
+  PL_ARG(h && h->tracking && B >= 1 && B <= h->B && (which == 0 || which == 1));
+  const PLFrontend::Tracking& t = *h->tr;
   const size_t cK = h->capK, cL = h->capL;
   PL_CUDA(cudaStreamSynchronize(h->stream));
-  if (point_match) PL_CUDA(cudaMemcpy(point_match, which ? h->d_tm2 : h->d_tm1, cK * B * sizeof(int), cudaMemcpyDeviceToHost));
-  if (n_point_matches) PL_CUDA(cudaMemcpy(n_point_matches, which ? h->d_tnm2 : h->d_tnm1, B * sizeof(int), cudaMemcpyDeviceToHost));
-  if (line_match) PL_CUDA(cudaMemcpy(line_match, which ? h->d_lm2 : h->d_lm1, cL * B * sizeof(int), cudaMemcpyDeviceToHost));
-  if (n_line_matches) PL_CUDA(cudaMemcpy(n_line_matches, which ? h->d_lnm2 : h->d_lnm1, B * sizeof(int), cudaMemcpyDeviceToHost));
-  if (map_pos) PL_CUDA(cudaMemcpy(map_pos, h->d_tpos, cK * 3 * B * sizeof(float), cudaMemcpyDeviceToHost));
-  if (point_in_view) PL_CUDA(cudaMemcpy(point_in_view, which ? h->d_tview : h->d_tvalid, cK * B, cudaMemcpyDeviceToHost));
-  if (line_in_view) PL_CUDA(cudaMemcpy(line_in_view, which ? h->d_lqview : h->d_lqvalid, cL * B, cudaMemcpyDeviceToHost));
+  if (point_match) PL_CUDA(cudaMemcpy(point_match, which ? t.d_tm2 : t.d_tm1, cK * B * sizeof(int), cudaMemcpyDeviceToHost));
+  if (n_point_matches) PL_CUDA(cudaMemcpy(n_point_matches, which ? t.d_tnm2 : t.d_tnm1, B * sizeof(int), cudaMemcpyDeviceToHost));
+  if (line_match) PL_CUDA(cudaMemcpy(line_match, which ? t.d_lm2 : t.d_lm1, cL * B * sizeof(int), cudaMemcpyDeviceToHost));
+  if (n_line_matches) PL_CUDA(cudaMemcpy(n_line_matches, which ? t.d_lnm2 : t.d_lnm1, B * sizeof(int), cudaMemcpyDeviceToHost));
+  if (map_pos) PL_CUDA(cudaMemcpy(map_pos, t.d_tpos, cK * 3 * B * sizeof(float), cudaMemcpyDeviceToHost));
+  if (point_in_view) PL_CUDA(cudaMemcpy(point_in_view, which ? t.d_tview : t.d_tvalid, cK * B, cudaMemcpyDeviceToHost));
+  if (line_in_view) PL_CUDA(cudaMemcpy(line_in_view, which ? t.d_lqview : t.d_lqvalid, cL * B, cudaMemcpyDeviceToHost));
   return PL_OK;
 }
 extern "C" int pl_frontend_set_wrap(PLFrontend* h, int on) { PL_ARG(h); h->wrap = on ? 1 : 0; return PL_OK; }
 extern "C" int pl_frontend_check_overflow(PLFrontend* h) {
   PL_ARG(h);
-  int rc = pl_orb_check_overflow(h->orb);
-  const int rc2 = pl_line_check_overflow(h->line);
+  int rc = pl_orb_check_overflow(h->orb.get());
+  const int rc2 = pl_line_check_overflow(h->line.get());
   return rc ? rc : rc2;
 }
 
@@ -346,7 +329,7 @@ extern "C" int pl_frontend_run_dev(PLFrontend* h, const uint8_t* imgs, int strid
   auto line_chain = [&]() -> int {
   // --- line chain (on the undistorted frames when the camera has distortion, Frame.cc:220-225: the line handle undistorts the
   // raw frames with the camera's map, pl_frontend_set_camera)
-  if ((rc = pl_line_extract_batch_dev(h->line, imgs, stride, frame_stride, B, nullptr, h->d_kl, h->d_ldesc, h->d_lf, h->d_nl, sL))) return rc;
+  if ((rc = pl_line_extract_batch_dev(h->line.get(), imgs, stride, frame_stride, B, nullptr, h->d_kl, h->d_ldesc, h->d_lf, h->d_nl, sL))) return rc;
   // slot 0 of every feature array is "the frame before frame 0": the last frame of the PREVIOUS step (sequence replay: the
   // copy follows the matching), or, in wrap mode, the last frame of this batch (the copy precedes the matching)
   auto carry_lines = [&]() -> int {
@@ -359,28 +342,29 @@ extern "C" int pl_frontend_run_dev(PLFrontend* h, const uint8_t* imgs, int strid
   if ((rc = pl_lsd_search_double_dev(h->d_ldesc_prev, h->d_nl_prev, h->d_ldesc, h->d_nl, (int)cL, (int)cL, B, 50.f, 0.7f, 1, h->d_lm,
                                      h->d_nlm, sL))) return rc;
   if (h->tracking) {   // lines: TrackWithMotionModel (Tracking.cc:1347, th = 15) then SearchLocalLines (:1855, th = 1), LSDmatcher(0.7)
+    const PLFrontend::Tracking& t = *h->tr;
     const dim3 g((unsigned)((cL + 127) / 128), B);
-    k_track_lines<<<g, 128, 0, sL>>>((const KL68*)h->d_kl_prev, h->d_nl_prev, (int)cL, h->d_lqvalid, h->d_lqproj, h->d_lqlen, h->d_lqvcos);
+    k_track_lines<<<g, 128, 0, sL>>>((const KL68*)h->d_kl_prev.get(), h->d_nl_prev, (int)cL, t.d_lqvalid, t.d_lqproj, t.d_lqlen, t.d_lqvcos);
     PL_LAUNCH_CHECK();
-    if ((rc = pl_lsd_search_by_projection_dev(0, h->d_kl, h->d_lf, h->d_ldesc, h->d_nl, (int)cL, B, h->d_bounds, h->d_nl_prev, (int)cL, h->d_lqvalid,
-                                              h->d_lqproj, h->d_ldesc_prev, h->d_lqlen, 15.f, 0.7f, nullptr, h->d_lm1, h->d_lnm1, h->d_lscratch, sL))) return rc;
-    k_track_mark<<<B, 256, 0, sL>>>(h->d_lm1, h->d_nl, h->d_lqvalid, (int)cL, h->d_lqview, h->d_lpre);
+    if ((rc = pl_lsd_search_by_projection_dev(0, h->d_kl, h->d_lf, h->d_ldesc, h->d_nl, (int)cL, B, h->d_bounds, h->d_nl_prev, (int)cL, t.d_lqvalid,
+                                              t.d_lqproj, h->d_ldesc_prev, t.d_lqlen, 15.f, 0.7f, nullptr, t.d_lm1, t.d_lnm1, t.d_lscratch, sL))) return rc;
+    k_track_mark<<<B, 256, 0, sL>>>(t.d_lm1, h->d_nl, t.d_lqvalid, (int)cL, t.d_lqview, t.d_lpre);
     PL_LAUNCH_CHECK();
-    if ((rc = pl_lsd_search_by_projection_dev(1, h->d_kl, h->d_lf, h->d_ldesc, h->d_nl, (int)cL, B, h->d_bounds, h->d_nl_prev, (int)cL, h->d_lqview,
-                                              h->d_lqproj, h->d_ldesc_prev, h->d_lqvcos, 1.f, 0.7f, h->d_lpre, h->d_lm2, h->d_lnm2, h->d_lscratch, sL))) return rc;
+    if ((rc = pl_lsd_search_by_projection_dev(1, h->d_kl, h->d_lf, h->d_ldesc, h->d_nl, (int)cL, B, h->d_bounds, h->d_nl_prev, (int)cL, t.d_lqview,
+                                              t.d_lqproj, h->d_ldesc_prev, t.d_lqvcos, 1.f, 0.7f, t.d_lpre, t.d_lm2, t.d_lnm2, t.d_lscratch, sL))) return rc;
   }
   if (!h->wrap && (rc = carry_lines())) return rc;
   return PL_OK;
   };
   auto orb_chain = [&]() -> int {
   // --- ORB chain (slot 0 <- frame B-1 so that frame b's predecessor is slot b, a plain offset)
-  if ((rc = pl_orb_extract_batch_dev(h->orb, imgs, stride, frame_stride, B, h->d_kps, h->d_desc, h->d_n, st))) return rc;
+  if ((rc = pl_orb_extract_batch_dev(h->orb.get(), imgs, stride, frame_stride, B, h->d_kps, h->d_desc, h->d_n, st))) return rc;
   // mvKeysUn: the matcher works on undistorted keypoints (aliases of the raw ones without a distorting camera)
   const PLKeyPoint *ku_prev = h->d_kps_prev, *ku = h->d_kps;
   PLKeyPoint* kudst = nullptr;
   if (h->und) {
     kudst = h->d_kpsu_prev + cK;
-    if ((rc = pl_undistort_keypoints_dev(h->und, h->d_kps, h->d_n, (int)cK, B, kudst, st))) return rc;
+    if ((rc = pl_undistort_keypoints_dev(h->und.get(), h->d_kps, h->d_n, (int)cK, B, kudst, st))) return rc;
     ku_prev = h->d_kpsu_prev; ku = kudst;
   }
   auto carry_points = [&]() -> int {
@@ -396,19 +380,20 @@ extern "C" int pl_frontend_run_dev(PLFrontend* h, const uint8_t* imgs, int strid
   if ((rc = pl_orb_search_for_initialization_dev(ku_prev, h->d_desc_prev, h->d_n_prev, ku, h->d_desc, h->d_n, (int)cK, B,
                                                  h->d_bounds, h->d_pm, h->d_m12, h->d_nm, 100, 0.9f, 1, h->d_scr, st))) return rc;
   if (h->tracking) {   // points: TrackWithMotionModel (Tracking.cc:1345-1357: th = 15, again with 2 th if < 20 matches), SearchLocalPoints (:1799)
+    const PLFrontend::Tracking& t = *h->tr;
     const PLKeyPoint* kraw_prev = h->d_kps_prev;
     const dim3 g((unsigned)((cK + 127) / 128), B);
-    k_track_points<<<g, 128, 0, st>>>(ku_prev, kraw_prev, h->d_n_prev, (int)cK, h->d_T0, h->d_K, h->d_tvalid, h->d_tpos, h->d_toct, h->d_tang,
-                                      h->d_tproj, h->d_tvcos);
+    k_track_points<<<g, 128, 0, st>>>(ku_prev, kraw_prev, h->d_n_prev, (int)cK, h->d_T0, h->d_K, t.d_tvalid, t.d_tpos, t.d_toct, t.d_tang,
+                                      t.d_tproj, t.d_tvcos);
     PL_LAUNCH_CHECK();
     for (int pass = 0; pass < 2; pass++)
-      if ((rc = pl_orb_search_by_projection_last_dev(ku, h->d_desc, h->d_n, (int)cK, B, h->d_bounds, h->d_T0, h->d_K, h->d_sf, h->cfg.orb_nlevels,
-                                                     h->d_n_prev, (int)cK, h->d_tvalid, h->d_tpos, h->d_desc_prev, h->d_toct, h->d_tang,
-                                                     pass ? 30.f : 15.f, 1, nullptr, pass ? h->d_tnm1 : nullptr, 20, h->d_tm1, h->d_tnm1, st))) return rc;
-    k_track_mark<<<B, 256, 0, st>>>(h->d_tm1, h->d_n, h->d_tvalid, (int)cK, h->d_tview, h->d_tpre);
+      if ((rc = pl_orb_search_by_projection_last_dev(ku, h->d_desc, h->d_n, (int)cK, B, h->d_bounds, h->d_T0, h->d_K, t.d_sf, h->cfg.orb_nlevels,
+                                                     h->d_n_prev, (int)cK, t.d_tvalid, t.d_tpos, h->d_desc_prev, t.d_toct, t.d_tang,
+                                                     pass ? 30.f : 15.f, 1, nullptr, pass ? t.d_tnm1.get() : nullptr, 20, t.d_tm1, t.d_tnm1, st))) return rc;
+    k_track_mark<<<B, 256, 0, st>>>(t.d_tm1, h->d_n, t.d_tvalid, (int)cK, t.d_tview, t.d_tpre);
     PL_LAUNCH_CHECK();
-    if ((rc = pl_orb_search_by_projection_points_dev(ku, h->d_desc, h->d_n, (int)cK, B, h->d_bounds, h->d_sf, h->d_n_prev, (int)cK, h->d_tview,
-                                                     h->d_tproj, h->d_toct, h->d_tvcos, h->d_desc_prev, 1.f, 0.8f, h->d_tpre, h->d_tm2, h->d_tnm2, st))) return rc;
+    if ((rc = pl_orb_search_by_projection_points_dev(ku, h->d_desc, h->d_n, (int)cK, B, h->d_bounds, t.d_sf, h->d_n_prev, (int)cK, t.d_tview,
+                                                     t.d_tproj, t.d_toct, t.d_tvcos, h->d_desc_prev, 1.f, 0.8f, t.d_tpre, t.d_tm2, t.d_tnm2, st))) return rc;
   }
   if (!h->wrap && (rc = carry_points())) return rc;
   return PL_OK;
@@ -443,15 +428,17 @@ extern "C" int pl_frontend_run_dev(PLFrontend* h, const uint8_t* imgs, int strid
 extern "C" int pl_frontend_set_camera(PLFrontend* h, const float* K, const float* dist5) {
   PL_ARG(h && K && dist5);
   PL_CUDA(cudaDeviceSynchronize());
-  pl_line_set_undistort(h->line, nullptr);
-  pl_undistort_destroy(h->und); h->und = nullptr;
+  pl_line_set_undistort(h->line.get(), nullptr);
+  h->und.reset();
   float bounds[4];
   int rc = pl_frame_image_bounds(K, dist5, h->cfg.width, h->cfg.height, bounds);
   if (rc) return rc;
   if (dist5[0] != 0.0f) {
-    if ((rc = pl_undistort_create(K, dist5, h->cfg.width, h->cfg.height, &h->und))) return rc;
-    if ((rc = pl_line_set_undistort(h->line, h->und))) return rc;
-    if (!h->d_kpsu_prev && (rc = dev_alloc(&h->d_kpsu_prev, (size_t)h->capK * (h->B + 1)))) return rc;
+    if (!h->d_kpsu_prev && (rc = h->d_kpsu_prev.alloc((size_t)h->capK * (h->B + 1)))) return rc;
+    PLUndistort* und = nullptr;
+    if ((rc = pl_undistort_create(K, dist5, h->cfg.width, h->cfg.height, &und))) return rc;
+    h->und.reset(und);
+    if ((rc = pl_line_set_undistort(h->line.get(), und))) return rc;
   }
   PL_CUDA(cudaMemcpy(h->d_bounds, bounds, sizeof(bounds), cudaMemcpyHostToDevice));
   return PL_OK;
@@ -517,7 +504,7 @@ extern "C" int pl_frontend_wait(PLFrontend* h, int keep_in_flight) {
   PL_ARG(h && keep_in_flight >= 0 && keep_in_flight <= 1);
   bool finished = false;
   while (h->submitted - h->completed > keep_in_flight) {      // steps complete in submission order
-    PL_CUDA(cudaEventSynchronize(h->evStep[h->completed & 1]));
+    PL_CUDA(cudaEventSynchronize(h->io->evStep[h->completed & 1]));
     h->completed++;
     finished = true;
   }
@@ -531,48 +518,49 @@ extern "C" int pl_frontend_submit(PLFrontend* h, const uint8_t* imgs, int stride
          n_pt_matches && line_matches && n_line_matches && poses && inliers);
   const int W = h->cfg.width, H = h->cfg.height;
   size_t off[14];
-  if (!h->sUp) {   // first use: allocate the streaming state
+  if (!h->io) {   // first use: allocate the streaming state
     const size_t fb = (size_t)W * H * h->B;
-    int rc;
-    if ((rc = dev_alloc(&h->d_in[0], fb)) || (rc = dev_alloc(&h->d_in[1], fb)) || (rc = dev_alloc(&h->d_stage, fe_out_bytes(h, h->B, off)))) return rc;
-    PL_CUDA(cudaStreamCreateWithFlags(&h->sUp, cudaStreamNonBlocking));
-    PL_CUDA(cudaStreamCreateWithFlags(&h->sDown, cudaStreamNonBlocking));
-    for (cudaEvent_t* e : {&h->evUp[0], &h->evUp[1], &h->evFree[0], &h->evFree[1], &h->evSnap, &h->evOut, &h->evStep[0], &h->evStep[1]})
-      PL_CUDA(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
-    for (int k = 0; k < 2; k++) PL_CUDA(cudaEventRecord(h->evFree[k], h->stream));
-    PL_CUDA(cudaEventRecord(h->evOut, h->sDown));
+    auto io = std::make_unique<PLFrontend::Streaming>();
+    PL_TRY(io->d_in[0].alloc(fb)); PL_TRY(io->d_in[1].alloc(fb)); PL_TRY(io->d_stage.alloc(fe_out_bytes(h, h->B, off)));
+    PL_TRY(io->sUp.create(cudaStreamNonBlocking)); PL_TRY(io->sDown.create(cudaStreamNonBlocking));
+    for (Event* e : {&io->evUp[0], &io->evUp[1], &io->evFree[0], &io->evFree[1], &io->evSnap, &io->evOut, &io->evStep[0], &io->evStep[1]})
+      PL_TRY(e->create(cudaEventDisableTiming));
+    for (int k = 0; k < 2; k++) PL_CUDA(cudaEventRecord(io->evFree[k], h->stream));
+    PL_CUDA(cudaEventRecord(io->evOut, io->sDown));
+    h->io = std::move(io);
   }
+  PLFrontend::Streaming& io = *h->io;
   if (h->submitted - h->completed >= 2) { int rc = pl_frontend_wait(h, 1); if (rc) return rc; }   // at most two steps in flight
   fe_out_bytes(h, B, off);
   const int k = h->slot;
   cudaStream_t st = h->stream;
   // upload into buffer k once the step that last read it has finished
-  PL_CUDA(cudaStreamWaitEvent(h->sUp, h->evFree[k], 0));
+  PL_CUDA(cudaStreamWaitEvent(io.sUp, io.evFree[k], 0));
   if (stride == W && frame_stride == (size_t)W * H)
-    PL_CUDA(cudaMemcpyAsync(h->d_in[k], imgs, (size_t)W * H * B, cudaMemcpyHostToDevice, h->sUp));
+    PL_CUDA(cudaMemcpyAsync(io.d_in[k], imgs, (size_t)W * H * B, cudaMemcpyHostToDevice, io.sUp));
   else
     for (int b = 0; b < B; b++)
-      PL_CUDA(cudaMemcpy2DAsync(h->d_in[k] + (size_t)b * W * H, W, imgs + (size_t)b * frame_stride, stride, W, H, cudaMemcpyHostToDevice, h->sUp));
-  PL_CUDA(cudaEventRecord(h->evUp[k], h->sUp));
+      PL_CUDA(cudaMemcpy2DAsync(io.d_in[k] + (size_t)b * W * H, W, imgs + (size_t)b * frame_stride, stride, W, H, cudaMemcpyHostToDevice, io.sUp));
+  PL_CUDA(cudaEventRecord(io.evUp[k], io.sUp));
   // compute
-  PL_CUDA(cudaStreamWaitEvent(st, h->evUp[k], 0));
-  int rc = pl_frontend_run_dev(h, h->d_in[k], W, (size_t)W * H, B, st);
+  PL_CUDA(cudaStreamWaitEvent(st, io.evUp[k], 0));
+  int rc = pl_frontend_run_dev(h, io.d_in[k], W, (size_t)W * H, B, st);
   if (rc) return rc;
-  PL_CUDA(cudaEventRecord(h->evFree[k], st));
+  PL_CUDA(cudaEventRecord(io.evFree[k], st));
   // snapshot of the step's outputs (device to device), once the previous snapshot has left for the host
-  PL_CUDA(cudaStreamWaitEvent(st, h->evOut, 0));
+  PL_CUDA(cudaStreamWaitEvent(st, io.evOut, 0));
   const size_t cK = h->capK, cL = h->capL, b = B;
   const void* src[13] = {h->d_kps, h->d_desc, h->d_n, h->d_kl, h->d_ldesc, h->d_lf, h->d_nl, h->d_m12, h->d_nm, h->d_lm, h->d_nlm, h->d_Tout, h->d_inl};
   void* dst[13] = {kps, desc, n, keylines, ldesc, linefunc, nl, pt_matches, n_pt_matches, line_matches, n_line_matches, poses, inliers};
   const size_t sz[13] = {cK * b * sizeof(PLKeyPoint), cK * b * 32, b * 4, cL * b * 68, cL * b * 32, cL * b * 24, b * 4, cK * b * 4, b * 4,
                          cL * b * 4, b * 4, 64 * b * 2, 4 * b * 2};
-  for (int i = 0; i < 13; i++) PL_CUDA(cudaMemcpyAsync(h->d_stage + off[i], src[i], sz[i], cudaMemcpyDeviceToDevice, st));
-  PL_CUDA(cudaEventRecord(h->evSnap, st));
+  for (int i = 0; i < 13; i++) PL_CUDA(cudaMemcpyAsync(io.d_stage + off[i], src[i], sz[i], cudaMemcpyDeviceToDevice, st));
+  PL_CUDA(cudaEventRecord(io.evSnap, st));
   // download
-  PL_CUDA(cudaStreamWaitEvent(h->sDown, h->evSnap, 0));
-  for (int i = 0; i < 13; i++) PL_CUDA(cudaMemcpyAsync(dst[i], h->d_stage + off[i], sz[i], cudaMemcpyDeviceToHost, h->sDown));
-  PL_CUDA(cudaEventRecord(h->evOut, h->sDown));
-  PL_CUDA(cudaEventRecord(h->evStep[h->submitted & 1], h->sDown));
+  PL_CUDA(cudaStreamWaitEvent(io.sDown, io.evSnap, 0));
+  for (int i = 0; i < 13; i++) PL_CUDA(cudaMemcpyAsync(dst[i], io.d_stage + off[i], sz[i], cudaMemcpyDeviceToHost, io.sDown));
+  PL_CUDA(cudaEventRecord(io.evOut, io.sDown));
+  PL_CUDA(cudaEventRecord(io.evStep[h->submitted & 1], io.sDown));
   h->slot ^= 1;
   h->submitted++;
   return PL_OK;
@@ -612,9 +600,9 @@ extern "C" int pl_frontend_fetch(PLFrontend* h, int B, PLKeyPoint* kps, uint8_t*
 
 // hooks used by bench.py: timing of the dominant kernel and a device-to-device copy of the pose records that the
 // multi-GPU run all-gathers (SURVEY.md §8e)
-extern "C" int pl_frontend_set_timing(PLFrontend* h, int on) { PL_ARG(h); return pl_line_set_timing(h->line, on); }
-extern "C" int pl_frontend_grow_ms(PLFrontend* h, float* ms) { PL_ARG(h); return pl_line_grow_ms(h->line, ms); }
-extern "C" long long pl_frontend_grow_bytes_per_frame(const PLFrontend* h) { return h ? pl_line_grow_bytes_per_frame(h->line) : 0; }
+extern "C" int pl_frontend_set_timing(PLFrontend* h, int on) { PL_ARG(h); return pl_line_set_timing(h->line.get(), on); }
+extern "C" int pl_frontend_grow_ms(PLFrontend* h, float* ms) { PL_ARG(h); return pl_line_grow_ms(h->line.get(), ms); }
+extern "C" long long pl_frontend_grow_bytes_per_frame(const PLFrontend* h) { return h ? pl_line_grow_bytes_per_frame(h->line.get()) : 0; }
 extern "C" int pl_frontend_copy_poses_dev(PLFrontend* h, int B, float* dst, void* stream) {
   PL_ARG(h && dst && B >= 1 && B <= h->B);
   PL_CUDA(cudaMemcpyAsync(dst, h->d_Tout + 16 * (size_t)B, 64 * (size_t)B, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
@@ -678,9 +666,9 @@ extern "C" int pl_frontend_track_local_map_dev(PLFrontend* h, PLMap* map, int B,
   const int nlev = h->cfg.orb_nlevels;
   if (!h->d_orb_tab) {
     std::vector<float> tab(2 * (size_t)nlev);
-    int rc = pl_orb_tables(h->orb, tab.data(), nullptr, nullptr, tab.data() + nlev, nullptr, nullptr, nullptr);
+    int rc = pl_orb_tables(h->orb.get(), tab.data(), nullptr, nullptr, tab.data() + nlev, nullptr, nullptr, nullptr);
     if (rc) return rc;
-    if ((rc = dev_alloc(&h->d_orb_tab, tab.size()))) return rc;
+    if ((rc = h->d_orb_tab.alloc(tab.size()))) return rc;
     PL_CUDA(cudaMemcpy(h->d_orb_tab, tab.data(), tab.size() * sizeof(float), cudaMemcpyHostToDevice));
   }
   PLTrackFrames F;

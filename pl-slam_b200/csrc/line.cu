@@ -712,35 +712,35 @@ using namespace pl;
 struct PLLine {
   PLLineConfig cfg;
   LineParams P;
-  cudaStream_t stream = nullptr;
-  uint8_t* d_scaled = nullptr;
-  float2* d_seedcs = nullptr;
+  Stream stream;
+  DevBuf<uint8_t> d_scaled;
+  DevBuf<float2> d_seedcs;
   // region growing (lsd_grow_ordered.cuh): pixel records, squared gradients, region lists, far-pixel masks, weight table
-  int4* d_rec = nullptr; int* d_sq = nullptr;
-  unsigned *d_region = nullptr, *d_far = nullptr; double* d_wtab = nullptr;
+  DevBuf<int4> d_rec; DevBuf<int> d_sq;
+  DevBuf<unsigned> d_region, d_far; DevBuf<double> d_wtab;
   int region_stride = 0;                // words of d_region per frame
-  GradRec* d_gtab = nullptr; float2* d_gtab_seed = nullptr;   // (gx, gy) -> level-line record, built once (k_lsd_grad_table)
+  DevBuf<GradRec> d_gtab; DevBuf<float2> d_gtab_seed;   // (gx, gy) -> level-line record, built once (k_lsd_grad_table)
   // k_lsd_seed_order: pixels per CTA (Q) and per warp (U), order positions per CTA (S), dynamic shared memory, clusters
   // resident on the device (0: the frame does not fit the cluster, k_lsd_hist/scan/scatter sort it)
   int seed_q = 0, seed_u = 0, seed_s = 0, seed_clusters = 0;
   int seed_min_batch = 132 * kSerialFramesPerSM;   // default: the cluster sort from this batch on
   int last_seed_cluster = 0;            // the LAST call sorted with k_lsd_seed_order
   size_t seed_smem = 0;
-  unsigned short* d_counts = nullptr;   // k_lsd_hist/scan/scatter
-  int *d_offsets = nullptr, *d_ndef = nullptr, *d_maxs = nullptr, *d_nseg = nullptr, *d_overflow = nullptr;
-  unsigned* d_order = nullptr;
-  float4* d_segs = nullptr;
-  short2* d_dxy = nullptr;
-  // host-pointer API staging
-  uint8_t* d_img = nullptr; PLKeyLineRec* d_kls = nullptr; uint8_t* d_desc = nullptr; double* d_lf = nullptr; int* d_nl = nullptr;
-  uint8_t* d_mask = nullptr;
+  DevBuf<unsigned short> d_counts;     // k_lsd_hist/scan/scatter
+  DevBuf<int> d_offsets, d_ndef, d_maxs, d_nseg, d_overflow;
+  DevBuf<unsigned> d_order;
+  DevBuf<float4> d_segs;
+  DevBuf<short2> d_dxy;
+  // host-pointer API staging (made on first use)
+  struct HostStaging { DevBuf<uint8_t> d_img, d_desc, d_mask; DevBuf<PLKeyLineRec> d_kls; DevBuf<double> d_lf; DevBuf<int> d_nl; };
+  std::unique_ptr<HostStaging> io;
   const PLUndistort* und = nullptr;     // pl_line_set_undistort: the frames are raw, k_lsd_front undistorts them (owned by the caller)
-  uint8_t* d_und = nullptr;             // undistorted frames of batches below 32 frames per SM (made on first use)
+  DevBuf<uint8_t> d_und;                // undistorted frames of batches below 32 frames per SM (made on first use)
   size_t key_smem = 0;
   int last_B = 0;
   // optional device timing of the dominant kernel (bench.py roofline): events on the launching stream
   int timing = 0;
-  cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+  Event ev0, ev1;
 };
 
 static const unsigned char h_comb[64] = {0, 1, 0, 2, 0, 3, 0, 4, 0, 5, 0, 6, 1, 2, 1, 3, 1, 4, 1, 5, 1, 6, 2, 3, 2, 4, 2, 5, 2, 6, 2, 7,
@@ -748,11 +748,6 @@ static const unsigned char h_comb[64] = {0, 1, 0, 2, 0, 3, 0, 4, 0, 5, 0, 6, 1, 
 
 extern "C" void pl_line_destroy(PLLine* h) {
   if (!h) return;
-  cudaFree(h->d_gtab); cudaFree(h->d_gtab_seed); cudaFree(h->d_scaled); cudaFree(h->d_seedcs); cudaFree(h->d_rec); cudaFree(h->d_sq); cudaFree(h->d_region); cudaFree(h->d_far); cudaFree(h->d_wtab); cudaFree(h->d_counts); cudaFree(h->d_offsets);
-  cudaFree(h->d_ndef); cudaFree(h->d_maxs); cudaFree(h->d_nseg); cudaFree(h->d_overflow); cudaFree(h->d_order);
-  cudaFree(h->d_segs); cudaFree(h->d_dxy); cudaFree(h->d_und); cudaFree(h->d_img); cudaFree(h->d_kls);
-  cudaFree(h->d_desc); cudaFree(h->d_lf); cudaFree(h->d_nl); cudaFree(h->d_mask);
-  if (h->stream) cudaStreamDestroy(h->stream);
   delete h;
 }
 
@@ -761,7 +756,7 @@ extern "C" int pl_line_create(const PLLineConfig* cfg, PLLine** out) {
   PL_ARG(cfg->width >= 64 && cfg->height >= 64 && cfg->width < 8000 && cfg->height < 8000 && cfg->nfeatures > 0 && cfg->max_batch >= 1);
   int rc = require_device();
   if (rc) return rc;
-  PLLine* h = new PLLine;
+  std::unique_ptr<PLLine> h(new PLLine);
   h->cfg = *cfg;
   LineParams& P = h->P;
   P.w = cfg->width; P.h = cfg->height;
@@ -791,33 +786,31 @@ extern "C" int pl_line_create(const PLLineConfig* cfg, PLLine** out) {
   P.nfeatures = cfg->nfeatures; P.capL = cfg->nfeatures + 1; P.min_line_length = cfg->min_line_length;
   { size_t c2 = 1; while (c2 < (size_t)P.seg_cap) c2 <<= 1; h->key_smem = c2 * 8; }
   const size_t B = cfg->max_batch, npx = P.npx;
-#define LN_TRY(e) do { int _r = (e); if (_r) { pl_line_destroy(h); return _r; } } while (0)
-#define LN_CUDA(e) do { cudaError_t _e = (e); if (_e != cudaSuccess) { set_error("%s -> %s", #e, cudaGetErrorString(_e)); pl_line_destroy(h); return PL_ERR_CUDA; } } while (0)
-  LN_CUDA(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
-  LN_TRY(dev_alloc(&h->d_scaled, npx * B)); LN_TRY(dev_alloc(&h->d_seedcs, npx * B)); LN_TRY(dev_alloc(&h->d_rec, npx * B));
-  LN_TRY(dev_alloc(&h->d_sq, npx * B));
+  PL_TRY(h->stream.create(cudaStreamNonBlocking));
+  PL_TRY(h->d_scaled.alloc(npx * B)); PL_TRY(h->d_seedcs.alloc(npx * B)); PL_TRY(h->d_rec.alloc(npx * B));
+  PL_TRY(h->d_sq.alloc(npx * B));
   {
     int dev = 0, sms = 132;
     cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     h->seed_min_batch = sms * kSerialFramesPerSM;
     // a region holds at most npx pixels; reduce_round's swap-remove scratch follows it (fill_off = npx)
     h->region_stride = 2 * P.npx;
-    LN_TRY(dev_alloc(&h->d_region, (size_t)h->region_stride * B)); LN_TRY(dev_alloc(&h->d_far, npx * B));
+    PL_TRY(h->d_region.alloc((size_t)h->region_stride * B)); PL_TRY(h->d_far.alloc(npx * B));
     const int nw = 2 * kGradR * kGradR + 1;
-    LN_TRY(dev_alloc(&h->d_wtab, (size_t)nw));
+    PL_TRY(h->d_wtab.alloc((size_t)nw));
     k_lsd_wtab<<<(nw + 255) / 256, 256, 0, h->stream>>>(h->d_wtab, nw);
-    LN_CUDA(cudaGetLastError());
+    PL_CUDA(cudaGetLastError());
     count_launch();
   }
-  LN_TRY(dev_alloc(&h->d_counts, (size_t)kBins * P.nchunk * B)); LN_TRY(dev_alloc(&h->d_offsets, (size_t)kBins * P.nchunk * B));
-  LN_TRY(dev_alloc(&h->d_ndef, B)); LN_TRY(dev_alloc(&h->d_maxs, B)); LN_TRY(dev_alloc(&h->d_nseg, B)); LN_TRY(dev_alloc(&h->d_overflow, 1));
-  LN_TRY(dev_alloc(&h->d_order, npx * B)); LN_TRY(dev_alloc(&h->d_segs, (size_t)P.seg_cap * B));
-  LN_TRY(dev_alloc(&h->d_dxy, (size_t)P.w * P.h * B));
-  LN_CUDA(cudaMemset(h->d_overflow, 0, sizeof(int)));
-  LN_TRY(dev_alloc(&h->d_gtab, (size_t)kGradN * kGradN)); LN_TRY(dev_alloc(&h->d_gtab_seed, (size_t)kGradN * kGradN));
+  PL_TRY(h->d_counts.alloc((size_t)kBins * P.nchunk * B)); PL_TRY(h->d_offsets.alloc((size_t)kBins * P.nchunk * B));
+  PL_TRY(h->d_ndef.alloc(B)); PL_TRY(h->d_maxs.alloc(B)); PL_TRY(h->d_nseg.alloc(B)); PL_TRY(h->d_overflow.alloc(1));
+  PL_TRY(h->d_order.alloc(npx * B)); PL_TRY(h->d_segs.alloc((size_t)P.seg_cap * B));
+  PL_TRY(h->d_dxy.alloc((size_t)P.w * P.h * B));
+  PL_CUDA(cudaMemset(h->d_overflow, 0, sizeof(int)));
+  PL_TRY(h->d_gtab.alloc((size_t)kGradN * kGradN)); PL_TRY(h->d_gtab_seed.alloc((size_t)kGradN * kGradN));
   k_lsd_grad_table<<<(kGradN * kGradN + 255) / 256, 256, 0, h->stream>>>(h->d_gtab, h->d_gtab_seed);
-  LN_CUDA(cudaGetLastError());
-  LN_CUDA(cudaStreamSynchronize(h->stream));
+  PL_CUDA(cudaGetLastError());
+  PL_CUDA(cudaStreamSynchronize(h->stream));
   count_launch();
   {  // LBD weights (binary_descriptor_custom.cpp:217-259), integer divisions as in the reference
     float gG[63], gL[21];
@@ -825,11 +818,11 @@ extern "C" int pl_line_create(const PLLineConfig* cfg, PLLine** out) {
     for (int i = 0; i < 21; i++) { double d = i - u; gL[i] = (float)exp(d * d * inv); }
     u = (9 * 7 - 1) / 2; sigma = u; inv = -1 / (2 * sigma * sigma);
     for (int i = 0; i < 63; i++) { double d = i - u; gG[i] = (float)exp(d * d * inv); }
-    LN_CUDA(cudaMemcpyToSymbol(c_gaussG, gG, sizeof(gG)));
-    LN_CUDA(cudaMemcpyToSymbol(c_gaussL, gL, sizeof(gL)));
-    LN_CUDA(cudaMemcpyToSymbol(c_comb, h_comb, sizeof(h_comb)));
+    PL_CUDA(cudaMemcpyToSymbol(c_gaussG, gG, sizeof(gG)));
+    PL_CUDA(cudaMemcpyToSymbol(c_gaussL, gL, sizeof(gL)));
+    PL_CUDA(cudaMemcpyToSymbol(c_comb, h_comb, sizeof(h_comb)));
   }
-  LN_CUDA(cudaFuncSetAttribute(k_keylines, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->key_smem));
+  PL_CUDA(cudaFuncSetAttribute(k_keylines, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->key_smem));
   {  // seed order on chip: 8 CTAs share the frame's rows 0..sh-2 and its (sw-1)(sh-1) possible order positions
     const int nrow = (P.sh - 1) * P.sw, maxdef = (P.sw - 1) * (P.sh - 1);
     h->seed_q = (nrow + kSeedCta - 1) / kSeedCta;
@@ -841,14 +834,14 @@ extern "C" int pl_line_create(const PLLineConfig* cfg, PLLine** out) {
     cudaDeviceGetAttribute(&smem_max, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
     // 16-bit per-warp counters hold within-CTA offsets: at most 65535 pixels per CTA
     if (h->seed_q <= 65535 && h->seed_smem + 2 * 1024 <= (size_t)smem_max) {
-      LN_CUDA(cudaFuncSetAttribute(k_lsd_seed_order, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->seed_smem));
+      PL_CUDA(cudaFuncSetAttribute(k_lsd_seed_order, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->seed_smem));
       cudaLaunchConfig_t lc = {};
       lc.gridDim = dim3(kSeedCta, 1, 1); lc.blockDim = dim3(kSeedWarps * 32, 1, 1); lc.dynamicSmemBytes = h->seed_smem;
-      LN_CUDA(cudaOccupancyMaxActiveClusters(&h->seed_clusters, (void*)k_lsd_seed_order, &lc));
+      PL_CUDA(cudaOccupancyMaxActiveClusters(&h->seed_clusters, (void*)k_lsd_seed_order, &lc));
     }
   }
   // cfg->lsd_used_in_global is accepted for ABI compatibility and ignored: the USED state is the ownership word of the pixel record
-  *out = h;
+  *out = h.release();
   return PL_OK;
 }
 
@@ -867,12 +860,12 @@ extern "C" int pl_line_set_undistort(PLLine* h, const PLUndistort* und) {
 // Device timing of k_lsd_grow_ordered (the dominant kernel): enable, run, then read the duration of the LAST launch.
 extern "C" int pl_line_set_timing(PLLine* h, int on) {
   PL_ARG(h);
-  if (on && !h->ev0) { PL_CUDA(cudaEventCreate(&h->ev0)); PL_CUDA(cudaEventCreate(&h->ev1)); }
+  if (on) for (Event* e : {&h->ev0, &h->ev1}) if (!*e) PL_TRY(e->create(cudaEventDefault));
   h->timing = on;
   return PL_OK;
 }
 extern "C" int pl_line_grow_ms(PLLine* h, float* ms) {
-  PL_ARG(h && ms && h->ev0);
+  PL_ARG(h && ms && h->ev1);
   PL_CUDA(cudaEventSynchronize(h->ev1));
   PL_CUDA(cudaEventElapsedTime(ms, h->ev0, h->ev1));
   return PL_OK;
@@ -914,7 +907,7 @@ extern "C" int pl_line_extract_batch_dev(PLLine* h, const uint8_t* imgs, int str
     const uint8_t* src = imgs; int sstride = stride; long long sframe = (long long)frame_stride;
     if (h->und && !serial) {
       const size_t fb = (size_t)P.w * P.h;
-      if (!h->d_und && (rc = dev_alloc(&h->d_und, fb * h->cfg.max_batch))) return rc;
+      if (!h->d_und && (rc = h->d_und.alloc(fb * h->cfg.max_batch))) return rc;
       // the remap only reads the map: the handle stays the caller's
       if ((rc = pl_undistort_remap_batch_dev(const_cast<PLUndistort*>(h->und), imgs, stride, frame_stride, B, h->d_und, P.w, fb, st))) return rc;
       src = h->d_und; sstride = P.w; sframe = (long long)fb;
@@ -922,9 +915,9 @@ extern "C" int pl_line_extract_batch_dev(PLLine* h, const uint8_t* imgs, int str
     const bool map = h->und && serial;
     const dim3 grd(std::max((P.sw + kFrontSX - 1) / kFrontSX, (P.w + kFrontUX - 1) / kFrontUX),
                    std::max((P.sh + kFrontSY - 1) / kFrontSY, (P.h + kFrontUY - 1) / kFrontUY), (B + kFrontFrames - 1) / kFrontFrames);
-    const float4* T = reinterpret_cast<const float4*>(h->d_gtab);
-    const RemapEntry* mp = map ? h->und->d_map : nullptr;
-    const int4* tab = map ? h->und->d_tab : nullptr;
+    const float4* T = reinterpret_cast<const float4*>(h->d_gtab.get());
+    const RemapEntry* mp = map ? h->und->d_map.get() : nullptr;
+    const int4* tab = map ? h->und->d_tab.get() : nullptr;
     cudaLaunchConfig_t lc = {};
     lc.gridDim = grd; lc.blockDim = dim3(kFrontThreads); lc.dynamicSmemBytes = map ? kFrontMapSmem : 0; lc.stream = st;
     cudaLaunchAttribute at[1];
@@ -983,35 +976,28 @@ extern "C" int pl_line_check_overflow(PLLine* h) {
   return PL_OK;
 }
 
-static int line_staging(PLLine* h) {
-  if (h->d_img) return PL_OK;
-  const size_t B = h->cfg.max_batch;
-  int rc;
-  if ((rc = dev_alloc(&h->d_img, (size_t)h->P.w * h->P.h * B))) return rc;
-  if ((rc = dev_alloc(&h->d_kls, (size_t)h->P.capL * B))) return rc;
-  if ((rc = dev_alloc(&h->d_desc, (size_t)h->P.capL * 32 * B))) return rc;
-  if ((rc = dev_alloc(&h->d_lf, (size_t)h->P.capL * 3 * B))) return rc;
-  if ((rc = dev_alloc(&h->d_nl, B))) return rc;
-  if ((rc = dev_alloc(&h->d_mask, (size_t)h->P.w * h->P.h))) return rc;
-  return PL_OK;
-}
-
 extern "C" int pl_line_extract_batch(PLLine* h, const uint8_t* imgs, int stride, size_t frame_stride, int B,
                                      const uint8_t* mask, void* keylines, uint8_t* desc, double* linefunc, int* n) {
   PL_ARG(h && imgs && keylines && desc && linefunc && n && B >= 1 && B <= h->cfg.max_batch && stride >= h->cfg.width);
-  int rc = line_staging(h);
-  if (rc) return rc;
+  if (!h->io) {
+    const size_t Bm = h->cfg.max_batch, npx = (size_t)h->P.w * h->P.h, cap = h->P.capL;
+    auto io = std::make_unique<PLLine::HostStaging>();
+    PL_TRY(io->d_img.alloc(npx * Bm)); PL_TRY(io->d_kls.alloc(cap * Bm)); PL_TRY(io->d_desc.alloc(cap * 32 * Bm));
+    PL_TRY(io->d_lf.alloc(cap * 3 * Bm)); PL_TRY(io->d_nl.alloc(Bm)); PL_TRY(io->d_mask.alloc(npx));
+    h->io = std::move(io);
+  }
+  const PLLine::HostStaging& io = *h->io;
   const int W = h->P.w, H = h->P.h;
   for (int b = 0; b < B; b++)
-    PL_CUDA(cudaMemcpy2DAsync(h->d_img + (size_t)b * W * H, W, imgs + (size_t)b * frame_stride, stride, W, H, cudaMemcpyHostToDevice, h->stream));
-  if (mask) PL_CUDA(cudaMemcpyAsync(h->d_mask, mask, (size_t)W * H, cudaMemcpyHostToDevice, h->stream));
-  rc = pl_line_extract_batch_dev(h, h->d_img, W, (size_t)W * H, B, mask ? h->d_mask : nullptr, h->d_kls, h->d_desc, h->d_lf, h->d_nl, h->stream);
+    PL_CUDA(cudaMemcpy2DAsync(io.d_img + (size_t)b * W * H, W, imgs + (size_t)b * frame_stride, stride, W, H, cudaMemcpyHostToDevice, h->stream));
+  if (mask) PL_CUDA(cudaMemcpyAsync(io.d_mask, mask, (size_t)W * H, cudaMemcpyHostToDevice, h->stream));
+  int rc = pl_line_extract_batch_dev(h, io.d_img, W, (size_t)W * H, B, mask ? io.d_mask.get() : nullptr, io.d_kls, io.d_desc, io.d_lf, io.d_nl, h->stream);
   if (rc) return rc;
   const size_t cap = h->P.capL;
-  PL_CUDA(cudaMemcpyAsync(keylines, h->d_kls, cap * B * sizeof(PLKeyLineRec), cudaMemcpyDeviceToHost, h->stream));
-  PL_CUDA(cudaMemcpyAsync(desc, h->d_desc, cap * B * 32, cudaMemcpyDeviceToHost, h->stream));
-  PL_CUDA(cudaMemcpyAsync(linefunc, h->d_lf, cap * B * 3 * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
-  PL_CUDA(cudaMemcpyAsync(n, h->d_nl, (size_t)B * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  PL_CUDA(cudaMemcpyAsync(keylines, io.d_kls, cap * B * sizeof(PLKeyLineRec), cudaMemcpyDeviceToHost, h->stream));
+  PL_CUDA(cudaMemcpyAsync(desc, io.d_desc, cap * B * 32, cudaMemcpyDeviceToHost, h->stream));
+  PL_CUDA(cudaMemcpyAsync(linefunc, io.d_lf, cap * B * 3 * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  PL_CUDA(cudaMemcpyAsync(n, io.d_nl, (size_t)B * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
   PL_CUDA(cudaStreamSynchronize(h->stream));
   return pl_line_check_overflow(h);
 }

@@ -737,21 +737,17 @@ struct PLOrb {
   std::vector<float> scale, invScale, sigma2, invSigma2;
   std::vector<int> perLevel;
   std::vector<CellInfo> cells;
-  cudaStream_t stream = nullptr;
+  Stream stream;
   // device
-  CellInfo* d_cells = nullptr;
-  short4* d_tabs = nullptr;
-  uint8_t* d_pyr = nullptr;
-  uint8_t* d_blur = nullptr;   // blurred levels 0.. (K4a output)
-  uint32_t *d_slots = nullptr, *d_keysA = nullptr, *d_keysB = nullptr, *d_sel = nullptr;
-  int *d_counts = nullptr, *d_nsel = nullptr, *d_overflow = nullptr;
-  // staging for the host-pointer API
-  uint8_t* d_img = nullptr;
-  PLKeyPoint* d_kps = nullptr;
-  uint8_t* d_desc = nullptr;
-  int* d_n = nullptr;
-  uint8_t* h_pin = nullptr;  // pinned staging (images in, results out)
-  size_t pin_bytes = 0;
+  DevBuf<CellInfo> d_cells;
+  DevBuf<short4> d_tabs;
+  DevBuf<uint8_t> d_pyr;
+  DevBuf<uint8_t> d_blur;   // blurred levels 0.. (K4a output)
+  DevBuf<uint32_t> d_slots, d_keysA, d_keysB, d_sel;
+  DevBuf<int> d_counts, d_nsel, d_overflow;
+  // staging for the host-pointer API (made on first use)
+  struct HostStaging { DevBuf<uint8_t> d_img; DevBuf<PLKeyPoint> d_kps; DevBuf<uint8_t> d_desc; DevBuf<int> d_n; };
+  std::unique_ptr<HostStaging> io;
   // last call (for pl_orb_get_level / debug taps)
   const uint8_t* last_img = nullptr;
   int last_stride = 0;
@@ -787,7 +783,7 @@ extern "C" int pl_orb_create(const PLOrbConfig* cfg, PLOrb** out) {
   PL_ARG(cfg->scale_factor > 1.0f && cfg->min_th_fast >= 1 && cfg->ini_th_fast >= cfg->min_th_fast);
   int rc = require_device();
   if (rc) return rc;
-  PLOrb* h = new PLOrb;
+  std::unique_ptr<PLOrb> h(new PLOrb);
   h->cfg = *cfg;
   const int nl = cfg->nlevels;
   // scale tables, quotas: ORBextractor ctor (ORBextractor.cc:410-446); scaleFactor is held in a double member
@@ -822,7 +818,7 @@ extern "C" int pl_orb_create(const PLOrbConfig* cfg, PLOrb** out) {
     LevelInfo& L = P.lv[l];
     L.w = cvRoundf_h((float)cfg->width * h->invScale[l]);
     L.h = cvRoundf_h((float)cfg->height * h->invScale[l]);
-    if (L.w < 2 * kEdge + 8 || L.h < 2 * kEdge + 8) { delete h; set_error("level %d too small", l); return PL_ERR_ARG; }
+    if (L.w < 2 * kEdge + 8 || L.h < 2 * kEdge + 8) { set_error("level %d too small", l); return PL_ERR_ARG; }
     L.pitch = (L.w + 63) / 64 * 64;
     L.off = off;
     L.bpitch = L.pitch; L.boff = boff;
@@ -840,9 +836,9 @@ extern "C" int pl_orb_create(const PLOrbConfig* cfg, PLOrb** out) {
     const int minBX = kEdge - 3, minBY = minBX, maxBX = L.w - kEdge + 3, maxBY = L.h - kEdge + 3;
     const float width = (float)(maxBX - minBX), height = (float)(maxBY - minBY);
     const int nCols = (int)(width / 30.f), nRows = (int)(height / 30.f);
-    if (nCols < 1 || nRows < 1) { delete h; set_error("level %d has no FAST cells", l); return PL_ERR_ARG; }
+    if (nCols < 1 || nRows < 1) { set_error("level %d has no FAST cells", l); return PL_ERR_ARG; }
     const int wCell = (int)ceilf(width / nCols), hCell = (int)ceilf(height / nRows);
-    if (wCell + 6 > kMaxWin || hCell + 6 > kMaxWin) { delete h; set_error("FAST cell larger than %d", kMaxWin); return PL_ERR_ARG; }
+    if (wCell + 6 > kMaxWin || hCell + 6 > kMaxWin) { set_error("FAST cell larger than %d", kMaxWin); return PL_ERR_ARG; }
     L.cell0 = (int)h->cells.size();
     for (int i = 0; i < nRows; i++) {
       const float iniY = (float)(minBY + i * hCell);
@@ -863,7 +859,7 @@ extern "C" int pl_orb_create(const PLOrbConfig* cfg, PLOrb** out) {
     L.ncells = (int)h->cells.size() - L.cell0;
     L.regW = maxBX - minBX; L.regH = maxBY - minBY;
     L.nIni = (int)roundf((float)L.regW / (float)L.regH);
-    if (L.nIni < 1) { delete h; set_error("aspect ratio gives 0 quadtree roots (reference divides by zero)"); return PL_ERR_ARG; }
+    if (L.nIni < 1) { set_error("aspect ratio gives 0 quadtree roots (reference divides by zero)"); return PL_ERR_ARG; }
     L.hX = (float)L.regW / L.nIni;
     L.keyoff = keyoff; L.keycap = L.ncells * P.slotcap;
     keyoff += L.keycap;
@@ -892,45 +888,37 @@ extern "C" int pl_orb_create(const PLOrbConfig* cfg, PLOrb** out) {
       while (fit > 0 && quad_smem_for(fit) > (size_t)smem_max) fit--;
       set_error("a per-level quota of %d features needs %zu B of quadtree shared memory, over the device's %d B; at most %d "
                 "features fit on one level (mnFeaturesPerLevel)", maxN, h->quad_smem, smem_max, fit);
-      delete h;
       return PL_ERR_ARG;
     }
   }
   const int B = cfg->max_batch;
-#define ORB_TRY(e) do { int _r = (e); if (_r) { pl_orb_destroy(h); return _r; } } while (0)
-#define ORB_CUDA(e) do { cudaError_t _e = (e); if (_e != cudaSuccess) { set_error("%s -> %s", #e, cudaGetErrorString(_e)); pl_orb_destroy(h); return PL_ERR_CUDA; } } while (0)
-  ORB_CUDA(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
+  PL_TRY(h->stream.create(cudaStreamNonBlocking));
   static_assert(sizeof(h_pattern) == sizeof(char4) * 256, "pattern size");
-  ORB_CUDA(cudaMemcpyToSymbol(g_pattern, h_pattern, sizeof(h_pattern)));
-  ORB_CUDA(cudaMemcpyToSymbol(c_umax, umax, sizeof(umax)));
-  ORB_TRY(dev_alloc(&h->d_cells, h->cells.size()));
-  ORB_CUDA(cudaMemcpy(h->d_cells, h->cells.data(), h->cells.size() * sizeof(CellInfo), cudaMemcpyHostToDevice));
-  ORB_TRY(dev_alloc(&h->d_tabs, std::max<size_t>(tabs.size(), 1)));
-  if (!tabs.empty()) ORB_CUDA(cudaMemcpy(h->d_tabs, tabs.data(), tabs.size() * sizeof(short4), cudaMemcpyHostToDevice));
-  ORB_TRY(dev_alloc(&h->d_pyr, (size_t)std::max<long long>(off, 256) * B));
+  PL_CUDA(cudaMemcpyToSymbol(g_pattern, h_pattern, sizeof(h_pattern)));
+  PL_CUDA(cudaMemcpyToSymbol(c_umax, umax, sizeof(umax)));
+  PL_TRY(h->d_cells.alloc(h->cells.size()));
+  PL_CUDA(cudaMemcpy(h->d_cells, h->cells.data(), h->cells.size() * sizeof(CellInfo), cudaMemcpyHostToDevice));
+  PL_TRY(h->d_tabs.alloc(std::max<size_t>(tabs.size(), 1)));
+  if (!tabs.empty()) PL_CUDA(cudaMemcpy(h->d_tabs, tabs.data(), tabs.size() * sizeof(short4), cudaMemcpyHostToDevice));
+  PL_TRY(h->d_pyr.alloc((size_t)std::max<long long>(off, 256) * B));
   // FAST windows of the pyramid levels are staged by TMA bulk copies (pitch and level offsets are multiples of 64 / 256)
   h->fast_bulk = getenv("PLSLAM_NO_TMA") ? 0u : (((1u << nl) - 1u) & ~1u);
-  ORB_TRY(dev_alloc(&h->d_blur, (size_t)boff * B));
-  ORB_TRY(dev_alloc(&h->d_slots, (size_t)P.ncells * P.slotcap * B));
-  ORB_TRY(dev_alloc(&h->d_counts, (size_t)P.ncells * B));
-  ORB_TRY(dev_alloc(&h->d_keysA, (size_t)P.key_frame * B));
-  ORB_TRY(dev_alloc(&h->d_keysB, (size_t)P.key_frame * B));
-  ORB_TRY(dev_alloc(&h->d_sel, (size_t)P.selcap * nl * B));
-  ORB_TRY(dev_alloc(&h->d_nsel, (size_t)nl * B));
-  ORB_TRY(dev_alloc(&h->d_overflow, 1));
-  ORB_CUDA(cudaMemset(h->d_overflow, 0, sizeof(int)));
-  ORB_CUDA(cudaFuncSetAttribute(k_quadtree, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->quad_smem));
-  *out = h;
+  PL_TRY(h->d_blur.alloc((size_t)boff * B));
+  PL_TRY(h->d_slots.alloc((size_t)P.ncells * P.slotcap * B));
+  PL_TRY(h->d_counts.alloc((size_t)P.ncells * B));
+  PL_TRY(h->d_keysA.alloc((size_t)P.key_frame * B));
+  PL_TRY(h->d_keysB.alloc((size_t)P.key_frame * B));
+  PL_TRY(h->d_sel.alloc((size_t)P.selcap * nl * B));
+  PL_TRY(h->d_nsel.alloc((size_t)nl * B));
+  PL_TRY(h->d_overflow.alloc(1));
+  PL_CUDA(cudaMemset(h->d_overflow, 0, sizeof(int)));
+  PL_CUDA(cudaFuncSetAttribute(k_quadtree, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->quad_smem));
+  *out = h.release();
   return PL_OK;
 }
 
 extern "C" void pl_orb_destroy(PLOrb* h) {
   if (!h) return;
-  cudaFree(h->d_cells); cudaFree(h->d_tabs); cudaFree(h->d_pyr); cudaFree(h->d_blur); cudaFree(h->d_slots); cudaFree(h->d_counts);
-  cudaFree(h->d_keysA); cudaFree(h->d_keysB); cudaFree(h->d_sel); cudaFree(h->d_nsel); cudaFree(h->d_overflow);
-  cudaFree(h->d_img); cudaFree(h->d_kps); cudaFree(h->d_desc); cudaFree(h->d_n);
-  if (h->h_pin) cudaFreeHost(h->h_pin);
-  if (h->stream) cudaStreamDestroy(h->stream);
   delete h;
 }
 
@@ -1004,34 +992,28 @@ extern "C" int pl_orb_check_overflow(PLOrb* h) {
   return PL_OK;
 }
 
-static int orb_ensure_staging(PLOrb* h) {
-  if (h->d_img) return PL_OK;
-  const int B = h->cfg.max_batch;
-  const size_t img_bytes = (size_t)h->cfg.width * h->cfg.height;
-  int rc;
-  if ((rc = dev_alloc(&h->d_img, img_bytes * B))) return rc;
-  if ((rc = dev_alloc(&h->d_kps, (size_t)h->P.cap * B))) return rc;
-  if ((rc = dev_alloc(&h->d_desc, (size_t)h->P.cap * 32 * B))) return rc;
-  if ((rc = dev_alloc(&h->d_n, (size_t)B))) return rc;
-  return PL_OK;
-}
-
 extern "C" int pl_orb_extract_batch(PLOrb* h, const uint8_t* imgs, int stride, size_t frame_stride, int B,
                                     PLKeyPoint* kps, uint8_t* desc, int* n) {
   PL_ARG(h && imgs && kps && desc && n);
   PL_ARG(B >= 1 && B <= h->cfg.max_batch && stride >= h->cfg.width);
-  int rc = orb_ensure_staging(h);
-  if (rc) return rc;
+  if (!h->io) {
+    const size_t Bm = h->cfg.max_batch, cap = h->P.cap;
+    auto io = std::make_unique<PLOrb::HostStaging>();
+    PL_TRY(io->d_img.alloc((size_t)h->cfg.width * h->cfg.height * Bm));
+    PL_TRY(io->d_kps.alloc(cap * Bm)); PL_TRY(io->d_desc.alloc(cap * 32 * Bm)); PL_TRY(io->d_n.alloc(Bm));
+    h->io = std::move(io);
+  }
+  const PLOrb::HostStaging& io = *h->io;
   const int W = h->cfg.width, H = h->cfg.height;
   for (int b = 0; b < B; b++)
-    PL_CUDA(cudaMemcpy2DAsync(h->d_img + (size_t)b * W * H, W, imgs + (size_t)b * frame_stride, stride, W, H,
+    PL_CUDA(cudaMemcpy2DAsync(io.d_img + (size_t)b * W * H, W, imgs + (size_t)b * frame_stride, stride, W, H,
                               cudaMemcpyHostToDevice, h->stream));
-  rc = pl_orb_extract_batch_dev(h, h->d_img, W, (size_t)W * H, B, h->d_kps, h->d_desc, h->d_n, h->stream);
+  int rc = pl_orb_extract_batch_dev(h, io.d_img, W, (size_t)W * H, B, io.d_kps, io.d_desc, io.d_n, h->stream);
   if (rc) return rc;
   const size_t cap = (size_t)h->P.cap;
-  PL_CUDA(cudaMemcpyAsync(kps, h->d_kps, cap * B * sizeof(PLKeyPoint), cudaMemcpyDeviceToHost, h->stream));
-  PL_CUDA(cudaMemcpyAsync(desc, h->d_desc, cap * B * 32, cudaMemcpyDeviceToHost, h->stream));
-  PL_CUDA(cudaMemcpyAsync(n, h->d_n, (size_t)B * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  PL_CUDA(cudaMemcpyAsync(kps, io.d_kps, cap * B * sizeof(PLKeyPoint), cudaMemcpyDeviceToHost, h->stream));
+  PL_CUDA(cudaMemcpyAsync(desc, io.d_desc, cap * B * 32, cudaMemcpyDeviceToHost, h->stream));
+  PL_CUDA(cudaMemcpyAsync(n, io.d_n, (size_t)B * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
   PL_CUDA(cudaStreamSynchronize(h->stream));
   return pl_orb_check_overflow(h);
 }

@@ -22,8 +22,9 @@ struct CamD { double fx, fy, cx, cy, k1, k2, p1, p2, k3; };
 // pl_undistort_create: the map of one camera and frame size, on the device
 struct PLUndistort {
   int w, h; pl::CamD cam; float K[4], D[5];
-  pl::RemapEntry* d_map = nullptr;
-  int4* d_tab = nullptr;
-  uint8_t *d_src = nullptr, *d_dst = nullptr; int staged = 0;
-  cudaStream_t stream = nullptr;
+  pl::DevBuf<pl::RemapEntry> d_map;
+  pl::DevBuf<int4> d_tab;
+  struct HostStaging { pl::DevBuf<uint8_t> d_src, d_dst; };   // pl_undistort_remap (made on first use)
+  std::unique_ptr<HostStaging> io;
+  pl::Stream stream;
 };

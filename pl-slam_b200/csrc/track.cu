@@ -17,19 +17,21 @@
 
 struct PLMap {
   int n_points = 0, n_lines = 0;
-  float *pt_pos = nullptr, *pt_normal = nullptr, *pt_min = nullptr, *pt_max = nullptr;
-  uint8_t* pt_desc = nullptr;
-  double *ln_pos = nullptr, *ln_normal = nullptr;
-  float *ln_min = nullptr, *ln_max = nullptr;
-  uint8_t* ln_desc = nullptr;
-  int* flag = nullptr;            // sticky: [0] an index outside the map was met, [1] a local list outgrew its capacity
-  cudaStream_t stream = nullptr;
-  // the keyframe graph (pl_map_set_keyframes); CSR rows per keyframe, obs per map point
-  int n_kf = 0;
-  float *kf_Tcw = nullptr, *kf_Twc = nullptr;
-  uint8_t* kf_bad = nullptr;
-  int *kf_parent = nullptr, *kf_pt_off = nullptr, *kf_pt = nullptr, *kf_ln_off = nullptr, *kf_ln = nullptr;
-  int *kf_cov_off = nullptr, *kf_cov = nullptr, *kf_child_off = nullptr, *kf_child = nullptr, *obs_off = nullptr, *obs = nullptr;
+  pl::DevBuf<float> pt_pos, pt_normal, pt_min, pt_max;
+  pl::DevBuf<uint8_t> pt_desc;
+  pl::DevBuf<double> ln_pos, ln_normal;
+  pl::DevBuf<float> ln_min, ln_max;
+  pl::DevBuf<uint8_t> ln_desc;
+  pl::DevBuf<int> flag;           // sticky: [0] an index outside the map was met, [1] a local list outgrew its capacity
+  pl::Stream stream;
+  // the keyframe graph (pl_map_set_keyframes; NULL before the first); CSR rows per keyframe, obs per map point
+  struct KeyframeGraph {
+    int n_kf = 0;
+    pl::DevBuf<float> Tcw, Twc;
+    pl::DevBuf<uint8_t> bad;
+    pl::DevBuf<int> parent, pt_off, pt, ln_off, ln, cov_off, cov, child_off, child, obs_off, obs;
+  };
+  std::unique_ptr<KeyframeGraph> kf;
 };
 
 namespace pl {
@@ -292,23 +294,14 @@ static int track_local_map_run(PLMap* map, const PLTrackFrames* F, const int* po
 }  // namespace pl
 using namespace pl;
 
-static void free_keyframes(PLMap* m) {
-  for (void* p : {(void*)m->kf_Tcw, (void*)m->kf_Twc, (void*)m->kf_bad, (void*)m->kf_parent, (void*)m->kf_pt_off, (void*)m->kf_pt,
-                  (void*)m->kf_ln_off, (void*)m->kf_ln, (void*)m->kf_cov_off, (void*)m->kf_cov, (void*)m->kf_child_off,
-                  (void*)m->kf_child, (void*)m->obs_off, (void*)m->obs})
-    cudaFree(p);
-  m->kf_Tcw = m->kf_Twc = nullptr; m->kf_bad = nullptr;
-  m->kf_parent = m->kf_pt_off = m->kf_pt = m->kf_ln_off = m->kf_ln = m->kf_cov_off = m->kf_cov = nullptr;
-  m->kf_child_off = m->kf_child = m->obs_off = m->obs = nullptr;
-  m->n_kf = 0;
+// n elements of src in a new buffer of max(n, room) elements
+template <typename T> static int upload(DevBuf<T>& d, const void* src, size_t n, size_t room) {
+  PL_TRY(d.alloc(std::max(n, room)));
+  if (n) PL_CUDA(cudaMemcpy(d, src, n * sizeof(T), cudaMemcpyHostToDevice));
+  return PL_OK;
 }
 extern "C" void pl_map_destroy(PLMap* m) {
   if (!m) return;
-  free_keyframes(m);
-  for (void* p : {(void*)m->pt_pos, (void*)m->pt_normal, (void*)m->pt_min, (void*)m->pt_max, (void*)m->pt_desc, (void*)m->ln_pos,
-                  (void*)m->ln_normal, (void*)m->ln_min, (void*)m->ln_max, (void*)m->ln_desc, (void*)m->flag})
-    cudaFree(p);
-  if (m->stream) cudaStreamDestroy(m->stream);
   delete m;
 }
 extern "C" int pl_map_create(const PLMapDesc* d, PLMap** out) {
@@ -316,24 +309,18 @@ extern "C" int pl_map_create(const PLMapDesc* d, PLMap** out) {
   PL_ARG(d->n_points == 0 || (d->pt_pos && d->pt_normal && d->pt_min_dist && d->pt_max_dist && d->pt_desc));
   PL_ARG(d->n_lines == 0 || (d->ln_pos && d->ln_normal && d->ln_min_dist && d->ln_max_dist && d->ln_desc));
   int rc = require_device(); if (rc) return rc;
-  PLMap* m = new PLMap;
+  std::unique_ptr<PLMap> m(new PLMap);
   m->n_points = d->n_points; m->n_lines = d->n_lines;
-  const size_t np = std::max(d->n_points, 1), nl = std::max(d->n_lines, 1);
-  cudaError_t e = cudaSuccess;
-  auto up = [&](auto** dst, const void* src, size_t n_alloc, size_t bytes) {
-    if (e == cudaSuccess) e = cudaMalloc((void**)dst, n_alloc);
-    if (e == cudaSuccess && bytes) e = cudaMemcpy(*dst, src, bytes, cudaMemcpyHostToDevice);
-  };
+  // a map without points or lines still gets one entry of each array
   const size_t P = d->n_points, L = d->n_lines;
-  up(&m->pt_pos, d->pt_pos, np * 12, P * 12); up(&m->pt_normal, d->pt_normal, np * 12, P * 12);
-  up(&m->pt_min, d->pt_min_dist, np * 4, P * 4); up(&m->pt_max, d->pt_max_dist, np * 4, P * 4); up(&m->pt_desc, d->pt_desc, np * 32, P * 32);
-  up(&m->ln_pos, d->ln_pos, nl * 48, L * 48); up(&m->ln_normal, d->ln_normal, nl * 24, L * 24);
-  up(&m->ln_min, d->ln_min_dist, nl * 4, L * 4); up(&m->ln_max, d->ln_max_dist, nl * 4, L * 4); up(&m->ln_desc, d->ln_desc, nl * 32, L * 32);
-  up(&m->flag, nullptr, 8, 0);
-  if (e == cudaSuccess) e = cudaMemset(m->flag, 0, 8);
-  if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking);
-  if (e != cudaSuccess) { set_error("pl_map_create: %s", cudaGetErrorString(e)); pl_map_destroy(m); return PL_ERR_CUDA; }
-  *out = m;
+  PL_TRY(upload(m->pt_pos, d->pt_pos, P * 3, 3)); PL_TRY(upload(m->pt_normal, d->pt_normal, P * 3, 3));
+  PL_TRY(upload(m->pt_min, d->pt_min_dist, P, 1)); PL_TRY(upload(m->pt_max, d->pt_max_dist, P, 1)); PL_TRY(upload(m->pt_desc, d->pt_desc, P * 32, 32));
+  PL_TRY(upload(m->ln_pos, d->ln_pos, L * 6, 6)); PL_TRY(upload(m->ln_normal, d->ln_normal, L * 3, 3));
+  PL_TRY(upload(m->ln_min, d->ln_min_dist, L, 1)); PL_TRY(upload(m->ln_max, d->ln_max_dist, L, 1)); PL_TRY(upload(m->ln_desc, d->ln_desc, L * 32, 32));
+  PL_TRY(m->flag.alloc(2));
+  PL_CUDA(cudaMemset(m->flag, 0, 8));
+  PL_TRY(m->stream.create(cudaStreamNonBlocking));
+  *out = m.release();
   return PL_OK;
 }
 extern "C" int pl_map_check_indices(PLMap* m) {
@@ -1059,21 +1046,18 @@ extern "C" int pl_map_set_keyframes(PLMap* m, const PLKeyFrameGraphDesc* g) {
   for (int k = 0; k < K; k++) std::sort(child.begin() + g->child_offset[k], child.begin() + g->child_offset[k + 1]);
   std::vector<uint8_t> bad(K, 0);
   if (g->bad) for (int k = 0; k < K; k++) bad[k] = g->bad[k] != 0;
-  free_keyframes(m);
-  cudaError_t e = cudaSuccess;
-  auto up = [&](auto** dst, const void* src, size_t bytes) {
-    if (e == cudaSuccess) e = cudaMalloc((void**)dst, std::max<size_t>(bytes, 16));
-    if (e == cudaSuccess && bytes) e = cudaMemcpy(*dst, src, bytes, cudaMemcpyHostToDevice);
-  };
+  // the new graph replaces the old one only once all of it is on the device; every array takes at least 16 bytes
+  auto G = std::make_unique<PLMap::KeyframeGraph>();
   const size_t k = K, np = m->n_points;
-  up(&m->kf_Tcw, g->Tcw, k * 64); up(&m->kf_Twc, g->Twc, k * 64); up(&m->kf_bad, bad.data(), k); up(&m->kf_parent, g->parent, k * 4);
-  up(&m->kf_pt_off, g->pt_slot_offset, (k + 1) * 4); up(&m->kf_pt, g->pt_slot, (size_t)g->pt_slot_offset[K] * 4);
-  up(&m->kf_ln_off, g->ln_slot_offset, (k + 1) * 4); up(&m->kf_ln, g->ln_slot, (size_t)g->ln_slot_offset[K] * 4);
-  up(&m->kf_cov_off, g->cov_offset, (k + 1) * 4); up(&m->kf_cov, g->cov, (size_t)g->cov_offset[K] * 4);
-  up(&m->kf_child_off, g->child_offset, (k + 1) * 4); up(&m->kf_child, child.data(), child.size() * 4);
-  up(&m->obs_off, g->obs_offset, (np + 1) * 4); up(&m->obs, g->obs, (size_t)g->obs_offset[np] * 4);
-  if (e != cudaSuccess) { set_error("pl_map_set_keyframes: %s", cudaGetErrorString(e)); free_keyframes(m); return PL_ERR_CUDA; }
-  m->n_kf = K;
+  PL_TRY(upload(G->Tcw, g->Tcw, k * 16, 4)); PL_TRY(upload(G->Twc, g->Twc, k * 16, 4));
+  PL_TRY(upload(G->bad, bad.data(), k, 16)); PL_TRY(upload(G->parent, g->parent, k, 4));
+  PL_TRY(upload(G->pt_off, g->pt_slot_offset, k + 1, 4)); PL_TRY(upload(G->pt, g->pt_slot, (size_t)g->pt_slot_offset[K], 4));
+  PL_TRY(upload(G->ln_off, g->ln_slot_offset, k + 1, 4)); PL_TRY(upload(G->ln, g->ln_slot, (size_t)g->ln_slot_offset[K], 4));
+  PL_TRY(upload(G->cov_off, g->cov_offset, k + 1, 4)); PL_TRY(upload(G->cov, g->cov, (size_t)g->cov_offset[K], 4));
+  PL_TRY(upload(G->child_off, g->child_offset, k + 1, 4)); PL_TRY(upload(G->child, child.data(), child.size(), 4));
+  PL_TRY(upload(G->obs_off, g->obs_offset, np + 1, 4)); PL_TRY(upload(G->obs, g->obs, (size_t)g->obs_offset[np], 4));
+  G->n_kf = K;
+  m->kf = std::move(G);
   return PL_OK;
 }
 
@@ -1091,15 +1075,16 @@ extern "C" int pl_map_check_capacity(PLMap* m) {
 extern "C" int pl_track_update_local_map_dev(PLMap* map, int B, const int* point_map, int cap_points, const int* ok, const int* vo,
                                              const PLLocalMap* L, void* stream) {
   PL_ARG(map && L && point_map && B >= 1 && cap_points >= 1);
-  if (map->n_kf < 1) { set_error("pl_track_update_local_map_dev: the map has no keyframe graph (pl_map_set_keyframes)"); return PL_ERR_ARG; }
+  if (!map->kf) { set_error("pl_track_update_local_map_dev: the map has no keyframe graph (pl_map_set_keyframes)"); return PL_ERR_ARG; }
   PL_ARG(L->kf && L->n_kf && L->ref_kf && L->pt_index && L->pt_count && L->ln_index && L->ln_count);
   PL_ARG(L->cap_kf >= 1 && L->cap_local_points >= 1 && L->cap_local_lines >= 1);
   ULMArgs A;
-  A.n_kf = map->n_kf; A.n_points = map->n_points; A.n_lines = map->n_lines;
+  const PLMap::KeyframeGraph& G = *map->kf;
+  A.n_kf = G.n_kf; A.n_points = map->n_points; A.n_lines = map->n_lines;
   A.bit_words = (std::max(std::max(map->n_points, map->n_lines), 1) + 31) / 32;
-  A.bad = map->kf_bad; A.parent = map->kf_parent; A.pt_off = map->kf_pt_off; A.pt = map->kf_pt; A.ln_off = map->kf_ln_off; A.ln = map->kf_ln;
-  A.cov_off = map->kf_cov_off; A.cov = map->kf_cov; A.child_off = map->kf_child_off; A.child = map->kf_child;
-  A.obs_off = map->obs_off; A.obs = map->obs;
+  A.bad = G.bad; A.parent = G.parent; A.pt_off = G.pt_off; A.pt = G.pt; A.ln_off = G.ln_off; A.ln = G.ln;
+  A.cov_off = G.cov_off; A.cov = G.cov; A.child_off = G.child_off; A.child = G.child;
+  A.obs_off = G.obs_off; A.obs = G.obs;
   A.point_map = point_map; A.cap = cap_points; A.ok = ok; A.vo = vo;
   A.kf = L->kf; A.n_kf_out = L->n_kf; A.cap_kf = L->cap_kf; A.ref_kf = L->ref_kf;
   A.lp = L->pt_index; A.n_lp = L->pt_count; A.cap_lp = L->cap_local_points; A.ll = L->ln_index; A.n_ll = L->ln_count;
@@ -1140,16 +1125,16 @@ extern "C" int pl_track_local_map_lists_dev(PLMap* map, const PLTrackFrames* F, 
 
 extern "C" int pl_track_relative_pose_dev(PLMap* map, int B, const float* Tcw, const int* ref_kf, float* Tcr, void* stream) {
   PL_ARG(map && B >= 1 && Tcw && ref_kf && Tcr);
-  if (map->n_kf < 1) { set_error("pl_track_relative_pose_dev: the map has no keyframe graph (pl_map_set_keyframes)"); return PL_ERR_ARG; }
-  k_ref_pose<<<(B + 127) / 128, 128, 0, stream ? (cudaStream_t)stream : map->stream>>>(B, Tcw, ref_kf, map->kf_Twc, map->n_kf, Tcr, map->flag);
+  if (!map->kf) { set_error("pl_track_relative_pose_dev: the map has no keyframe graph (pl_map_set_keyframes)"); return PL_ERR_ARG; }
+  k_ref_pose<<<(B + 127) / 128, 128, 0, stream ? (cudaStream_t)stream : map->stream>>>(B, Tcw, ref_kf, map->kf->Twc, map->kf->n_kf, Tcr, map->flag);
   PL_LAUNCH_CHECK();
   return PL_OK;
 }
 
 extern "C" int pl_track_last_pose_dev(PLMap* map, int B, const float* Tcr, const int* ref_kf, float* Tcw_last, void* stream) {
   PL_ARG(map && B >= 1 && Tcr && ref_kf && Tcw_last);
-  if (map->n_kf < 1) { set_error("pl_track_last_pose_dev: the map has no keyframe graph (pl_map_set_keyframes)"); return PL_ERR_ARG; }
-  k_ref_pose<<<(B + 127) / 128, 128, 0, stream ? (cudaStream_t)stream : map->stream>>>(B, Tcr, ref_kf, map->kf_Tcw, map->n_kf, Tcw_last,
+  if (!map->kf) { set_error("pl_track_last_pose_dev: the map has no keyframe graph (pl_map_set_keyframes)"); return PL_ERR_ARG; }
+  k_ref_pose<<<(B + 127) / 128, 128, 0, stream ? (cudaStream_t)stream : map->stream>>>(B, Tcr, ref_kf, map->kf->Tcw, map->kf->n_kf, Tcw_last,
                                                                                       map->flag);
   PL_LAUNCH_CHECK();
   return PL_OK;

@@ -1,6 +1,8 @@
 """pl_track_update_local_map_dev, pl_track_local_map_lists_dev and the reference-keyframe poses against the restatement of
 tests/localmap_scene.py, and the whole localisation chain (LocalizationChain) against the separate calls, eagerly and replayed
 from one CUDA graph."""
+import gc
+
 import numpy as np
 import pytest
 
@@ -87,6 +89,10 @@ def test_capacity_overflow_reports_true_counts(quirk):
 def test_upload_refuses_bad_graphs(quirk):
     g, cases, names, M, (pm, kf, n_kf, ref), out = quirk
     d = ls.to_desc(g)
+    gc.collect()
+    held = pl.device_bytes()
+    M.set_keyframes(d)                                              # the same graph again: replaced, not added
+    assert pl.device_bytes() == held
     for key, edit in (("pt_slot", lambda a: a.__setitem__(0, g["n_points"])), ("cov", lambda a: a.__setitem__(0, len(g["bad"]))),
                       ("obs", lambda a: a.__setitem__(0, -1)), ("child_offset", lambda a: a.__setitem__(3, a[4] + 1)),
                       ("parent", lambda a: a.__setitem__(0, -2))):
@@ -97,6 +103,7 @@ def test_upload_refuses_bad_graphs(quirk):
     big = dict(d, Tcw=np.zeros((16385, 4, 4), np.float32), Twc=np.zeros((16385, 4, 4), np.float32))
     with pytest.raises(pl.PLError):
         M.set_keyframes(big)
+    assert pl.device_bytes() == held
     again = pl.update_local_map(M, pm, kf, n_kf, ref, CLP, CLL)       # the graph in place is kept
     for k, v in out.items():
         assert np.array_equal(again[k], v), k
