@@ -10,6 +10,7 @@
 // This is the measured "step" of bench.py and the e2e entry point (host buffers in, host buffers out).
 
 #include "common.cuh"
+#include "search.cuh"
 #include <vector>
 #include <string>
 #include <cstdio>
@@ -160,6 +161,14 @@ extern "C" int pl_frontend_create(const PLFrontendConfig* cfg, PLFrontend** out)
   PL_TRY(pl_line_create(&lc, &line));
   h->line.reset(line);
   h->capK = pl_orb_capacity(orb); h->capL = pl_line_capacity(line);
+  // every step matches consecutive frames at these capacities: refuse the ones the matchers cannot take here, not in each run
+  if (h->capK > kMatchMaxKeys) {
+    set_error("orb_nfeatures %d at %d levels gives a keypoint capacity of %d, over the matchers' %d; at most %d features fit at "
+              "%d levels", cfg->orb_nfeatures, cfg->orb_nlevels, h->capK, kMatchMaxKeys, kMatchMaxKeys - (h->capK - cfg->orb_nfeatures),
+              cfg->orb_nlevels);
+    return PL_ERR_ARG;
+  }
+  PL_TRY(search_double_fits(h->capL, h->capL));
   for (Stream* s : {&h->stream, &h->sLine, &h->sLm}) PL_TRY(s->create(cudaStreamNonBlocking));
   for (Event* e : {&h->evStart, &h->evLine, &h->evLm}) PL_TRY(e->create(cudaEventDisableTiming));
   // The three chains run on separate streams (PLSLAM_FRONTEND_OVERLAP=0: one stream): the low-occupancy kernels (matchers,

@@ -651,10 +651,12 @@ __device__ void line_candidates(const KeyLine68* kl, const double* lfunc, const 
         if (cosSita < TH) continue;
         const double* F = lfunc + 3 * id;
         const float dist = (float)(F[0] * (double)xs[i] + F[1] * (double)ys[i] + F[2]);
-        if (fabsf(dist) < r) atomicMin(&first[id], base + c * 1024 + (j - cb));   // order key: probe, cell rank, slot
+        // order key: probe, cell rank, slot.  A cell holds up to cap < 65536 lines, so the slot gets 16 bits; with 1024 a cell
+        // crossed by more lines would sort its slot 1024 + k like slot k of the next cell
+        if (fabsf(dist) < r) atomicMin(&first[id], base + c * 65536 + (j - cb));
       }
     }
-    base += 4000000;   // > 3072 cells * 1024
+    base += NCELL * 65536;   // three probes: < 2^30, clear of the distance bits of k_line_search's key
     __syncwarp();
   }
   __syncwarp();
@@ -1078,7 +1080,7 @@ extern "C" int pl_orb_search_for_initialization_dev(const PLKeyPoint* keys1, con
                                                     int* matches12, int* nmatches, int window_size, float nnratio,
                                                     int check_orientation, int* scratch, void* stream) {
   PL_ARG(keys1 && desc1 && n1 && keys2 && desc2 && n2 && bounds && prev_matched && matches12 && nmatches && scratch);
-  PL_ARG(cap > 0 && cap <= 6144 && B > 0);
+  PL_ARG(cap > 0 && cap <= kMatchMaxKeys && B > 0);
   size_t sm = grid_smem_bytes(cap);
   PL_CUDA(cudaFuncSetAttribute(k_search_init, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
   k_search_init<<<B, 32, sm, (cudaStream_t)stream>>>(keys1, desc1, n1, keys2, desc2, n2, cap, bounds, prev_matched,
@@ -1117,7 +1119,7 @@ extern "C" int pl_orb_search_by_projection_last(const PLKeyPoint* keys_cur, cons
                                                 const uint8_t* last_desc, const int* last_octave,
                                                 const float* last_angle, float th, int check_orientation,
                                                 const uint8_t* cur_preassigned, int* cur_match) {
-  PL_ARG(keys_cur && desc_cur && bounds && Tcw && K && scale_factors && cur_match && n_cur >= 0 && n_cur <= 6144 && n_last >= 0);
+  PL_ARG(keys_cur && desc_cur && bounds && Tcw && K && scale_factors && cur_match && n_cur >= 0 && n_cur <= kMatchMaxKeys && n_last >= 0);
   int rc = require_device(); if (rc) return rc;
   Staging s;
   const int cap = std::max(n_cur, 1), capl = std::max(n_last, 1);
@@ -1180,7 +1182,7 @@ int pl::search_by_projection_last_launch(const PLKeyPoint* keys_cur, const uint8
                                          float th, int check_orientation, const uint8_t* cur_preassigned, const int* gate_nmatches,
                                          int gate_min, int* cur_match, int* nmatches, void* stream) {
   PL_ARG(keys_cur && desc_cur && n_cur && bounds && Tcw && K && scale_factors && n_last && last_valid && last_pos && last_desc &&
-         last_octave && last_angle && cur_match && nmatches && B >= 1 && cap >= 1 && cap <= 6144 && cap_last >= 1);
+         last_octave && last_angle && cur_match && nmatches && B >= 1 && cap >= 1 && cap <= kMatchMaxKeys && cap_last >= 1);
   ProjLastArgs A;
   A.last_row = last_row;
   A.keys = keys_cur; A.desc = desc_cur; A.n = n_cur; A.cap = cap; A.bounds = bounds; A.Tcw = Tcw; A.K = K; A.scaleFactors = scale_factors;
@@ -1199,7 +1201,7 @@ int pl::search_by_projection_points_launch(const PLKeyPoint* keys, const uint8_t
                                            const uint8_t* mp_desc, float th, const float* th_frame, const int* desc_row, float nnratio,
                                            const uint8_t* preassigned, int* match, int* nmatches, void* stream) {
   PL_ARG(keys && desc && n && bounds && scale_factors && n_mp && in_view && proj && level && view_cos && mp_desc && match && nmatches &&
-         B >= 1 && cap >= 1 && cap <= 6144 && cap_mp >= 1);
+         B >= 1 && cap >= 1 && cap <= kMatchMaxKeys && cap_mp >= 1);
   ProjPointsArgs A{};
   A.th_frame = th_frame; A.desc_row = desc_row;
   A.keys = keys; A.desc = desc; A.n = n; A.cap = cap; A.bounds = bounds; A.scaleFactors = scale_factors; A.n_mp = n_mp; A.cap_mp = cap_mp;
@@ -1234,11 +1236,30 @@ extern "C" int pl_match_bf_knn2(const uint8_t* d1, int n1, const uint8_t* d2, in
   return s.fetch();
 }
 
+// m1[cap1], m2[cap2], bd0 and bd1[max(cap1, cap2)] of k_search_double
+static size_t search_double_smem(int cap1, int cap2) { return (size_t)(cap1 + cap2 + 2 * std::max(cap1, cap2)) * sizeof(short); }
+int pl::search_double_fits(int cap1, int cap2) {
+  int dev = 0, optin = 0;
+  cudaFuncAttributes fa;
+  PL_CUDA(cudaGetDevice(&dev));
+  PL_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+  PL_CUDA(cudaFuncGetAttributes(&fa, k_search_double));
+  const size_t room = optin > (int)fa.sharedSizeBytes ? (size_t)optin - fa.sharedSizeBytes : 0;
+  if (search_double_smem(cap1, cap2) > room) {
+    set_error("line matching of %d against %d lines needs %zu B of shared memory beside k_search_double's %zu static B, over the "
+              "device's %d B per block; at most %zu lines per side fit", cap1, cap2, search_double_smem(cap1, cap2),
+              (size_t)fa.sharedSizeBytes, optin, room / (4 * sizeof(short)));
+    return PL_ERR_ARG;
+  }
+  return PL_OK;
+}
+
 extern "C" int pl_lsd_search_double_dev(const uint8_t* d1, const int* n1, const uint8_t* d2, const int* n2, int cap1,
                                         int cap2, int B, float th, float nnratio, int mutual, int* matches,
                                         int* nmatches, void* stream) {
   PL_ARG(d1 && n1 && d2 && n2 && matches && nmatches && cap1 > 0 && cap2 > 0 && cap1 < 32000 && cap2 < 32000 && B > 0);
-  size_t sm = (size_t)(cap1 + cap2 + 2 * std::max(cap1, cap2)) * sizeof(short);
+  PL_TRY(search_double_fits(cap1, cap2));
+  const size_t sm = search_double_smem(cap1, cap2);
   PL_CUDA(cudaFuncSetAttribute(k_search_double, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
   k_search_double<<<B, 128, sm, (cudaStream_t)stream>>>(d1, n1, d2, n2, cap1, cap2, th, nnratio, mutual, matches,
                                                         nmatches);
@@ -1541,7 +1562,7 @@ extern "C" int pl_orb_search_by_projection_keyframe(const PLKeyPoint* keys_cur, 
                                                     const float* pos, const uint8_t* mp_desc, const float* min_dist,
                                                     const float* max_dist, const float* kf_angle, float th, int orb_dist,
                                                     int check_orientation, const uint8_t* cur_preassigned, int* cur_match) {
-  PL_ARG(keys_cur && desc_cur && bounds && Tcw && Ow && K && scale_factors && cur_match && n_cur >= 0 && n_cur <= 6144 && n_kf >= 0 && nlevels > 0);
+  PL_ARG(keys_cur && desc_cur && bounds && Tcw && Ow && K && scale_factors && cur_match && n_cur >= 0 && n_cur <= kMatchMaxKeys && n_kf >= 0 && nlevels > 0);
   PL_ARG(n_kf == 0 || (kf_valid && pos && mp_desc && min_dist && max_dist && kf_angle));
   int rc = require_device(); if (rc) return rc;
   Staging s;

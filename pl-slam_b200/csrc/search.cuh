@@ -9,6 +9,12 @@
 #include "common.cuh"
 
 namespace pl {
+// Largest keypoint capacity of the windowed point searches: their grid's 16-bit items and its `fill` area (one rotation bin byte
+// per query) hold at most this many keypoints per frame.
+constexpr int kMatchMaxKeys = 6144;
+// PL_OK if k_search_double's shared memory for line capacities cap1 and cap2 fits the device's opt-in limit per block beside the
+// kernel's static shared memory, else PL_ERR_ARG with a message naming the largest equal capacity that fits.
+int search_double_fits(int cap1, int cap2);
 int search_by_projection_last_launch(const PLKeyPoint* keys_cur, const uint8_t* desc_cur, const int* n_cur, int cap, int B,
                                      const float* bounds, const float* Tcw, const float* K, const float* scale_factors, int nlevels,
                                      const int* n_last, int cap_last, const uint8_t* last_valid, const float* last_pos,

@@ -41,9 +41,13 @@ def test_search_for_triangulation_edge_cases():
         M.SearchForTriangulation(*y)
 
 
-@pytest.mark.parametrize("seed,th", [(6, 3.0), (8, 3.0), (9, 1.0), (10, 6.0)])
-def test_fuse_search(seed, th):
-    f = synth.synth_fuse_problem(seed)
+FUSE_CASES = [(6, 3.0, 1800), (8, 3.0, 1800), (9, 1.0, 1800), (10, 6.0, 1800), (13, 3.0, 2049), (14, 3.0, 4000), (15, 6.0, 7000)]
+
+
+# the keypoint count joins a case's id past 1800: up to 2048 the grid keeps each octave beside its keypoint's index, above it not
+@pytest.mark.parametrize("seed,th,n_kp", FUSE_CASES, ids=[f"{s}-{t}" + (f"-{n}" if n != 1800 else "") for s, t, n in FUSE_CASES])
+def test_fuse_search(seed, th, n_kp):
+    f = synth.synth_fuse_problem(seed, n_kp=n_kp)
     args = (f["keys"], f["desc"], f["bounds"], f["Tcw"], f["Ow"], f["K"], f["scale_factors"], f["inv_level_sigma2"],
             f["log_scale_factor"], f["skip"], f["pos"], f["normal"], f["min_dist"], f["max_dist"], f["mp_desc"], th)
     obi, obd = oracle.fuse_search(*args)
@@ -91,10 +95,15 @@ def test_search_by_bow(seed, ori, ratio):
     assert pl.ORBmatcher(ratio, ori).SearchByBoW(a["keys"], a["desc"], a["has_mp"], b["keys"], b["desc"], {}, b["fv"])[0] == 0
 
 
-@pytest.mark.parametrize("seed,th,dist,ori", [(6, 10.0, 100, True), (8, 3.0, 64, True), (9, 10.0, 100, False), (10, 3.0, 64, False)])
-def test_search_by_projection_keyframe(seed, th, dist, ori):
+RELOC_CASES = [(6, 10.0, 100, True, 1800), (8, 3.0, 64, True, 1800), (9, 10.0, 100, False, 1800), (10, 3.0, 64, False, 1800),
+               (13, 10.0, 100, True, 2049), (14, 3.0, 64, False, 6144)]
+
+
+@pytest.mark.parametrize("seed,th,dist,ori,n_kp", RELOC_CASES,
+                         ids=[f"{s}-{t}-{d}-{o}" + (f"-{n}" if n != 1800 else "") for s, t, d, o, n in RELOC_CASES])
+def test_search_by_projection_keyframe(seed, th, dist, ori, n_kp):
     from test_oracle_localmap import _reloc_args
-    args, pre = _reloc_args(seed, th, dist)
+    args, pre = _reloc_args(seed, th, dist, n_kp)
     onm, om = oracle.search_by_projection_keyframe(*args, ori, pre)
     nm, m = pl.ORBmatcher(0.9, ori).SearchByProjectionKeyFrame(*args, pre)
     assert onm > 10 and nm == onm and np.array_equal(m, om)

@@ -110,8 +110,8 @@ def test_search_by_bow_known_answers():
     assert nm2 == 1 and m2[0] == 0
 
 
-def _reloc_args(seed, th=10.0, dist=100):
-    f = synth.synth_fuse_problem(seed)
+def _reloc_args(seed, th=10.0, dist=100, n_kp=1800):
+    f = synth.synth_fuse_problem(seed, n_kp=n_kp)
     rng = np.random.default_rng(seed)
     ang = rng.uniform(0, 360, len(f["pos"])).astype(np.float32)
     k = f["keys"].copy(); k["angle"] = rng.uniform(0, 360, len(k))

@@ -108,17 +108,39 @@ def test_quota_over_shared_memory_is_refused():
     _assert_same(kps, desc, *oracle.OrbOracle(fit, 1.2, 1, 20, 7).extract(img))
 
 
-def test_frontend_tracking_at_a_non_default_orb_setting():
-    """One front-end step with ORB at (1500, 1.1, 10, 12, 5), a distorting camera and the tracking stage: the extractor's
-    level count and scale table reach the projection searches (their window radius th * scale[octave]).  Each output equals
-    the oracle's on the same inputs, as in test_frontend_gpu.test_tracking_stage_matches_oracle."""
-    B, nf, sfac, nl, ini, mn = 3, 1500, 1.1, 10, 12, 5
+def test_matcher_capacities_are_refused_at_creation():
+    """A front end whose keypoint capacity (nfeatures + 4 * nlevels) is over the matchers' 6144, or whose line capacity is over
+    what the line matcher's shared memory holds, is refused at creation with a message naming the limit; 6144 - 4 * nlevels
+    features are accepted."""
+    from test_match_batched_gpu import _search_double_limit
+    with pytest.raises(pl.PLError, match=r"error -1: .*keypoint capacity of 7032, over the matchers' 6144; at most 6112 features fit at 8 levels"):
+        pl.Frontend(640, 480, max_batch=1, orb=(7000, 1.2, 8, 20, 7))
+    with pytest.raises(pl.PLError, match=r"error -1: .*at most 6104 features fit at 10 levels"):
+        pl.Frontend(640, 480, max_batch=1, orb=(6105, 1.2, 10, 20, 7))
+    fe = pl.Frontend(640, 480, max_batch=1, orb=(6112, 1.2, 8, 20, 7))
+    del fe
+    fit = _search_double_limit()
+    with pytest.raises(pl.PLError, match=rf"error -1: .* at most {fit} lines per side"):
+        pl.Frontend(640, 480, max_batch=1, lines=(fit, 0.0))
+
+
+def _frontend_tracking_step(w, h, nf, sfac, nl, ini, mn):
+    """One front-end step of 3 frames at a w x h frame with ORB at (nf, sfac, nl, ini, mn), the TUM1 camera scaled to the frame
+    (distorting) and the tracking stage; every output equals the oracle's on the same inputs, as in
+    test_frontend_gpu.test_tracking_stage_matches_oracle.  Returns the front end's outputs."""
+    B = 3
     K, D = synth.TUM1_K, synth.TUM1_DIST
+    if (w, h) != (640, 480):
+        K = tuple(float(v) for v in np.array(K) * (w / 640, h / 480, w / 640, h / 480))
+    # hd: the VGA sequence scaled up, whose smoother texture keeps LSD under the front end's 8192 segments per frame (a native
+    # 1920 x 1080 synthetic frame gives over 13000) while ORB still finds its 5000 keypoints
     frames = synth.synth_sequence(B, 640, 480, seed=14)
-    problems = [synth.synth_pose_problem(130 + k) for k in range(B)]
+    if (w, h) != (640, 480):
+        frames = np.stack([oracle.resize_linear_u8(f, w, h) for f in frames])
+    problems = [synth.synth_pose_problem(130 + k, K=K, w=w, h=h) for k in range(B)]
     for p in problems[1:]:
         p["K"] = problems[0]["K"]
-    fe = pl.Frontend(640, 480, max_batch=B, orb=(nf, sfac, nl, ini, mn), lm_caps=(320, 88))
+    fe = pl.Frontend(w, h, max_batch=B, orb=(nf, sfac, nl, ini, mn), lm_caps=(320, 88))
     fe.set_camera(K, D)
     fe.set_wrap(True)
     fe.set_pose_problems(problems)
@@ -129,7 +151,7 @@ def test_frontend_tracking_at_a_non_default_orb_setting():
     o = oracle.OrbOracle(nf, sfac, nl, ini, mn)
     sf = o.tables()["scale"]
     assert len(sf) == nl
-    bounds = oracle.image_bounds(K, D, 640, 480)
+    bounds = oracle.image_bounds(K, D, w, h)
     Kp = np.asarray(problems[0]["K"], np.float32)
     for b in range(B):
         okps, odesc = o.extract(frames[b])
@@ -159,5 +181,20 @@ def test_frontend_tracking_at_a_non_default_orb_setting():
                                                      np.ones(npv, np.float32), pd, 1.0, 0.8, (m >= 0).astype(np.uint8))
         assert t1["n_pt"][b] == nm2 and np.array_equal(t1["pt_match"][b, :n], m2), b
         searched += nm + nm2
+    assert searched > 100
+    return out
+
+
+def test_frontend_tracking_at_a_non_default_orb_setting():
+    """ORB at (1500, 1.1, 10, 12, 5): the extractor's level count and scale table reach the projection searches (their window
+    radius th * scale[octave])."""
+    out = _frontend_tracking_step(640, 480, 1500, 1.1, 10, 12, 5)
     # keypoints on levels past the TUM setting's 8 take part in the matches
-    assert searched > 100 and any((out["kps"][b, :out["n"][b]]["octave"] >= 8).any() for b in range(B))
+    assert any((out["kps"][b, :out["n"][b]]["octave"] >= 8).any() for b in range(3))
+
+
+def test_frontend_tracking_past_the_packed_grid():
+    """1920 x 1080 with 5000 features: over 2048 keypoints per frame, so SearchForInitialization and the tracking searches of
+    the front end's batched chain run on the grid whose items are plain keypoint indices."""
+    out = _frontend_tracking_step(1920, 1080, 5000, 1.2, 8, 20, 7)
+    assert out["n"].min() > 2048
