@@ -323,9 +323,46 @@ typedef struct PLBAProblem {
 } PLBAProblem;
 /* stop_flag_dev: device-visible int (e.g. mapped pinned memory) polled like g2o's forceStopFlag; NULL = never stop.
  * Outputs: optimised keyframe poses, points, line end points; pe_erase / le_erase = observations the reference would
- * erase (:2005-2043), le_erase_kf = the keyframe index the reference pairs with line observation i (its i/2 quirk). */
+ * erase (:2005-2043), le_erase_kf = the keyframe index the reference pairs with line observation i (its i/2 quirk).
+ * PL_ERR_ARG for more than 7723 free keyframes (the dense reduced system, (6 n_free)^2 doubles, is indexed with an int). */
 int pl_local_ba(const PLBAProblem* p, const int* stop_flag_dev, float* kf_Tcw_out, float* pt_Xw_out, double* ln_Xw_out,
                 uint8_t* pe_erase, uint8_t* le_erase, int* le_erase_kf, int* iterations);
+
+/* W local windows in one launch, on device pointers, asynchronous.  Window w is the PLBAProblem made of row w: counts
+ * n_*[w] (device arrays [W]) and rows of capacity cap_* in [W][cap] layouts (kf_Tcw [W][cap_kf][16], kf_fixed [W][cap_kf],
+ * kf_K [W][cap_kf][4], K_end [W][4], pt_Xw [W][cap_pt][3], ln_Xw [W][cap_ln][6], pe_kf / pe_pt / pe_inv_sigma2 [W][cap_pe],
+ * pe_obs [W][cap_pe][2], le_kf / le_ln [W][cap_le], le_func [W][cap_le][3]); edge indices are relative to the window's own
+ * rows.  Same meaning and units as PLBAProblem. */
+typedef struct PLBAWindows {
+  int W;
+  int cap_kf, cap_pt, cap_ln, cap_pe, cap_le;
+  const int* n_kf; const int* n_pt; const int* n_ln; const int* n_pe; const int* n_le;
+  const float* kf_Tcw; const uint8_t* kf_fixed; const float* kf_K; const float* K_end;
+  const float* pt_Xw; const double* ln_Xw;
+  const int* pe_kf; const int* pe_pt; const float* pe_obs; const float* pe_inv_sigma2;
+  const int* le_kf; const int* le_ln; const double* le_func;
+} PLBAWindows;
+/* Outputs of pl_local_ba_dev (device arrays, all required), in the layouts of the inputs: kf_Tcw [W][cap_kf][16],
+ * pt_Xw [W][cap_pt][3], ln_Xw [W][cap_ln][6], pe_erase [W][cap_pe], le_erase / le_erase_kf [W][cap_le], iterations [W],
+ * status [W].  Entries past a window's counts are never written.  status[w] = 0: window w ran; 1: one of its counts is
+ * negative or over its capacity; 2: one of its edges names a keyframe or landmark outside its counts.  A window with a
+ * nonzero status writes only status[w] and iterations[w] = 0; its other outputs keep what they held. */
+typedef struct PLBAOut {
+  float* kf_Tcw; float* pt_Xw; double* ln_Xw; uint8_t* pe_erase; uint8_t* le_erase; int* le_erase_kf;
+  int* iterations; int* status;
+} PLBAOut;
+/* Device scratch of pl_local_ba_dev: per window, the dense reduced pose system of (6 cap_kf)^2 doubles, the edge Jacobians and
+ * the two CSR indices.  0 for arguments pl_local_ba_dev refuses. */
+size_t pl_local_ba_scratch_bytes(int W, int cap_kf, int cap_pt, int cap_ln, int cap_pe, int cap_le);
+/* pl_local_ba on W windows, one CTA per window, enqueued on `stream` (NULL = the legacy default stream): kernels only, no
+ * allocation, copy or synchronisation, so the call can be captured into a CUDA graph.  stop_flag_dev as in pl_local_ba, for
+ * every window.  scratch: pl_local_ba_scratch_bytes(W, caps) bytes of device memory, 16-byte aligned; nothing past them is
+ * written.  PL_ERR_ARG before anything is enqueued for a NULL windows / out / array / scratch (W > 0), W < 0, or a capacity
+ * outside its limits: 1 <= cap_kf <= 7723 (the kernel indexes the (6 cap_kf)^2 reduced system with an int), cap_pt, cap_ln,
+ * cap_pe, cap_le in 1 .. 2^24, and W * cap of every capacity within an int.  W = 0 enqueues nothing.  Counts and edge indices
+ * are checked on the device (status).  Windows are independent: each one's results equal pl_local_ba's on its problem, up to
+ * the last bits the fp64-atomic Schur sum leaves to chance. */
+int pl_local_ba_dev(const PLBAWindows* windows, const int* stop_flag_dev, const PLBAOut* out, void* scratch, void* stream);
 
 /* Optimizer::BundleAdjustment with lines (src/Optimizer.cc:275-638; GlobalBundleAdjustemnt :41-58 passes the whole map):
  * ONE Levenberg-Marquardt optimize(n_iterations) over all keyframes (kf_fixed = mnId == 0), map points and map-line end points,

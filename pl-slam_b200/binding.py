@@ -625,6 +625,131 @@ def LocalBundleAdjustmentWithLine(p, stop_flag_dev=None):
 Optimizer.LocalBundleAdjustmentWithLine = staticmethod(LocalBundleAdjustmentWithLine)
 
 
+class PLBAWindows(C.Structure):
+    _fields_ = ([("W", C.c_int)] + [(f"cap_{k}", C.c_int) for k in ("kf", "pt", "ln", "pe", "le")] +
+                [(f"n_{k}", vp) for k in ("kf", "pt", "ln", "pe", "le")] +
+                [(k, vp) for k in ("kf_Tcw", "kf_fixed", "kf_K", "K_end", "pt_Xw", "ln_Xw", "pe_kf", "pe_pt", "pe_obs", "pe_inv_sigma2",
+                                   "le_kf", "le_ln", "le_func")])
+
+
+class PLBAOut(C.Structure):
+    _fields_ = [(k, vp) for k in ("kf_Tcw", "pt_Xw", "ln_Xw", "pe_erase", "le_erase", "le_erase_kf", "iterations", "status")]
+
+
+BA_COUNTS = ("kf", "pt", "ln", "pe", "le")
+# field -> (the count its rows follow, row shape, dtype), in the [W][cap] layouts of PLBAWindows / PLBAOut
+BA_INPUTS = {"kf_Tcw": ("kf", (16,), np.float32), "kf_fixed": ("kf", (), np.uint8), "kf_K": ("kf", (4,), np.float32),
+             "pt_Xw": ("pt", (3,), np.float32), "ln_Xw": ("ln", (6,), np.float64), "pe_kf": ("pe", (), np.int32),
+             "pe_pt": ("pe", (), np.int32), "pe_obs": ("pe", (2,), np.float32), "pe_inv_sigma2": ("pe", (), np.float32),
+             "le_kf": ("le", (), np.int32), "le_ln": ("le", (), np.int32), "le_func": ("le", (3,), np.float64)}
+BA_OUTPUTS = {"kf_Tcw": ("kf", (16,), np.float32), "pt_Xw": ("pt", (3,), np.float32), "ln_Xw": ("ln", (6,), np.float64),
+              "pe_erase": ("pe", (), np.uint8), "le_erase": ("le", (), np.uint8), "le_erase_kf": ("le", (), np.int32)}
+
+
+def _ba_lib():
+    L = lib()
+    if not getattr(L, "_ba_types", False):
+        L.pl_local_ba_scratch_bytes.argtypes = [C.c_int] * 6
+        L.pl_local_ba_scratch_bytes.restype = C.c_size_t
+        L.pl_local_ba_dev.argtypes = [C.POINTER(PLBAWindows), vp, C.POINTER(PLBAOut), vp, vp]
+        L._ba_types = True
+    return L
+
+
+def ba_window_counts(p):
+    """{kf, pt, ln, pe, le} counts of one local window (dict as made by synth.synth_ba_problem)."""
+    return dict(kf=len(p["kf_fixed"]), pt=len(p["pt_Xw"]), ln=len(p["ln_Xw"]), pe=len(p["pe_kf"]), le=len(p["le_kf"]))
+
+
+def pack_ba_windows(problems, caps=None, fill=0):
+    """Local windows (dicts as made by synth.synth_ba_problem; their sizes may differ) -> host arrays in the [W][cap] layouts of
+    PLBAWindows: dict(W, caps={kf, pt, ln, pe, le}, n_kf .. n_le [W], K_end [W][4], and one [W][cap][...] array per field of
+    BA_INPUTS).  caps (optional dict): capacities at least each window's counts; by default the largest count (at least 1).
+    Every byte of a row past its window's count is `fill`."""
+    counts = [ba_window_counts(p) for p in problems]
+    W = len(problems)
+    c = {k: max([1] + [n[k] for n in counts]) for k in BA_COUNTS}
+    for k, v in (caps or {}).items():
+        if v < c[k]:
+            raise ValueError(f"cap_{k} = {v} is below a window's count {c[k]}")
+        c[k] = int(v)
+    out = dict(W=W, caps=c, K_end=np.array([np.asarray(p["K_end"], np.float32).reshape(4) for p in problems], np.float32).reshape(W, 4))
+    for k in BA_COUNTS:
+        out["n_" + k] = np.array([n[k] for n in counts], np.int32)
+    for f, (k, shape, dt) in BA_INPUTS.items():
+        a = np.empty((W, c[k]) + shape, dt)
+        a.view(np.uint8)[...] = fill
+        for w, p in enumerate(problems):
+            a[w, :counts[w][k]] = np.asarray(p[f], dt).reshape((-1,) + shape)
+        out[f] = a
+    return out
+
+
+def unpack_ba_rows(arrays, counts, fields):
+    """Per-window dicts of `fields` (name -> (count, ...), as BA_INPUTS / BA_OUTPUTS) from [W][cap] arrays, each trimmed to its
+    window's count: counts = {kf: [W], ...}.  Nothing past a count is read."""
+    W = len(counts["kf"])
+    return [{f: np.array(arrays[f][w, :int(counts[k][w])]) for f, (k, _, _) in fields.items()} for w in range(W)]
+
+
+class LocalBAWindows:
+    """W local windows on the device for pl_local_ba_dev (Optimizer::LocalBundleAdjustmentWithLine on each): the constructor
+    packs them (pack_ba_windows) into torch CUDA tensors and allocates the outputs and the scratch once; run() only enqueues the
+    launch, so it can be captured into a CUDA graph; results() waits for it and returns per-window dicts with the keys of
+    LocalBundleAdjustmentWithLine plus `status`.  Output rows are pre-filled with `out_fill` bytes."""
+
+    def __init__(self, problems, caps=None, out_fill=0):
+        import torch
+        h = pack_ba_windows(problems, caps)
+        self.W, self.caps = h["W"], h["caps"]
+        self.counts = {k: h["n_" + k] for k in BA_COUNTS}
+        self.inputs = {k: torch.from_numpy(np.ascontiguousarray(v)).cuda() for k, v in h.items() if isinstance(v, np.ndarray)}
+        W, c = self.W, self.caps
+        self.outputs = {f: torch.empty((W, c[k]) + shape, dtype=getattr(torch, np.dtype(dt).name), device="cuda")
+                        for f, (k, shape, dt) in BA_OUTPUTS.items()}
+        for t in self.outputs.values():
+            t.view(torch.uint8).fill_(out_fill)
+        self.outputs["iterations"] = torch.full((W,), -1, dtype=torch.int32, device="cuda")
+        self.outputs["status"] = torch.full((W,), -1, dtype=torch.int32, device="cuda")
+        L = _ba_lib()
+        caps_ = [c[k] for k in BA_COUNTS]
+        self.scratch = torch.empty(max(int(L.pl_local_ba_scratch_bytes(W, *caps_)), 1), dtype=torch.uint8, device="cuda")
+        ins = self.inputs
+        self._win = PLBAWindows(W, *caps_, *[ins["n_" + k].data_ptr() for k in BA_COUNTS],
+                                *[ins[f].data_ptr() for f in ("kf_Tcw", "kf_fixed", "kf_K", "K_end", "pt_Xw", "ln_Xw", "pe_kf",
+                                                              "pe_pt", "pe_obs", "pe_inv_sigma2", "le_kf", "le_ln", "le_func")])
+        self._out = PLBAOut(*[self.outputs[f].data_ptr() for f, _ in PLBAOut._fields_])
+        torch.cuda.synchronize()        # the uploads ran on the current stream; run() may use another one
+
+    def run(self, stream=None, stop_flag_dev=None):
+        """pl_local_ba_dev on `stream` (a torch.cuda.Stream; None = the legacy default stream): enqueues, does not wait.
+        stop_flag_dev: device address of an int32 polled like g2o's forceStopFlag, or None."""
+        s = None if stream is None else stream.cuda_stream
+        check(_ba_lib().pl_local_ba_dev(C.byref(self._win), stop_flag_dev, C.byref(self._out), self.scratch.data_ptr(), s))
+
+    def results(self):
+        import torch
+        torch.cuda.synchronize()
+        host = {k: v.cpu().numpy() for k, v in self.outputs.items()}
+        res = unpack_ba_rows(host, self.counts, BA_OUTPUTS)
+        for w, r in enumerate(res):
+            r["its"] = int(host["iterations"][w])
+            r["status"] = int(host["status"][w])
+        return res
+
+
+
+def LocalBundleAdjustmentWithLineBatch(problems, stream=None, stop_flag_dev=None):
+    """Optimizer::LocalBundleAdjustmentWithLine on several windows in one pl_local_ba_dev launch (one CTA per window).
+    Returns one dict per window: the keys of LocalBundleAdjustmentWithLine plus `status` (0 = ran)."""
+    b = LocalBAWindows(problems)
+    b.run(stream, stop_flag_dev)
+    return b.results()
+
+
+Optimizer.LocalBundleAdjustmentWithLineBatch = staticmethod(LocalBundleAdjustmentWithLineBatch)
+
+
 def GlobalBundleAdjustemnt(p, nIterations=5, bRobust=True, stop_flag=None):
     """Optimizer::GlobalBundleAdjustemnt / BundleAdjustment with lines (Optimizer.cc:41-58,275-638; the reference's spelling) on
     a flattened map (dict as made by synth.synth_ba_problem; K_end is not read).  stop_flag: None or an int32 numpy scalar
