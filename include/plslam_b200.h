@@ -530,6 +530,61 @@ int pl_lsd_fuse_search(const void* keylines, int nl, const uint8_t* kf_point_des
                        const double* pos, const double* normal, const float* min_dist, const float* max_dist, const uint8_t* ml_desc,
                        float th, int* best_idx, int* best_dist, int* stop_at);
 
+/* ------------------------------------------------------------------ many Fuse searches in one launch (LocalMapping::SearchInNeighbors)
+ * The search halves of pl_orb_fuse_search / pl_lsd_fuse_search for P problems at once, on device pointers, enqueued on `stream`
+ * (NULL = the legacy default stream): kernels only, no allocation, copy or synchronisation, so the calls can be captured into a
+ * CUDA graph.  The host-pointer functions above are their P = 1 case.
+ *
+ * Problem p searches the landmarks of entries offset[p] .. offset[p] + count[p] - 1 against keyframe kf[p] with radius factor
+ * th[p], and writes the result of its j-th entry to best_idx / best_dist [out_offset[p] + j].  Entry e names landmark entry_lm[e]
+ * and carries its own skip byte entry_skip[e] (skip = !pMP || isBad() || IsInKeyFrame(target): it depends on the target).
+ * Problems may share a keyframe and an entry range; their output ranges must not overlap. */
+typedef struct PLFuseProblems {
+  int P;
+  const int* kf; const float* th; const int* offset; const int* count; const int* out_offset;   /* [P] */
+  int n_entries; const int* entry_lm; const uint8_t* entry_skip;                                /* [n_entries] */
+  int n_out;                                                                                    /* length of the outputs */
+} PLFuseProblems;
+/* Point keyframes: rows of capacity cap, keys_un [n_kf][cap] (mvKeysUn), desc [n_kf][cap][32], n [n_kf]; per keyframe Tcw
+ * [n_kf][16], Ow [n_kf][3], K [n_kf][4] (fx fy cx cy), bounds [n_kf][4]; the scale tables are shared by every keyframe. */
+typedef struct PLFuseKeyframes {
+  int n_kf, cap;
+  const PLKeyPoint* keys_un; const uint8_t* desc; const int* n;
+  const float* Tcw; const float* Ow; const float* K; const float* bounds;
+  const float* scale_factors; const float* inv_level_sigma2; int nlevels; float log_scale_factor;
+} PLFuseKeyframes;
+/* Map points, as pl_orb_fuse_search takes them: pos / normal [n][3], raw min / max distance [n], desc [n][32]. */
+typedef struct PLFusePoints {
+  int n; const float* pos; const float* normal; const float* min_dist; const float* max_dist; const uint8_t* desc;
+} PLFusePoints;
+/* Line keyframes: keylines [n_kf][cap] (68-byte records), n [n_kf]; the keyframe's POINT descriptors pdesc [n_kf][cap_pdesc][32]
+ * with n_pdesc [n_kf] rows (see pl_lsd_fuse_search); Tcw, Ow, K, bounds as PLFuseKeyframes; scale_line / log_scale_factor_line
+ * shared. */
+typedef struct PLFuseLineKeyframes {
+  int n_kf, cap, cap_pdesc;
+  const void* keylines; const int* n; const uint8_t* pdesc; const int* n_pdesc;
+  const float* Tcw; const float* Ow; const float* K; const float* bounds;
+  float scale_line, log_scale_factor_line;
+} PLFuseLineKeyframes;
+/* Map lines, as pl_lsd_fuse_search takes them: pos [n][6] (start, end), normal [n][3], raw min / max distance [n], desc [n][32]. */
+typedef struct PLFuseLines {
+  int n; const double* pos; const double* normal; const float* min_dist; const float* max_dist; const uint8_t* desc;
+} PLFuseLines;
+/* status[p] = 0: problem p ran; 1: kf[p], its entry range or its output range lies outside its table; 2: its keyframe's count
+ * (n, or n_pdesc for lines) is negative or over the capacity; 3: one of its entries names a landmark outside the table.  A
+ * problem with a nonzero status writes nothing but status[p].  Lines: stop_at[p] = the position j inside the problem of the first
+ * entry that is not skipped and has an end point behind the camera (count[p] if none); entries from there on get -1 / 256.
+ * stop_at is decided on the skip bytes given: if the caller's surgery at an earlier target has since made that entry skipped,
+ * the reference steps over it, so the entries after it must be searched again (INTEGRATION.md, SearchInNeighbors).
+ * PL_ERR_ARG before anything is enqueued for P < 0 or n_entries, n_out, landmark count < 0; and, when P > 0, for a NULL table,
+ * array or output, n_kf < 1, nlevels < 1, cap outside 1 .. 6144 (points) or 1 .. 32768 (lines), cap_pdesc outside 1 .. 32768,
+ * or n_kf * cap beyond an int.  P = 0 enqueues nothing.  Each problem equals pl_orb_fuse_search / pl_lsd_fuse_search on its
+ * keyframe and the landmarks of its entries, bit for bit. */
+int pl_orb_fuse_search_dev(const PLFuseKeyframes* kfs, const PLFusePoints* points, const PLFuseProblems* problems, int* best_idx,
+                           int* best_dist, int* status, void* stream);
+int pl_lsd_fuse_search_dev(const PLFuseLineKeyframes* kfs, const PLFuseLines* lines, const PLFuseProblems* problems, int* best_idx,
+                           int* best_dist, int* stop_at, int* status, void* stream);
+
 /* ------------------------------------------------------------------ tracking a batch of frames against a fixed map
  * Tracking::TrackLocalMapWithLines (src/Tracking.cc:1491-1562) with SearchLocalPoints (:1751-1801) and SearchLocalLines
  * (:1803-1855), in localisation mode (mbOnlyTracking), for B frames at once; every intermediate stays on the device.

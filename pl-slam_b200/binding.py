@@ -1030,6 +1030,183 @@ def _lsd_fuse_search(self, keylines, kf_point_desc, bounds, Tcw, Ow, K, scale_li
 LSDmatcher.FuseSearch = _lsd_fuse_search
 
 
+# ---------------------------------------------------------------------------------------------- many Fuse searches in one launch
+class PLFuseProblems(C.Structure):
+    _fields_ = [("P", C.c_int), ("kf", vp), ("th", vp), ("offset", vp), ("count", vp), ("out_offset", vp),
+                ("n_entries", C.c_int), ("entry_lm", vp), ("entry_skip", vp), ("n_out", C.c_int)]
+
+
+class PLFuseKeyframes(C.Structure):
+    _fields_ = [("n_kf", C.c_int), ("cap", C.c_int), ("keys_un", vp), ("desc", vp), ("n", vp), ("Tcw", vp), ("Ow", vp), ("K", vp),
+                ("bounds", vp), ("scale_factors", vp), ("inv_level_sigma2", vp), ("nlevels", C.c_int), ("log_scale_factor", C.c_float)]
+
+
+class PLFuseLineKeyframes(C.Structure):
+    _fields_ = [("n_kf", C.c_int), ("cap", C.c_int), ("cap_pdesc", C.c_int), ("keylines", vp), ("n", vp), ("pdesc", vp), ("n_pdesc", vp),
+                ("Tcw", vp), ("Ow", vp), ("K", vp), ("bounds", vp), ("scale_line", C.c_float), ("log_scale_factor_line", C.c_float)]
+
+
+class PLFuseLandmarks(C.Structure):      # PLFusePoints and PLFuseLines: the same fields, float or double positions
+    _fields_ = [("n", C.c_int), ("pos", vp), ("normal", vp), ("min_dist", vp), ("max_dist", vp), ("desc", vp)]
+
+
+def _fuse_lib():
+    L = lib()
+    if not getattr(L, "_fuse_types", False):
+        L.pl_orb_fuse_search_dev.argtypes = [C.POINTER(PLFuseKeyframes), C.POINTER(PLFuseLandmarks), C.POINTER(PLFuseProblems)] + [vp] * 4
+        L.pl_lsd_fuse_search_dev.argtypes = [C.POINTER(PLFuseLineKeyframes), C.POINTER(PLFuseLandmarks), C.POINTER(PLFuseProblems)] + [vp] * 5
+        L._fuse_types = True
+    return L
+
+
+def pack_fuse_keyframes(keyframes, lines=False, cap=None, cap_pdesc=None):
+    """Keyframes (dicts: keys [n] KP_DTYPE and desc [n][32] for points, kl [n] KEYLINE_DTYPE and pdesc [m][32] for lines; Tcw [16],
+    Ow [3], K [4], bounds [4]) -> host arrays in the [n_kf][cap] layouts of PLFuseKeyframes / PLFuseLineKeyframes.  cap /
+    cap_pdesc default to the largest count (at least 1); rows past a keyframe's count are zero."""
+    n_kf = len(keyframes)
+    cam = dict(Tcw=np.array([np.asarray(k["Tcw"], np.float32).reshape(16) for k in keyframes], np.float32).reshape(n_kf, 16),
+               Ow=np.array([np.asarray(k["Ow"], np.float32).reshape(3) for k in keyframes], np.float32).reshape(n_kf, 3),
+               K=np.array([np.asarray(k["K"], np.float32).reshape(4) for k in keyframes], np.float32).reshape(n_kf, 4),
+               bounds=np.array([np.asarray(k["bounds"], np.float32).reshape(4) for k in keyframes], np.float32).reshape(n_kf, 4))
+
+    def rows(name, dt, shape, c):
+        counts = np.array([len(k[name]) for k in keyframes], np.int32)
+        c = max([1] + list(counts)) if c is None else int(c)
+        if counts.size and counts.max() > c:
+            raise ValueError(f"a keyframe has {counts.max()} {name}, over the capacity {c}")
+        a = np.zeros((n_kf, c) + shape, dt)
+        for i, k in enumerate(keyframes):
+            a[i, :counts[i]] = np.asarray(k[name], dt).reshape((-1,) + shape)
+        return a, counts, c
+
+    if lines:
+        kl, n, cap = rows("kl", KEYLINE_DTYPE, (), cap)
+        pdesc, n_pdesc, cap_pdesc = rows("pdesc", np.uint8, (32,), cap_pdesc)
+        return dict(cam, keylines=kl, n=n, pdesc=pdesc, n_pdesc=n_pdesc, cap=cap, cap_pdesc=cap_pdesc)
+    keys, n, cap = rows("keys", KP_DTYPE, (), cap)
+    desc, _, _ = rows("desc", np.uint8, (32,), cap)
+    return dict(cam, keys_un=keys, desc=desc, n=n, cap=cap)
+
+
+def pack_fuse_problems(problems, entry_lists):
+    """Problems and their entry lists -> host arrays of PLFuseProblems.  entry_lists: (lm [m] landmark rows, skip [m]) pairs, packed
+    one after the other; problems: (kf, th, list) triples, `list` indexing entry_lists, so problems may share a list.  The outputs of
+    problem p follow those of problem p - 1: out_offset = running sum of the counts."""
+    lm = [np.asarray(l, np.int32).reshape(-1) for l, _ in entry_lists]
+    sk = [np.asarray(s, np.uint8).reshape(-1) for _, s in entry_lists]
+    if any(len(a) != len(b) for a, b in zip(lm, sk)):
+        raise ValueError("an entry list's landmark and skip arrays differ in length")
+    starts = np.cumsum([0] + [len(a) for a in lm]).astype(np.int32)
+    P = len(problems)
+    kf = np.array([int(p[0]) for p in problems], np.int32)
+    th = np.array([float(p[1]) for p in problems], np.float32)
+    offset = np.array([starts[p[2]] for p in problems], np.int32)
+    count = np.array([len(lm[p[2]]) for p in problems], np.int32)
+    out_offset = np.concatenate([[0], np.cumsum(count)[:-1]]).astype(np.int32) if P else np.zeros(0, np.int32)
+    return dict(P=P, kf=kf, th=th, offset=offset, count=count, out_offset=out_offset,
+                entry_lm=np.concatenate(lm + [np.zeros(0, np.int32)]), entry_skip=np.concatenate(sk + [np.zeros(0, np.uint8)]),
+                n_out=int(count.sum()))
+
+
+def pack_fuse_landmarks(landmarks, lines=False):
+    """Map points or lines (dict: pos [n][3] or [n][6], normal [n][3], min_dist, max_dist [n] raw, desc [n][32]) -> host arrays."""
+    ft = np.float64 if lines else np.float32
+    return dict(pos=np.ascontiguousarray(landmarks["pos"], ft).reshape(-1, 6 if lines else 3),
+                normal=np.ascontiguousarray(landmarks["normal"], ft).reshape(-1, 3),
+                min_dist=np.ascontiguousarray(landmarks["min_dist"], np.float32).reshape(-1),
+                max_dist=np.ascontiguousarray(landmarks["max_dist"], np.float32).reshape(-1),
+                desc=np.ascontiguousarray(landmarks["desc"], np.uint8).reshape(-1, 32))
+
+
+class FuseProblems:
+    """A batch of Fuse searches on the device for pl_orb_fuse_search_dev (lines=False) or pl_lsd_fuse_search_dev (lines=True): the
+    constructor packs the keyframe table, the landmark table and the problems (pack_fuse_keyframes, pack_fuse_landmarks,
+    pack_fuse_problems) into torch CUDA tensors and allocates the outputs once; run() only enqueues the launch, so it can be
+    captured into a CUDA graph; results() waits for it and returns one dict per problem: best_idx, best_dist (numpy, one per entry),
+    status, and stop_at for lines.  scales: scale_factors, inv_level_sigma2, log_scale_factor (points) or scale_line,
+    log_scale_factor_line (lines).  Outputs are pre-filled with `out_fill`."""
+
+    def __init__(self, keyframes, landmarks, problems, entry_lists, scales, lines=False, out_fill=-7):
+        import torch
+        self.lines = lines
+        k = pack_fuse_keyframes(keyframes, lines)
+        q = pack_fuse_problems(problems, entry_lists)
+        m = pack_fuse_landmarks(landmarks, lines)
+        dev = lambda a: torch.from_numpy(np.ascontiguousarray(a).view(np.uint8) if a.dtype.names else np.ascontiguousarray(a)).cuda()
+        self.host = dict(k=k, q=q, m=m)
+        self.inputs = {f"k_{n}": dev(v) for n, v in k.items() if isinstance(v, np.ndarray)}
+        self.inputs.update({f"q_{n}": dev(v) for n, v in q.items() if isinstance(v, np.ndarray)})
+        self.inputs.update({f"m_{n}": dev(v) for n, v in m.items()})
+        if not lines:
+            for n in ("scale_factors", "inv_level_sigma2"):
+                self.inputs[n] = dev(np.asarray(scales[n], np.float32))
+        P, n_out = q["P"], q["n_out"]
+        self.P, self.count = P, q["count"]
+        self.outputs = {n: torch.full((max(n_out, 1),), out_fill, dtype=torch.int32, device="cuda") for n in ("best_idx", "best_dist")}
+        self.outputs["status"] = torch.full((max(P, 1),), out_fill, dtype=torch.int32, device="cuda")
+        if lines:
+            self.outputs["stop_at"] = torch.full((max(P, 1),), out_fill, dtype=torch.int32, device="cuda")
+        i = lambda n: self.inputs[n].data_ptr()
+        self._q = PLFuseProblems(P, i("q_kf"), i("q_th"), i("q_offset"), i("q_count"), i("q_out_offset"), len(q["entry_lm"]),
+                                 i("q_entry_lm"), i("q_entry_skip"), n_out)
+        self._m = PLFuseLandmarks(len(m["desc"]), i("m_pos"), i("m_normal"), i("m_min_dist"), i("m_max_dist"), i("m_desc"))
+        n_kf = len(keyframes)
+        if lines:
+            self._k = PLFuseLineKeyframes(n_kf, k["cap"], k["cap_pdesc"], i("k_keylines"), i("k_n"), i("k_pdesc"), i("k_n_pdesc"), i("k_Tcw"),
+                                          i("k_Ow"), i("k_K"), i("k_bounds"), float(scales["scale_line"]), float(scales["log_scale_factor_line"]))
+        else:
+            self._k = PLFuseKeyframes(n_kf, k["cap"], i("k_keys_un"), i("k_desc"), i("k_n"), i("k_Tcw"), i("k_Ow"), i("k_K"), i("k_bounds"),
+                                      i("scale_factors"), i("inv_level_sigma2"), len(scales["scale_factors"]), float(scales["log_scale_factor"]))
+        torch.cuda.synchronize()        # the uploads ran on the current stream; run() may use another one
+
+    def run(self, stream=None):
+        """The launch on `stream` (a torch.cuda.Stream; None = the legacy default stream): enqueues, does not wait."""
+        s = None if stream is None else stream.cuda_stream
+        o = {n: t.data_ptr() for n, t in self.outputs.items()}
+        L = _fuse_lib()
+        if self.lines:
+            check(L.pl_lsd_fuse_search_dev(C.byref(self._k), C.byref(self._m), C.byref(self._q), o["best_idx"], o["best_dist"], o["stop_at"],
+                                           o["status"], s))
+        else:
+            check(L.pl_orb_fuse_search_dev(C.byref(self._k), C.byref(self._m), C.byref(self._q), o["best_idx"], o["best_dist"], o["status"], s))
+
+    def results(self):
+        import torch
+        torch.cuda.synchronize()
+        h = {n: t.cpu().numpy() for n, t in self.outputs.items()}
+        q = self.host["q"]
+        res = []
+        for p in range(self.P):
+            a, c = q["out_offset"][p], q["count"][p]
+            r = dict(best_idx=h["best_idx"][a:a + c].copy(), best_dist=h["best_dist"][a:a + c].copy(), status=int(h["status"][p]))
+            if self.lines:
+                r["stop_at"] = int(h["stop_at"][p])
+            res.append(r)
+        return res
+
+
+def _fuse_search_batch(self, keyframes, points, problems, entry_lists, scale_factors, inv_level_sigma2, log_scale_factor, stream=None):
+    """The search half of ORBmatcher::Fuse for many (keyframe, point list) problems in one pl_orb_fuse_search_dev launch.
+    keyframes, points, problems, entry_lists: see FuseProblems.  Returns one dict per problem (best_idx, best_dist, status)."""
+    b = FuseProblems(keyframes, points, problems, entry_lists,
+                     dict(scale_factors=scale_factors, inv_level_sigma2=inv_level_sigma2, log_scale_factor=log_scale_factor))
+    b.run(stream)
+    return b.results()
+
+
+def _lsd_fuse_search_batch(self, keyframes, lines, problems, entry_lists, scale_line, log_scale_factor_line, stream=None):
+    """The search half of LSDmatcher::Fuse for many (keyframe, line list) problems in one pl_lsd_fuse_search_dev launch.
+    Returns one dict per problem (best_idx, best_dist, stop_at, status)."""
+    b = FuseProblems(keyframes, lines, problems, entry_lists, dict(scale_line=scale_line, log_scale_factor_line=log_scale_factor_line),
+                     lines=True)
+    b.run(stream)
+    return b.results()
+
+
+ORBmatcher.FuseSearchBatch = _fuse_search_batch
+LSDmatcher.FuseSearchBatch = _lsd_fuse_search_batch
+
+
 # ---------------------------------------------------------------------------------------------- tracking against a fixed map
 class PLMapDesc(C.Structure):
     _fields_ = [("n_points", C.c_int), ("pt_pos", vp), ("pt_normal", vp), ("pt_min_dist", vp), ("pt_max_dist", vp), ("pt_desc", vp),

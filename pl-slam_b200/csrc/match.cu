@@ -19,6 +19,7 @@
 #include "common.cuh"
 #include "search.cuh"
 #include "libm_glibc.cuh"
+#include <climits>
 #include <vector>
 
 namespace pl {
@@ -798,12 +799,6 @@ __global__ void __launch_bounds__(256) k_search_triangulation(TriArgs A) {
   if (tid == 0) *A.nmatches = s_nm;
 }
 
-struct FuseArgs {
-  const PLKeyPoint* keys; const uint8_t* desc; int n; float bounds[4]; float T[16], Ow[3], K[4];
-  const float *scaleFactors, *invSigma2; float logScaleFactor; int nLevels;
-  int n_mp; const uint8_t* skip; const float *pos, *normal, *minDist, *maxDist; const uint8_t* mp_desc; float th;
-  int *best_idx, *best_dist;
-};
 struct SkipChi2 {
   const PLKeyPoint* k; const float* inv; float u, v;
   __device__ bool operator()(int id, int) const {
@@ -812,56 +807,96 @@ struct SkipChi2 {
     return (double)__fmul_rn(e2, inv[k[id].octave]) > 5.99;
   }
 };
+
+// Status of problem blockIdx.x of a Fuse batch (PLFuseProblems in plslam_b200.h), the same in every thread of the CTA: kf_ok(kf)
+// checks the keyframe's counts against its capacities.
+template <typename KfOk>
+__device__ int fuse_status(const PLFuseProblems& Q, int n_kf, int n_lm, KfOk kf_ok) {
+  const int p = blockIdx.x, kf = Q.kf[p];
+  const long long o = Q.offset[p], c = Q.count[p], oo = Q.out_offset[p];
+  if (kf < 0 || kf >= n_kf || o < 0 || c < 0 || o + c > Q.n_entries || oo < 0 || oo + c > Q.n_out) return 1;
+  if (!kf_ok(kf)) return 2;
+  bool ok = true;
+  for (long long j = threadIdx.x; j < c; j += blockDim.x) { const int m = Q.entry_lm[o + j]; ok = ok && m >= 0 && m < n_lm; }
+  return __syncthreads_and(ok) ? 0 : 3;
+}
+// The camera of problem blockIdx.x's keyframe in shared memory: Tcw, Ow, K, bounds.
+struct FuseCam { float T[16], Ow[3], K[4], bounds[4]; };
+__device__ void load_fuse_cam(FuseCam& c, const float* Tcw, const float* Ow, const float* K, const float* bounds, int kf) {
+  const int t = threadIdx.x;
+  if (t < 16) c.T[t] = Tcw[16LL * kf + t];
+  else if (t < 19) c.Ow[t - 16] = Ow[3LL * kf + t - 16];
+  else if (t < 23) c.K[t - 19] = K[4LL * kf + t - 19];
+  else if (t < 27) c.bounds[t - 23] = bounds[4LL * kf + t - 23];
+}
+
+// ORBmatcher::Fuse, search half: one CTA per problem.  Warp 0 builds the keyframe's bucket grid in shared memory, then the
+// problem's map points run one per warp.
+struct FuseBatch { PLFuseKeyframes K; PLFusePoints L; PLFuseProblems Q; int *best_idx, *best_dist, *status; };
 constexpr int kFuseWarps = 16;
-__global__ void __launch_bounds__(32 * kFuseWarps) k_fuse_search(FuseArgs A) {
+__global__ void __launch_bounds__(32 * kFuseWarps) k_fuse_search(const __grid_constant__ FuseBatch A) {
   extern __shared__ unsigned char smem[];
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  SmemGrid sg = carve_grid(smem, A.n);
-  const GridP g = make_grid(A.bounds);
+  __shared__ FuseCam cam;
   __shared__ int s_packed;
+  const PLFuseKeyframes& K = A.K; const PLFusePoints& L = A.L; const PLFuseProblems& Q = A.Q;
+  const int p = blockIdx.x, lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  const int st = fuse_status(Q, K.n_kf, L.n, [&](int kf) { return K.n[kf] >= 0 && K.n[kf] <= K.cap; });
+  if (threadIdx.x == 0) A.status[p] = st;
+  if (st) return;
+  const int kf = Q.kf[p], n = K.n[kf], cnt = Q.count[p];
+  const long long o = Q.offset[p], oo = Q.out_offset[p], row = (long long)kf * K.cap;
+  const PLKeyPoint* keys = K.keys_un + row;
+  const uint8_t* desc = K.desc + 32 * row;
+  const float th = Q.th[p];
+  load_fuse_cam(cam, K.Tcw, K.Ow, K.K, K.bounds, kf);
+  __syncthreads();
+  SmemGrid sg = carve_grid(smem, K.cap);
+  const GridP g = make_grid(cam.bounds);
   if (wid == 0) {
-    build_point_grid(A.keys, A.n, g, sg.start, sg.fill, sg.items, lane);
-    const bool pk = pack_octaves(A.keys, A.n, sg.start[NCELL], sg.items, lane);
+    build_point_grid(keys, n, g, sg.start, sg.fill, sg.items, lane);
+    const bool pk = pack_octaves(keys, n, sg.start[NCELL], sg.items, lane);
     if (lane == 0) s_packed = pk;
   }
   __syncthreads();
   const bool packed = s_packed != 0;
-  for (int i = wid; i < A.n_mp; i += kFuseWarps) {
+  const float* T = cam.T; const float* Ow = cam.Ow; const float* Kc = cam.K; const float* bounds = cam.bounds;
+  for (int j = wid; j < cnt; j += kFuseWarps) {
+    const long long i = Q.entry_lm[o + j];
     int bi = -1, bd = 256;
-    bool go = !(A.skip && A.skip[i]);
+    bool go = !Q.entry_skip[o + j];
     float u = 0.f, v = 0.f; int lvl = 0;
     if (go) {
-      const float P[3] = {A.pos[3 * i], A.pos[3 * i + 1], A.pos[3 * i + 2]};
+      const float P[3] = {L.pos[3 * i], L.pos[3 * i + 1], L.pos[3 * i + 2]};
       float Pc[3];
       for (int r = 0; r < 3; r++)
-        Pc[r] = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(A.T[4 * r], P[0]), __fmul_rn(A.T[4 * r + 1], P[1])), __fmul_rn(A.T[4 * r + 2], P[2])), A.T[4 * r + 3]);
+        Pc[r] = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(T[4 * r], P[0]), __fmul_rn(T[4 * r + 1], P[1])), __fmul_rn(T[4 * r + 2], P[2])), T[4 * r + 3]);
       go = !(Pc[2] < 0.0f);
       if (go) {
         const float invz = __fdiv_rn(1.0f, Pc[2]);
-        u = __fadd_rn(__fmul_rn(A.K[0], __fmul_rn(Pc[0], invz)), A.K[2]);
-        v = __fadd_rn(__fmul_rn(A.K[1], __fmul_rn(Pc[1], invz)), A.K[3]);
-        go = (u >= A.bounds[0] && u < A.bounds[2] && v >= A.bounds[1] && v < A.bounds[3]);     // KeyFrame::IsInImage
+        u = __fadd_rn(__fmul_rn(Kc[0], __fmul_rn(Pc[0], invz)), Kc[2]);
+        v = __fadd_rn(__fmul_rn(Kc[1], __fmul_rn(Pc[1], invz)), Kc[3]);
+        go = (u >= bounds[0] && u < bounds[2] && v >= bounds[1] && v < bounds[3]);     // KeyFrame::IsInImage
       }
       if (go) {
-        const float PO[3] = {__fsub_rn(P[0], A.Ow[0]), __fsub_rn(P[1], A.Ow[1]), __fsub_rn(P[2], A.Ow[2])};
+        const float PO[3] = {__fsub_rn(P[0], Ow[0]), __fsub_rn(P[1], Ow[1]), __fsub_rn(P[2], Ow[2])};
         const float dist3D = (float)sqrt((double)PO[0] * PO[0] + (double)PO[1] * PO[1] + (double)PO[2] * PO[2]);
-        go = !(dist3D < __fmul_rn(0.8f, A.minDist[i]) || dist3D > __fmul_rn(1.2f, A.maxDist[i]));
+        go = !(dist3D < __fmul_rn(0.8f, L.min_dist[i]) || dist3D > __fmul_rn(1.2f, L.max_dist[i]));
         if (go) {
-          const double dot = (double)PO[0] * A.normal[3 * i] + (double)PO[1] * A.normal[3 * i + 1] + (double)PO[2] * A.normal[3 * i + 2];
+          const double dot = (double)PO[0] * L.normal[3 * i] + (double)PO[1] * L.normal[3 * i + 1] + (double)PO[2] * L.normal[3 * i + 2];
           go = !(dot < 0.5 * (double)dist3D);
-          const float ratio = __fdiv_rn(A.maxDist[i], dist3D);
-          lvl = (int)ceilf(__fdiv_rn(glibc::logf_(ratio), A.logScaleFactor));
-          if (lvl < 0) lvl = 0; else if (lvl >= A.nLevels) lvl = A.nLevels - 1;
+          const float ratio = __fdiv_rn(L.max_dist[i], dist3D);
+          lvl = (int)ceilf(__fdiv_rn(glibc::logf_(ratio), K.log_scale_factor));
+          if (lvl < 0) lvl = 0; else if (lvl >= K.nlevels) lvl = K.nlevels - 1;
         }
       }
     }
     if (go) {     // warp-uniform: every lane computed the same scalars
-      SkipChi2 skip{A.keys, A.invSigma2, u, v};
-      const Top2 t = window_top2(A.keys, A.desc, sg.start, sg.items, g, u, v, __fmul_rn(A.th, A.scaleFactors[lvl]), lvl - 1, lvl,
-                                 A.mp_desc + 32 * (long long)i, skip, lane, packed);
+      SkipChi2 skip{keys, K.inv_level_sigma2, u, v};
+      const Top2 t = window_top2(keys, desc, sg.start, sg.items, g, u, v, __fmul_rn(th, K.scale_factors[lvl]), lvl - 1, lvl,
+                                 L.desc + 32 * i, skip, lane, packed);
       if (t.best != KEY_NONE) { bi = key_idx(t.best); bd = key_dist(t.best); }
     }
-    if (lane == 0) { A.best_idx[i] = bi; A.best_dist[i] = bd; }
+    if (lane == 0) { A.best_idx[oo + j] = bi; A.best_dist[oo + j] = bd; }
   }
 }
 
@@ -973,55 +1008,49 @@ __global__ void __launch_bounds__(32 * kDistWarps) k_distinctive(const uint8_t* 
 }
 
 // ------------------------------------------------------------------------------------------------ LSDmatcher::Fuse, search half
-struct LineFuseArgs {
-  const KeyLine68* kl; int nl; const uint8_t* pdesc; int n_pdesc; float bounds[4]; float T[16], Ow[3], K[4];
-  float scale_line, logScaleFactorLine; int n_ml; const uint8_t* skip; const double *pos, *normal; const float *minDist, *maxDist;
-  const uint8_t* ml_desc; float th; int *best_idx, *best_dist, *stop_at;
-};
-// One thread per map line (the keyframe has <= a few hundred lines; every candidate test is a handful of flops).
-// Quirks of the reference are listed at pl_lsd_fuse_search (plslam_b200.h) and restated in oracle_lsd_fuse_search.
-__global__ void __launch_bounds__(128) k_lsd_fuse_search(LineFuseArgs A) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= A.n_ml) return;
-  A.best_idx[i] = -1; A.best_dist[i] = 256;
-  if (A.skip[i]) return;
-  const float SP[3] = {(float)A.pos[6 * i], (float)A.pos[6 * i + 1], (float)A.pos[6 * i + 2]};
-  const float EP[3] = {(float)A.pos[6 * i + 3], (float)A.pos[6 * i + 4], (float)A.pos[6 * i + 5]};
-  float S[3], E[3];
+// End points of a map line (pos: start, end as doubles) in the world, as the reference's floats, and in the camera.
+__device__ __forceinline__ void line_ends(const float* T, const double* pos, float SP[3], float EP[3], float S[3], float E[3]) {
+#pragma unroll
+  for (int k = 0; k < 3; k++) { SP[k] = (float)pos[k]; EP[k] = (float)pos[3 + k]; }
 #pragma unroll
   for (int r = 0; r < 3; r++) {
-    S[r] = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(A.T[4 * r], SP[0]), __fmul_rn(A.T[4 * r + 1], SP[1])), __fmul_rn(A.T[4 * r + 2], SP[2])), A.T[4 * r + 3]);
-    E[r] = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(A.T[4 * r], EP[0]), __fmul_rn(A.T[4 * r + 1], EP[1])), __fmul_rn(A.T[4 * r + 2], EP[2])), A.T[4 * r + 3]);
+    S[r] = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(T[4 * r], SP[0]), __fmul_rn(T[4 * r + 1], SP[1])), __fmul_rn(T[4 * r + 2], SP[2])), T[4 * r + 3]);
+    E[r] = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(T[4 * r], EP[0]), __fmul_rn(T[4 * r + 1], EP[1])), __fmul_rn(T[4 * r + 2], EP[2])), T[4 * r + 3]);
   }
-  if (S[2] < 0.0f || E[2] < 0.0f) { atomicMin(A.stop_at, i); return; }      // `return false` of the whole call (:907)
+}
+// Best keyline of the keyframe for map line i (in front of the camera); bestIdx / bestDist keep -1 / 256 when nothing qualifies.
+__device__ void line_fuse_one(const FuseCam& cam, const KeyLine68* kls, int nl, const uint8_t* pdesc, int n_pdesc, float scale_line,
+                              float logScaleFactorLine, const PLFuseLines& L, long long i, float th, int& bestIdx, int& bestDist) {
+  const float* Kc = cam.K; const float* bounds = cam.bounds;
+  float SP[3], EP[3], S[3], E[3];
+  line_ends(cam.T, L.pos + 6 * i, SP, EP, S, E);
   const float invz1 = __fdiv_rn(1.0f, S[2]);
-  const float u1 = __fadd_rn(__fmul_rn(__fmul_rn(A.K[0], S[0]), invz1), A.K[2]), v1 = __fadd_rn(__fmul_rn(__fmul_rn(A.K[1], S[1]), invz1), A.K[3]);
-  if (!(u1 >= A.bounds[0] && u1 < A.bounds[2] && v1 >= A.bounds[1] && v1 < A.bounds[3])) return;
+  const float u1 = __fadd_rn(__fmul_rn(__fmul_rn(Kc[0], S[0]), invz1), Kc[2]), v1 = __fadd_rn(__fmul_rn(__fmul_rn(Kc[1], S[1]), invz1), Kc[3]);
+  if (!(u1 >= bounds[0] && u1 < bounds[2] && v1 >= bounds[1] && v1 < bounds[3])) return;
   const float invz2 = __fdiv_rn(1.0f, E[2]);
-  const float u2 = __fadd_rn(__fmul_rn(__fmul_rn(A.K[0], E[0]), invz2), A.K[2]), v2 = __fadd_rn(__fmul_rn(__fmul_rn(A.K[1], E[1]), invz2), A.K[3]);
-  if (!(u2 >= A.bounds[0] && u2 < A.bounds[2] && v2 >= A.bounds[1] && v2 < A.bounds[3])) return;
+  const float u2 = __fadd_rn(__fmul_rn(__fmul_rn(Kc[0], E[0]), invz2), Kc[2]), v2 = __fadd_rn(__fmul_rn(__fmul_rn(Kc[1], E[1]), invz2), Kc[3]);
+  if (!(u2 >= bounds[0] && u2 < bounds[2] && v2 >= bounds[1] && v2 < bounds[3])) return;
   float OM[3];
 #pragma unroll
-  for (int k = 0; k < 3; k++) OM[k] = __fsub_rn((float)(0.5 * (double)__fadd_rn(SP[k], EP[k])), A.Ow[k]);
+  for (int k = 0; k < 3; k++) OM[k] = __fsub_rn((float)(0.5 * (double)__fadd_rn(SP[k], EP[k])), cam.Ow[k]);
   const float dist = (float)sqrt((double)OM[0] * OM[0] + (double)OM[1] * OM[1] + (double)OM[2] * OM[2]);
-  if (dist < __fmul_rn(0.8f, A.minDist[i]) || dist > __fmul_rn(1.2f, A.maxDist[i])) return;
-  const float pn[3] = {(float)A.normal[3 * i], (float)A.normal[3 * i + 1], (float)A.normal[3 * i + 2]};
+  if (dist < __fmul_rn(0.8f, L.min_dist[i]) || dist > __fmul_rn(1.2f, L.max_dist[i])) return;
+  const float pn[3] = {(float)L.normal[3 * i], (float)L.normal[3 * i + 1], (float)L.normal[3 * i + 2]};
   const double dot = (double)OM[0] * pn[0] + (double)OM[1] * pn[1] + (double)OM[2] * pn[2];
   if (dot < 0.5 * (double)dist) return;
-  const float ratio = __fdiv_rn(A.maxDist[i], dist);
-  const int lvl = (int)ceilf(__fdiv_rn(glibc::logf_(ratio), A.logScaleFactorLine));
+  const float ratio = __fdiv_rn(L.max_dist[i], dist);
+  const int lvl = (int)ceilf(__fdiv_rn(glibc::logf_(ratio), logScaleFactorLine));
   float sf = 1.0f;
-  if (lvl >= 0) { for (int k = 0; k < lvl; k++) sf = __fmul_rn(sf, A.scale_line); }
-  else { for (int k = 0; k < -lvl; k++) sf = __fmul_rn(sf, A.scale_line); sf = __fdiv_rn(1.0f, sf); }
-  const float radius = __fmul_rn(A.th, sf), r2 = __fmul_rn(radius, radius);
+  if (lvl >= 0) { for (int k = 0; k < lvl; k++) sf = __fmul_rn(sf, scale_line); }
+  else { for (int k = 0; k < -lvl; k++) sf = __fmul_rn(sf, scale_line); sf = __fdiv_rn(1.0f, sf); }
+  const float radius = __fmul_rn(th, sf), r2 = __fmul_rn(radius, radius);
   float d1x = __fsub_rn(u1, u2), d1y = __fsub_rn(v1, v2);
   const float n1 = __fsqrt_rn(__fadd_rn(__fmul_rn(d1x, d1x), __fmul_rn(d1y, d1y)));
   d1x = __fdiv_rn(d1x, n1); d1y = __fdiv_rn(d1y, n1);
   const double mxd = 0.5 * (double)__fadd_rn(u1, u2), myd = 0.5 * (double)__fadd_rn(v1, v2);
-  int bestDist = 256, bestIdx = -1;
-  const uint8_t* q = A.ml_desc + 32 * (long long)i;
-  for (int j = 0; j < A.nl; j++) {
-    const KeyLine68& kl = A.kl[j];
+  const uint8_t* q = L.desc + 32 * i;
+  for (int j = 0; j < nl; j++) {
+    const KeyLine68& kl = kls[j];
     const double ax = mxd - (double)kl.ptx, ay = myd - (double)kl.pty;
     const float distance = (float)(ax * ax + ay * ay);
     if (distance > r2) continue;
@@ -1031,11 +1060,49 @@ __global__ void __launch_bounds__(128) k_lsd_fuse_search(LineFuseArgs A) {
     const float cs = fabsf(__fadd_rn(__fmul_rn(d1x, d2x), __fmul_rn(d1y, d2y)));
     if (cs < 0.998f) continue;
     if (kl.octave < lvl - 1 || kl.octave > lvl) continue;
-    if (j >= A.n_pdesc) continue;
-    const int d = hamming256(q, A.pdesc + 32 * (long long)j);
+    if (j >= n_pdesc) continue;
+    const int d = hamming256(q, pdesc + 32 * (long long)j);
     if (d < bestDist) { bestDist = d; bestIdx = j; }
   }
-  A.best_idx[i] = bestIdx; A.best_dist[i] = bestDist;
+}
+struct LineFuseBatch { PLFuseLineKeyframes K; PLFuseLines L; PLFuseProblems Q; int *best_idx, *best_dist, *stop_at, *status; };
+// One CTA per problem, one thread per map line (a keyframe has at most a few hundred lines; every candidate test is a handful of
+// flops).  Quirks of the reference are listed at pl_lsd_fuse_search (plslam_b200.h) and restated in oracle_lsd_fuse_search.
+constexpr int kLineFuseThreads = 128;
+__global__ void __launch_bounds__(kLineFuseThreads) k_lsd_fuse_search(const __grid_constant__ LineFuseBatch A) {
+  __shared__ FuseCam cam;
+  __shared__ int s_stop;
+  const PLFuseLineKeyframes& K = A.K; const PLFuseLines& L = A.L; const PLFuseProblems& Q = A.Q;
+  const int p = blockIdx.x, tid = threadIdx.x;
+  const int st = fuse_status(Q, K.n_kf, L.n, [&](int kf) {
+    return K.n[kf] >= 0 && K.n[kf] <= K.cap && K.n_pdesc[kf] >= 0 && K.n_pdesc[kf] <= K.cap_pdesc;
+  });
+  if (tid == 0) A.status[p] = st;
+  if (st) return;
+  const int kf = Q.kf[p], nl = K.n[kf], n_pdesc = K.n_pdesc[kf], cnt = Q.count[p];
+  const long long o = Q.offset[p], oo = Q.out_offset[p];
+  const KeyLine68* kls = reinterpret_cast<const KeyLine68*>(K.keylines) + (long long)kf * K.cap;
+  const uint8_t* pdesc = K.pdesc + 32LL * kf * K.cap_pdesc;
+  const float th = Q.th[p];
+  load_fuse_cam(cam, K.Tcw, K.Ow, K.K, K.bounds, kf);
+  if (tid == 0) s_stop = cnt;
+  __syncthreads();
+  // the first map line with an end point behind the camera ends the reference's loop (`return false`, :907)
+  for (int j = tid; j < cnt; j += kLineFuseThreads) {
+    if (Q.entry_skip[o + j]) continue;
+    float SP[3], EP[3], S[3], E[3];
+    line_ends(cam.T, L.pos + 6LL * Q.entry_lm[o + j], SP, EP, S, E);
+    if (S[2] < 0.0f || E[2] < 0.0f) atomicMin(&s_stop, j);
+  }
+  __syncthreads();
+  const int stop = s_stop;
+  if (tid == 0) A.stop_at[p] = stop;
+  for (int j = tid; j < cnt; j += kLineFuseThreads) {
+    int bestIdx = -1, bestDist = 256;
+    if (j < stop && !Q.entry_skip[o + j])
+      line_fuse_one(cam, kls, nl, pdesc, n_pdesc, K.scale_line, K.log_scale_factor_line, L, Q.entry_lm[o + j], th, bestIdx, bestDist);
+    A.best_idx[oo + j] = bestIdx; A.best_dist[oo + j] = bestDist;
+  }
 }
 
 extern "C" int pl_descriptor_distance_batch(const uint8_t* a, const uint8_t* b, int n, int* out) {
@@ -1468,6 +1535,42 @@ extern "C" int pl_orb_search_for_triangulation(const PLKeyPoint* keys1_un, const
   return nm;
 }
 
+// PL_OK if a Fuse batch's problem table can be read as plslam_b200.h states (PLFuseProblems); the rest is checked on the device.
+static int fuse_problems_ok(const PLFuseProblems* Q, int* best_idx, int* best_dist, int* status) {
+  PL_ARG(Q && Q->P >= 0 && Q->n_entries >= 0 && Q->n_out >= 0);
+  if (Q->P == 0) return PL_OK;
+  PL_ARG(Q->kf && Q->th && Q->offset && Q->count && Q->out_offset && status);
+  PL_ARG(Q->n_entries == 0 || (Q->entry_lm && Q->entry_skip));
+  PL_ARG(Q->n_out == 0 || (best_idx && best_dist));
+  return PL_OK;
+}
+
+static int orb_fuse_launch(const PLFuseKeyframes& K, const PLFusePoints& L, const PLFuseProblems& Q, int* best_idx, int* best_dist,
+                           int* status, void* stream) {
+  const size_t sm = grid_smem_bytes(K.cap);
+  PL_CUDA(cudaFuncSetAttribute(k_fuse_search, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
+  const FuseBatch A{K, L, Q, best_idx, best_dist, status};
+  k_fuse_search<<<Q.P, 32 * kFuseWarps, sm, (cudaStream_t)stream>>>(A);
+  PL_LAUNCH_CHECK();
+  return PL_OK;
+}
+
+extern "C" int pl_orb_fuse_search_dev(const PLFuseKeyframes* kfs, const PLFusePoints* points, const PLFuseProblems* problems, int* best_idx,
+                                      int* best_dist, int* status, void* stream) {
+  PL_TRY(fuse_problems_ok(problems, best_idx, best_dist, status));
+  PL_ARG(points && points->n >= 0);
+  if (problems->P == 0) return PL_OK;
+  PL_ARG(kfs);
+  const PLFuseKeyframes& K = *kfs;
+  const PLFusePoints& L = *points;
+  PL_ARG(K.n_kf >= 1 && K.cap >= 1 && K.cap <= kMatchMaxKeys && (long long)K.n_kf * K.cap <= INT_MAX && K.nlevels >= 1);
+  PL_ARG(K.keys_un && K.desc && K.n && K.Tcw && K.Ow && K.K && K.bounds && K.scale_factors && K.inv_level_sigma2);
+  PL_ARG(L.n == 0 || (L.pos && L.normal && L.min_dist && L.max_dist && L.desc));
+  PL_TRY(require_device());
+  return orb_fuse_launch(K, L, *problems, best_idx, best_dist, status, stream);
+}
+
+// The P = 1 case of pl_orb_fuse_search_dev: one keyframe of capacity n, entry i = map point i.
 extern "C" int pl_orb_fuse_search(const PLKeyPoint* keys_un, const uint8_t* desc, int n, const float* bounds, const float* Tcw,
                                   const float* Ow, const float* K, const float* scale_factors, const float* inv_level_sigma2,
                                   int nlevels, float log_scale_factor, int n_mp, const uint8_t* skip, const float* pos,
@@ -1478,20 +1581,21 @@ extern "C" int pl_orb_fuse_search(const PLKeyPoint* keys_un, const uint8_t* desc
   PL_ARG(n_mp == 0 || (pos && normal && min_dist && max_dist && mp_desc));
   int rc = require_device(); if (rc) return rc;
   if (n_mp == 0) return PL_OK;
+  float cam[28];        // Tcw, Ow, K, bounds, th: one upload
+  memcpy(cam, Tcw, 64); memcpy(cam + 16, Ow, 12); memcpy(cam + 19, K, 16); memcpy(cam + 23, bounds, 16); cam[27] = th;
+  const int ints[5] = {n, 0, 0, n_mp, 0};     // keypoint count; kf, offset, count, out_offset of the one problem
+  std::vector<int> lm(n_mp);
+  for (int i = 0; i < n_mp; i++) lm[i] = i;
   Staging s;
-  FuseArgs A;
-  A.keys = s.in(keys_un, n); A.desc = s.in(desc, (size_t)n * 32); A.n = n;
-  memcpy(A.bounds, bounds, 16); memcpy(A.T, Tcw, 64); memcpy(A.Ow, Ow, 12); memcpy(A.K, K, 16);
-  A.scaleFactors = s.in(scale_factors, nlevels); A.invSigma2 = s.in(inv_level_sigma2, nlevels);
-  A.logScaleFactor = log_scale_factor; A.nLevels = nlevels; A.n_mp = n_mp;
-  A.skip = skip ? s.in(skip, n_mp) : nullptr; A.pos = s.in(pos, (size_t)n_mp * 3); A.normal = s.in(normal, (size_t)n_mp * 3);
-  A.minDist = s.in(min_dist, n_mp); A.maxDist = s.in(max_dist, n_mp); A.mp_desc = s.in(mp_desc, (size_t)n_mp * 32); A.th = th;
-  A.best_idx = s.out(best_idx, n_mp); A.best_dist = s.out(best_dist, n_mp);
+  const float* dc = s.in(cam, 28); const int* di = s.in(ints, 5);
+  const PLFuseKeyframes Kt{1, std::max(n, 1), s.in(keys_un, n), s.in(desc, (size_t)n * 32), di, dc, dc + 16, dc + 19, dc + 23,
+                           s.in(scale_factors, nlevels), s.in(inv_level_sigma2, nlevels), nlevels, log_scale_factor};
+  const PLFusePoints L{n_mp, s.in(pos, (size_t)n_mp * 3), s.in(normal, (size_t)n_mp * 3), s.in(min_dist, n_mp), s.in(max_dist, n_mp),
+                       s.in(mp_desc, (size_t)n_mp * 32)};
+  const PLFuseProblems Q{1, di + 1, dc + 27, di + 2, di + 3, di + 4, n_mp, s.in(lm.data(), n_mp), skip ? s.in(skip, n_mp) : s.out<uint8_t>(n_mp), n_mp};
+  int* dbi = s.out(best_idx, n_mp); int* dbd = s.out(best_dist, n_mp); int* dst = s.out<int>(1);
   if ((rc = s.status())) return rc;
-  const size_t sm = grid_smem_bytes(std::max(n, 1));
-  PL_CUDA(cudaFuncSetAttribute(k_fuse_search, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
-  k_fuse_search<<<1, 32 * kFuseWarps, sm>>>(A);
-  PL_LAUNCH_CHECK();
+  PL_TRY(orb_fuse_launch(Kt, L, Q, dbi, dbd, dst, nullptr));
   return s.fetch();
 }
 
@@ -1603,6 +1707,31 @@ extern "C" int pl_mappoint_distinctive_descriptors(const uint8_t* desc, const in
   return s.fetch();
 }
 
+static int lsd_fuse_launch(const PLFuseLineKeyframes& K, const PLFuseLines& L, const PLFuseProblems& Q, int* best_idx, int* best_dist,
+                           int* stop_at, int* status, void* stream) {
+  const LineFuseBatch A{K, L, Q, best_idx, best_dist, stop_at, status};
+  k_lsd_fuse_search<<<Q.P, kLineFuseThreads, 0, (cudaStream_t)stream>>>(A);
+  PL_LAUNCH_CHECK();
+  return PL_OK;
+}
+
+extern "C" int pl_lsd_fuse_search_dev(const PLFuseLineKeyframes* kfs, const PLFuseLines* lines, const PLFuseProblems* problems, int* best_idx,
+                                      int* best_dist, int* stop_at, int* status, void* stream) {
+  PL_TRY(fuse_problems_ok(problems, best_idx, best_dist, status));
+  PL_ARG(lines && lines->n >= 0);
+  if (problems->P == 0) return PL_OK;
+  PL_ARG(kfs);
+  const PLFuseLineKeyframes& K = *kfs;
+  const PLFuseLines& L = *lines;
+  PL_ARG(stop_at && K.n_kf >= 1 && K.cap >= 1 && K.cap <= 32768 && K.cap_pdesc >= 1 && K.cap_pdesc <= 32768);
+  PL_ARG((long long)K.n_kf * K.cap <= INT_MAX && (long long)K.n_kf * K.cap_pdesc <= INT_MAX);
+  PL_ARG(K.keylines && K.n && K.pdesc && K.n_pdesc && K.Tcw && K.Ow && K.K && K.bounds);
+  PL_ARG(L.n == 0 || (L.pos && L.normal && L.min_dist && L.max_dist && L.desc));
+  PL_TRY(require_device());
+  return lsd_fuse_launch(K, L, *problems, best_idx, best_dist, stop_at, status, stream);
+}
+
+// The P = 1 case of pl_lsd_fuse_search_dev: one keyframe, entry i = map line i.
 extern "C" int pl_lsd_fuse_search(const void* keylines, int nl, const uint8_t* kf_point_desc, int n_pdesc, const float* bounds, const float* Tcw,
                                   const float* Ow, const float* K, float scale_line, float log_scale_factor_line, int n_ml,
                                   const uint8_t* skip, const double* pos, const double* normal, const float* min_dist, const float* max_dist,
@@ -1612,19 +1741,20 @@ extern "C" int pl_lsd_fuse_search(const void* keylines, int nl, const uint8_t* k
   int rc = require_device(); if (rc) return rc;
   *stop_at = n_ml;
   if (n_ml == 0) return PL_OK;
+  float cam[28];        // Tcw, Ow, K, bounds, th: one upload
+  memcpy(cam, Tcw, 64); memcpy(cam + 16, Ow, 12); memcpy(cam + 19, K, 16); memcpy(cam + 23, bounds, 16); cam[27] = th;
+  const int ints[6] = {nl, n_pdesc, 0, 0, n_ml, 0};     // line and descriptor counts; kf, offset, count, out_offset of the one problem
+  std::vector<int> lm(n_ml);
+  for (int i = 0; i < n_ml; i++) lm[i] = i;
   Staging s;
-  LineFuseArgs A;
-  A.kl = reinterpret_cast<const KeyLine68*>(s.in(static_cast<const uint8_t*>(keylines), (size_t)nl * 68)); A.nl = nl;
-  A.pdesc = s.in(kf_point_desc, (size_t)n_pdesc * 32); A.n_pdesc = n_pdesc;
-  memcpy(A.bounds, bounds, 16); memcpy(A.T, Tcw, 64); memcpy(A.Ow, Ow, 12); memcpy(A.K, K, 16);
-  A.scale_line = scale_line; A.logScaleFactorLine = log_scale_factor_line; A.n_ml = n_ml;
-  A.skip = s.in(skip, n_ml); A.pos = s.in(pos, (size_t)n_ml * 6); A.normal = s.in(normal, (size_t)n_ml * 3);
-  A.minDist = s.in(min_dist, n_ml); A.maxDist = s.in(max_dist, n_ml); A.ml_desc = s.in(ml_desc, (size_t)n_ml * 32); A.th = th;
-  A.best_idx = s.out(best_idx, n_ml); A.best_dist = s.out(best_dist, n_ml); A.stop_at = s.in(stop_at, 1);
+  const float* dc = s.in(cam, 28); const int* di = s.in(ints, 6);
+  const PLFuseLineKeyframes Kt{1, std::max(nl, 1), std::max(n_pdesc, 1), s.in(static_cast<const uint8_t*>(keylines), (size_t)nl * 68), di,
+                               s.in(kf_point_desc, (size_t)n_pdesc * 32), di + 1, dc, dc + 16, dc + 19, dc + 23, scale_line, log_scale_factor_line};
+  const PLFuseLines L{n_ml, s.in(pos, (size_t)n_ml * 6), s.in(normal, (size_t)n_ml * 3), s.in(min_dist, n_ml), s.in(max_dist, n_ml),
+                      s.in(ml_desc, (size_t)n_ml * 32)};
+  const PLFuseProblems Q{1, di + 2, dc + 27, di + 3, di + 4, di + 5, n_ml, s.in(lm.data(), n_ml), s.in(skip, n_ml), n_ml};
+  int* dbi = s.out(best_idx, n_ml); int* dbd = s.out(best_dist, n_ml); int* dstop = s.out(stop_at, 1); int* dst = s.out<int>(1);
   if ((rc = s.status())) return rc;
-  k_lsd_fuse_search<<<(n_ml + 127) / 128, 128>>>(A);
-  PL_LAUNCH_CHECK();
-  if ((rc = s.fetch()) || (rc = s.down(stop_at, A.stop_at, 1))) return rc;
-  for (int i = *stop_at; i < n_ml; i++) { best_idx[i] = -1; best_dist[i] = 256; }     // never reached by the reference's loop
-  return PL_OK;
+  PL_TRY(lsd_fuse_launch(Kt, L, Q, dbi, dbd, dstop, dst, nullptr));
+  return s.fetch();
 }
