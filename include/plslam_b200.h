@@ -181,7 +181,11 @@ typedef struct PLLineConfig {
   int nfeatures;            /* LINEextractor.nFeatures (nLSDFeature); the reference keeps up to nfeatures+1 lines */
   double min_line_length;   /* LINEextractor.min_line_length                                                    */
   int max_batch;
-  int segment_cap;          /* max LSD segments per frame before truncation; 0 = default 8192                     */
+  int segment_cap;          /* max LSD segments per frame before truncation; 0 = default 8192.  k_keylines sorts
+                               pow2(segment_cap) 8-byte keys in one block's shared memory, so the largest cap is the
+                               device's opt-in shared memory per block over 8, rounded down to a power of two (16384
+                               on H100); a larger or a negative cap is refused with PL_ERR_ARG.  A textured 1920x1080
+                               frame can exceed the default 8192 and then needs an explicit cap up to 16384.       */
   int lsd_used_in_global;   /* region-growing USED map: <0 shared memory, >0 global memory, 0 = global unless env PLSLAM_LSD_USED_GLOBAL=0 */
 } PLLineConfig;
 typedef struct PLLine PLLine;

@@ -754,8 +754,25 @@ extern "C" void pl_line_destroy(PLLine* h) {
 extern "C" int pl_line_create(const PLLineConfig* cfg, PLLine** out) {
   PL_ARG(cfg && out);
   PL_ARG(cfg->width >= 64 && cfg->height >= 64 && cfg->width < 8000 && cfg->height < 8000 && cfg->nfeatures > 0 && cfg->max_batch >= 1);
+  PL_ARG(cfg->segment_cap >= 0);
   int rc = require_device();
   if (rc) return rc;
+  {  // k_keylines sorts a frame's segments in shared memory: 8 B per key, segment_cap rounded up to a power of two
+    int dev = 0, optin = 0;
+    cudaFuncAttributes fa;
+    PL_CUDA(cudaGetDevice(&dev));
+    PL_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+    PL_CUDA(cudaFuncGetAttributes(&fa, k_keylines));
+    const size_t room = optin > (int)fa.sharedSizeBytes ? (size_t)optin - fa.sharedSizeBytes : 0;
+    size_t c2 = 1, fit = 1;
+    while (c2 < (size_t)(cfg->segment_cap > 0 ? cfg->segment_cap : 8192)) c2 <<= 1;
+    while (fit * 2 * 8 <= room) fit <<= 1;
+    if (c2 * 8 > room) {
+      set_error("segment_cap=%d: k_keylines sorts %zu keys of 8 B in shared memory, over the %zu B the device gives it per block; "
+                "at most segment_cap=%zu fits", cfg->segment_cap, c2, room, fit);
+      return PL_ERR_ARG;
+    }
+  }
   std::unique_ptr<PLLine> h(new PLLine);
   h->cfg = *cfg;
   LineParams& P = h->P;
