@@ -466,7 +466,8 @@ int pl_frame_is_in_frustum_lines(const float* Tcw, const float* Ow, const float*
  * keys*_un = mvKeysUn, has_mp* = GetMapPoint(i) != NULL, fv* = DBoW2 FeatureVector as CSR (node ids ascending as in std::map,
  * fv_start[nn+1], fv_items = feature indices in insertion order), F12 row-major 3x3, Cw1 = pKF1->GetCameraCenter(),
  * R2w/t2w = pKF2 rotation (row-major 3x3) / translation, K2 = {fx,fy,cx,cy}, scale_factors2 = mvScaleFactors,
- * level_sigma2_2 = mvLevelSigma2.  matches12[i] = idx2 or -1 (vMatchedPairs = the pairs with idx2 >= 0); returns nmatches. */
+ * level_sigma2_2 = mvLevelSigma2.  matches12[i] = idx2 or -1 (vMatchedPairs = the pairs with idx2 >= 0); returns nmatches.
+ * PL_ERR_ARG for a feature vector whose fv_start is not monotone or runs past n, or with an item outside 0 .. n - 1. */
 int pl_orb_search_for_triangulation(const PLKeyPoint* keys1_un, const uint8_t* desc1, const uint8_t* has_mp1, int n1,
                                     const PLKeyPoint* keys2_un, const uint8_t* desc2, const uint8_t* has_mp2, int n2,
                                     const unsigned* fv1_nodes, const int* fv1_start, const int* fv1_items, int nn1,
@@ -588,6 +589,54 @@ int pl_orb_fuse_search_dev(const PLFuseKeyframes* kfs, const PLFusePoints* point
                            int* best_dist, int* status, void* stream);
 int pl_lsd_fuse_search_dev(const PLFuseLineKeyframes* kfs, const PLFuseLines* lines, const PLFuseProblems* problems, int* best_idx,
                            int* best_dist, int* stop_at, int* status, void* stream);
+
+/* ------------------------------------------------------------------ many triangulation searches in one launch
+ * (LocalMapping::CreateNewMapPoints and CreateNewMapLinesConstraint)
+ * pl_orb_search_for_triangulation / pl_lsd_search_for_triangulation for P (KF1, KF2) problems at once, on device pointers, enqueued
+ * on `stream` (NULL = the legacy default stream): kernels only, no allocation, copy or synchronisation, so the calls can be
+ * captured into a CUDA graph.  The host-pointer functions above are their P = 1 case.
+ *
+ * Problem p searches keyframe kf1[p] against keyframe kf2[p] and writes match [out_offset[p] + i] for i < n[kf1[p]] (idx2 or -1),
+ * nmatches[p] and status[p].  F12 [P][9] is row-major (LocalMapping::ComputeF12(KF1, KF2)); the line call ignores it (it may be
+ * NULL).  Problems may share keyframes; their output ranges must not overlap. */
+typedef struct PLTriProblems {
+  int P;
+  const int* kf1; const int* kf2; const float* F12; const int* out_offset;   /* [P], F12 [P][9] */
+  int n_out;                                                                 /* length of the match output */
+} PLTriProblems;
+/* Point keyframes: rows of capacity cap, keys_un [n_kf][cap] (mvKeysUn), desc [n_kf][cap][32], has_mp [n_kf][cap]
+ * (GetMapPoint(i) != NULL at the snapshot), n [n_kf]; mFeatVec as CSR per keyframe: fv_nodes [n_kf][cap_nodes] (ascending and
+ * unique, as std::map keeps them), fv_start [n_kf][cap_nodes + 1], fv_items [n_kf][cap], nn [n_kf] nodes; the camera Tcw [n_kf][16]
+ * (row-major; R2w and t2w of a KF2), Ow [n_kf][3] (GetCameraCenter() as stored; Cw of a KF1), K [n_kf][4] (fx fy cx cy of a KF2);
+ * scale_factors / level_sigma2 [nlevels] (mvScaleFactors, mvLevelSigma2) shared by every keyframe. */
+typedef struct PLTriKeyframes {
+  int n_kf, cap, cap_nodes;
+  const PLKeyPoint* keys_un; const uint8_t* desc; const uint8_t* has_mp; const int* n;
+  const unsigned* fv_nodes; const int* fv_start; const int* fv_items; const int* nn;
+  const float* Tcw; const float* Ow; const float* K;
+  const float* scale_factors; const float* level_sigma2; int nlevels;
+} PLTriKeyframes;
+/* Line keyframes: ldesc [n_kf][cap][32] (mLineDescriptors), has_ml [n_kf][cap] (GetMapLine(i) != NULL), n [n_kf]. */
+typedef struct PLTriLineKeyframes {
+  int n_kf, cap;
+  const uint8_t* ldesc; const uint8_t* has_ml; const int* n;
+} PLTriLineKeyframes;
+/* status[p] = 0: problem p ran; 1: kf1[p] or kf2[p] lies outside the table, or its output range [out_offset[p], out_offset[p] +
+ * n[kf1[p]]) lies outside n_out; 2: a keyframe's n or nn is negative or over its capacity, or its fv_start is not monotone, starts
+ * below 0 or runs past n; 3: an fv_items entry of a keyframe lies outside 0 .. n - 1.  A problem with a nonzero status writes
+ * nothing but status[p].
+ * check_orientation = 1 keeps the rotation histogram per problem.  LocalMapping::CreateNewMapPoints uses 0, and only then are the
+ * keypoints of KF1 independent of each other, so that a caller may search every neighbour against one snapshot of has_mp and
+ * drop, at application, the pairs whose idx1 received a map point at an earlier neighbour (INTEGRATION.md, CreateNewMapPoints).
+ * PL_ERR_ARG before anything is enqueued for a NULL problem list, P < 0 or n_out < 0; and, when P > 0, for a NULL table, array
+ * or output (F12 may be NULL for lines), n_kf < 1, nlevels < 1, cap outside 1 .. 6144 (points) or beyond what pl_lsd_search_double_dev takes (lines: below
+ * 32000 and inside the device's shared memory), cap_nodes < 1, or n_kf * cap (n_kf * (cap_nodes + 1)) beyond an int.  P = 0
+ * enqueues nothing.  Each problem equals pl_orb_search_for_triangulation / pl_lsd_search_for_triangulation on its two keyframes,
+ * bit for bit. */
+int pl_orb_search_for_triangulation_dev(const PLTriKeyframes* kfs, const PLTriProblems* problems, int check_orientation,
+                                        int* matches12, int* nmatches, int* status, void* stream);
+int pl_lsd_search_for_triangulation_dev(const PLTriLineKeyframes* kfs, const PLTriProblems* problems, float th, float nnratio,
+                                        int is_double, int* matched_pairs, int* nmatches, int* status, void* stream);
 
 /* ------------------------------------------------------------------ tracking a batch of frames against a fixed map
  * Tracking::TrackLocalMapWithLines (src/Tracking.cc:1491-1562) with SearchLocalPoints (:1751-1801) and SearchLocalLines

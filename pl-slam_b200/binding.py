@@ -1030,6 +1030,33 @@ def _lsd_fuse_search(self, keylines, kf_point_desc, bounds, Tcw, Ow, K, scale_li
 LSDmatcher.FuseSearch = _lsd_fuse_search
 
 
+# ---------------------------------------------------------------------------------------------- keyframe tables of the batched searches
+def _pad_rows(arrays, dt, shape, cap, what):
+    """Per-keyframe arrays -> ([n_kf][cap] + shape array of dtype dt, zero past each count; counts [n_kf]; cap).  cap defaults to
+    the largest count (at least 1)."""
+    counts = np.array([len(a) for a in arrays], np.int32)
+    cap = max([1] + list(counts)) if cap is None else int(cap)
+    if counts.size and counts.max() > cap:
+        raise ValueError(f"a keyframe has {counts.max()} {what}, over the capacity {cap}")
+    out = np.zeros((len(arrays), cap) + shape, dt)
+    for i, a in enumerate(arrays):
+        out[i, :counts[i]] = np.asarray(a, dt).reshape((-1,) + shape)
+    return out, counts, cap
+
+
+def _camera_rows(keyframes, **widths):
+    """Per-keyframe camera fields -> float32 [n_kf][width] arrays, one per field name."""
+    n_kf = len(keyframes)
+    return {name: np.array([np.asarray(k[name], np.float32).reshape(w) for k in keyframes], np.float32).reshape(n_kf, w)
+            for name, w in widths.items()}
+
+
+def _to_device(a):
+    """A host array (structured arrays as raw bytes) as a torch CUDA tensor."""
+    import torch
+    return torch.from_numpy(np.ascontiguousarray(a).view(np.uint8) if a.dtype.names else np.ascontiguousarray(a)).cuda()
+
+
 # ---------------------------------------------------------------------------------------------- many Fuse searches in one launch
 class PLFuseProblems(C.Structure):
     _fields_ = [("P", C.c_int), ("kf", vp), ("th", vp), ("offset", vp), ("count", vp), ("out_offset", vp),
@@ -1063,22 +1090,8 @@ def pack_fuse_keyframes(keyframes, lines=False, cap=None, cap_pdesc=None):
     """Keyframes (dicts: keys [n] KP_DTYPE and desc [n][32] for points, kl [n] KEYLINE_DTYPE and pdesc [m][32] for lines; Tcw [16],
     Ow [3], K [4], bounds [4]) -> host arrays in the [n_kf][cap] layouts of PLFuseKeyframes / PLFuseLineKeyframes.  cap /
     cap_pdesc default to the largest count (at least 1); rows past a keyframe's count are zero."""
-    n_kf = len(keyframes)
-    cam = dict(Tcw=np.array([np.asarray(k["Tcw"], np.float32).reshape(16) for k in keyframes], np.float32).reshape(n_kf, 16),
-               Ow=np.array([np.asarray(k["Ow"], np.float32).reshape(3) for k in keyframes], np.float32).reshape(n_kf, 3),
-               K=np.array([np.asarray(k["K"], np.float32).reshape(4) for k in keyframes], np.float32).reshape(n_kf, 4),
-               bounds=np.array([np.asarray(k["bounds"], np.float32).reshape(4) for k in keyframes], np.float32).reshape(n_kf, 4))
-
-    def rows(name, dt, shape, c):
-        counts = np.array([len(k[name]) for k in keyframes], np.int32)
-        c = max([1] + list(counts)) if c is None else int(c)
-        if counts.size and counts.max() > c:
-            raise ValueError(f"a keyframe has {counts.max()} {name}, over the capacity {c}")
-        a = np.zeros((n_kf, c) + shape, dt)
-        for i, k in enumerate(keyframes):
-            a[i, :counts[i]] = np.asarray(k[name], dt).reshape((-1,) + shape)
-        return a, counts, c
-
+    cam = _camera_rows(keyframes, Tcw=16, Ow=3, K=4, bounds=4)
+    rows = lambda name, dt, shape, c: _pad_rows([k[name] for k in keyframes], dt, shape, c, name)
     if lines:
         kl, n, cap = rows("kl", KEYLINE_DTYPE, (), cap)
         pdesc, n_pdesc, cap_pdesc = rows("pdesc", np.uint8, (32,), cap_pdesc)
@@ -1132,7 +1145,7 @@ class FuseProblems:
         k = pack_fuse_keyframes(keyframes, lines)
         q = pack_fuse_problems(problems, entry_lists)
         m = pack_fuse_landmarks(landmarks, lines)
-        dev = lambda a: torch.from_numpy(np.ascontiguousarray(a).view(np.uint8) if a.dtype.names else np.ascontiguousarray(a)).cuda()
+        dev = _to_device
         self.host = dict(k=k, q=q, m=m)
         self.inputs = {f"k_{n}": dev(v) for n, v in k.items() if isinstance(v, np.ndarray)}
         self.inputs.update({f"q_{n}": dev(v) for n, v in q.items() if isinstance(v, np.ndarray)})
@@ -1205,6 +1218,140 @@ def _lsd_fuse_search_batch(self, keyframes, lines, problems, entry_lists, scale_
 
 ORBmatcher.FuseSearchBatch = _fuse_search_batch
 LSDmatcher.FuseSearchBatch = _lsd_fuse_search_batch
+
+
+# ---------------------------------------------------------------------------------------------- many triangulation searches in one launch
+class PLTriProblems(C.Structure):
+    _fields_ = [("P", C.c_int), ("kf1", vp), ("kf2", vp), ("F12", vp), ("out_offset", vp), ("n_out", C.c_int)]
+
+
+class PLTriKeyframes(C.Structure):
+    _fields_ = [("n_kf", C.c_int), ("cap", C.c_int), ("cap_nodes", C.c_int), ("keys_un", vp), ("desc", vp), ("has_mp", vp), ("n", vp),
+                ("fv_nodes", vp), ("fv_start", vp), ("fv_items", vp), ("nn", vp), ("Tcw", vp), ("Ow", vp), ("K", vp),
+                ("scale_factors", vp), ("level_sigma2", vp), ("nlevels", C.c_int)]
+
+
+class PLTriLineKeyframes(C.Structure):
+    _fields_ = [("n_kf", C.c_int), ("cap", C.c_int), ("ldesc", vp), ("has_ml", vp), ("n", vp)]
+
+
+def _tri_lib():
+    L = lib()
+    if not getattr(L, "_tri_types", False):
+        L.pl_orb_search_for_triangulation_dev.argtypes = [C.POINTER(PLTriKeyframes), C.POINTER(PLTriProblems), C.c_int] + [vp] * 4
+        L.pl_lsd_search_for_triangulation_dev.argtypes = ([C.POINTER(PLTriLineKeyframes), C.POINTER(PLTriProblems), C.c_float, C.c_float,
+                                                            C.c_int] + [vp] * 4)
+        L._tri_types = True
+    return L
+
+
+def pack_tri_keyframes(keyframes, lines=False, cap=None, cap_nodes=None):
+    """Keyframes (dicts: keys [n] KP_DTYPE, desc [n][32], has_mp [n], fv (DBoW2 FeatureVector: dict node -> feature indices), Tcw
+    [16], Ow [3], K [4] for points; ldesc [n][32], has_ml [n] for lines) -> host arrays in the [n_kf][cap] layouts of PLTriKeyframes /
+    PLTriLineKeyframes.  cap / cap_nodes default to the largest count (at least 1); rows past a keyframe's count are zero."""
+    if lines:
+        ldesc, n, cap = _pad_rows([k["ldesc"] for k in keyframes], np.uint8, (32,), cap, "keylines")
+        has_ml, _, _ = _pad_rows([k["has_ml"] for k in keyframes], np.uint8, (), cap, "keylines")
+        return dict(ldesc=ldesc, has_ml=has_ml, n=n, cap=cap)
+    keys, n, cap = _pad_rows([k["keys"] for k in keyframes], KP_DTYPE, (), cap, "keypoints")
+    desc, _, _ = _pad_rows([k["desc"] for k in keyframes], np.uint8, (32,), cap, "keypoints")
+    has_mp, _, _ = _pad_rows([k["has_mp"] for k in keyframes], np.uint8, (), cap, "keypoints")
+    csr = [_fv_csr(k["fv"]) for k in keyframes]
+    nodes, nn, cap_nodes = _pad_rows([c[0] for c in csr], np.uint32, (), cap_nodes, "feature-vector nodes")
+    start, _, _ = _pad_rows([c[1] for c in csr], np.int32, (), cap_nodes + 1, "feature-vector nodes")
+    items, _, _ = _pad_rows([c[2] for c in csr], np.int32, (), cap, "feature-vector items")
+    return dict(_camera_rows(keyframes, Tcw=16, Ow=3, K=4), keys_un=keys, desc=desc, has_mp=has_mp, n=n, fv_nodes=nodes, fv_start=start,
+                fv_items=items, nn=nn, cap=cap, cap_nodes=cap_nodes)
+
+
+def pack_tri_problems(problems, counts):
+    """Problems (kf1, kf2) or (kf1, kf2, F12 [3][3]) -> host arrays of PLTriProblems; counts [n_kf] = the keyframes' n.  The output
+    of problem p (n[kf1] entries) follows that of problem p - 1; a problem whose kf1 lies outside the table gets no output range."""
+    P = len(problems)
+    kf1 = np.array([int(p[0]) for p in problems], np.int32)
+    kf2 = np.array([int(p[1]) for p in problems], np.int32)
+    F12 = np.array([np.asarray(p[2], np.float32).reshape(9) if len(p) > 2 else np.zeros(9, np.float32) for p in problems],
+                   np.float32).reshape(P, 9)
+    n = np.array([counts[k] if 0 <= k < len(counts) else 0 for k in kf1], np.int32)
+    out_offset = np.concatenate([[0], np.cumsum(n)[:-1]]).astype(np.int32) if P else np.zeros(0, np.int32)
+    return dict(P=P, kf1=kf1, kf2=kf2, F12=F12, out_offset=out_offset, n_out=int(n.sum()), count=n)
+
+
+class TriangulationProblems:
+    """A batch of triangulation searches on the device for pl_orb_search_for_triangulation_dev (lines=False) or
+    pl_lsd_search_for_triangulation_dev (lines=True): the constructor packs the keyframe table and the problems (pack_tri_keyframes,
+    pack_tri_problems) into torch CUDA tensors and allocates the outputs once; run() only enqueues the launch, so it can be captured
+    into a CUDA graph; results() waits for it and returns one dict per problem: matches (numpy [n[kf1]]: idx2 or -1), nmatches and
+    status.  Points: scales = (scale_factors, level_sigma2), options = check_orientation; lines: options = (th, nnratio, is_double).
+    Outputs are pre-filled with `out_fill`."""
+
+    def __init__(self, keyframes, problems, scales=None, lines=False, options=0, out_fill=-7):
+        import torch
+        self.lines, self.options = lines, options
+        k = pack_tri_keyframes(keyframes, lines)
+        q = pack_tri_problems(problems, k["n"])
+        self.host = dict(k=k, q=q)
+        self.inputs = {f"k_{n}": _to_device(v) for n, v in k.items() if isinstance(v, np.ndarray)}
+        self.inputs.update({f"q_{n}": _to_device(v) for n, v in q.items() if isinstance(v, np.ndarray)})
+        if not lines:
+            self.inputs["scale_factors"] = _to_device(np.asarray(scales[0], np.float32))
+            self.inputs["level_sigma2"] = _to_device(np.asarray(scales[1], np.float32))
+        self.P = q["P"]
+        self.outputs = dict(matches=torch.full((max(q["n_out"], 1),), out_fill, dtype=torch.int32, device="cuda"),
+                            nmatches=torch.full((max(self.P, 1),), out_fill, dtype=torch.int32, device="cuda"),
+                            status=torch.full((max(self.P, 1),), out_fill, dtype=torch.int32, device="cuda"))
+        i = lambda n: self.inputs[n].data_ptr()
+        self._q = PLTriProblems(self.P, i("q_kf1"), i("q_kf2"), None if lines else i("q_F12"), i("q_out_offset"), q["n_out"])
+        n_kf = len(keyframes)
+        if lines:
+            self._k = PLTriLineKeyframes(n_kf, k["cap"], i("k_ldesc"), i("k_has_ml"), i("k_n"))
+        else:
+            self._k = PLTriKeyframes(n_kf, k["cap"], k["cap_nodes"], i("k_keys_un"), i("k_desc"), i("k_has_mp"), i("k_n"), i("k_fv_nodes"),
+                                     i("k_fv_start"), i("k_fv_items"), i("k_nn"), i("k_Tcw"), i("k_Ow"), i("k_K"), i("scale_factors"),
+                                     i("level_sigma2"), len(scales[0]))
+        torch.cuda.synchronize()        # the uploads ran on the current stream; run() may use another one
+
+    def run(self, stream=None):
+        """The launch on `stream` (a torch.cuda.Stream; None = the legacy default stream): enqueues, does not wait."""
+        s = None if stream is None else stream.cuda_stream
+        o = {n: t.data_ptr() for n, t in self.outputs.items()}
+        L = _tri_lib()
+        if self.lines:
+            th, nnratio, is_double = self.options
+            check(L.pl_lsd_search_for_triangulation_dev(C.byref(self._k), C.byref(self._q), th, nnratio, int(is_double), o["matches"],
+                                                        o["nmatches"], o["status"], s))
+        else:
+            check(L.pl_orb_search_for_triangulation_dev(C.byref(self._k), C.byref(self._q), int(self.options), o["matches"],
+                                                        o["nmatches"], o["status"], s))
+
+    def results(self):
+        import torch
+        torch.cuda.synchronize()
+        h = {n: t.cpu().numpy() for n, t in self.outputs.items()}
+        q = self.host["q"]
+        return [dict(matches=h["matches"][q["out_offset"][p]:q["out_offset"][p] + q["count"][p]].copy(),
+                     nmatches=int(h["nmatches"][p]), status=int(h["status"][p])) for p in range(self.P)]
+
+
+def _search_for_triangulation_batch(self, keyframes, problems, scale_factors, level_sigma2, stream=None):
+    """ORBmatcher::SearchForTriangulation for many (KF1, KF2, F12) problems in one pl_orb_search_for_triangulation_dev launch.
+    keyframes, problems: see TriangulationProblems.  Returns one dict per problem (matches, nmatches, status)."""
+    b = TriangulationProblems(keyframes, problems, (scale_factors, level_sigma2), options=int(self.mbCheckOrientation))
+    b.run(stream)
+    return b.results()
+
+
+def _lsd_search_for_triangulation_batch(self, keyframes, problems, isDouble=True, th=None, stream=None):
+    """LSDmatcher::SearchForTriangulation for many (KF1, KF2) problems in one pl_lsd_search_for_triangulation_dev launch; th defaults
+    to TH_HIGH as in SearchForTriangulation.  Returns one dict per problem (matches, nmatches, status)."""
+    b = TriangulationProblems(keyframes, problems, lines=True,
+                              options=(float(self.TH_HIGH if th is None else th), float(self.mfNNratio), bool(isDouble)))
+    b.run(stream)
+    return b.results()
+
+
+ORBmatcher.SearchForTriangulationBatch = _search_for_triangulation_batch
+LSDmatcher.SearchForTriangulationBatch = _lsd_search_for_triangulation_batch
 
 
 # ---------------------------------------------------------------------------------------------- tracking against a fixed map

@@ -742,61 +742,175 @@ __global__ void __launch_bounds__(32) k_line_search(LineSearchArgs A) {
 //   ORBmatcher::SearchForTriangulation   src/ORBmatcher.cc:720-911
 //   ORBmatcher::Fuse (search half)       src/ORBmatcher.cc:914-1034
 // DBoW2 feature vectors and the map surgery after Fuse's search are outside the path (third-party / sequential map logic).
-struct TriArgs {
-  const PLKeyPoint *k1, *k2; const uint8_t *d1, *d2, *mp1, *mp2;
-  const int *q_idx1, *q_s, *q_e, *fv2_items; int nq, n1;
-  float F[9], ex, ey; const float *scale2, *sigma2_2; int checkOri;
-  int* matches12; int* nmatches; unsigned char* bins;
-};
-// One block.  Every query (idx1, candidate range in KF2's node) is independent: the reference never sets vbMatched2.
-__global__ void __launch_bounds__(256) k_search_triangulation(TriArgs A) {
+
+// Status of problem blockIdx.x of a triangulation batch (PLTriProblems in plslam_b200.h), the same in every thread of the CTA:
+// kf_ok(kf) checks a keyframe's counts against its capacities (status 2), items_ok(kf, t, stride) its CSR items (status 3).
+template <typename KfOk, typename ItemsOk>
+__device__ int tri_status(const PLTriProblems& Q, int n_kf, const int* n, KfOk kf_ok, ItemsOk items_ok) {
+  const int p = blockIdx.x, k1 = Q.kf1[p], k2 = Q.kf2[p];
+  if (k1 < 0 || k1 >= n_kf || k2 < 0 || k2 >= n_kf) return 1;
+  if (!__syncthreads_and(kf_ok(k1, threadIdx.x, blockDim.x) && kf_ok(k2, threadIdx.x, blockDim.x))) return 2;
+  const long long oo = Q.out_offset[p];
+  if (oo < 0 || oo + n[k1] > Q.n_out) return 1;
+  return __syncthreads_and(items_ok(k1, threadIdx.x, blockDim.x) && items_ok(k2, threadIdx.x, blockDim.x)) ? 0 : 3;
+}
+
+// Node b of the ascending list nodes[0 .. nn) that holds `node`, or -1: std::map's lower_bound.
+__device__ __forceinline__ int find_node(const unsigned* nodes, int nn, unsigned node) {
+  int lo = 0, hi = nn;
+  while (lo < hi) { const int mid = (lo + hi) >> 1; if (nodes[mid] < node) lo = mid + 1; else hi = mid; }
+  return lo < nn && nodes[lo] == node ? lo : -1;
+}
+
+// ORBmatcher::SearchForTriangulation: one CTA per problem, one thread per KF1 feature-vector item.  The reference walks the two
+// node lists together with lower_bound jumps (:760-884); both hold ascending unique keys, so it visits exactly the nodes of KF1
+// that KF2 also holds, and a binary search per item finds the same ones.  Every query (idx1, KF2's items of that node) is
+// independent: the reference never sets vbMatched2.  The rotation histogram is a CTA-level shared-memory histogram.
+struct TriBatch { PLTriKeyframes K; PLTriProblems Q; int checkOri; int *match, *nmatches, *status; };
+constexpr int kTriThreads = 256;
+__global__ void __launch_bounds__(kTriThreads) k_search_triangulation(const __grid_constant__ TriBatch A) {
   __shared__ int hist[HISTO];
   __shared__ int s_nm, s_keep[3];
-  const int tid = threadIdx.x;
+  __shared__ float s_F[9], s_e[2];
+  const PLTriKeyframes& K = A.K; const PLTriProblems& Q = A.Q;
+  const int p = blockIdx.x, tid = threadIdx.x;
+  const int st = tri_status(Q, K.n_kf, K.n,
+    [&](int kf, int t, int stride) {
+      const int n = K.n[kf], nn = K.nn[kf];
+      if (n < 0 || n > K.cap || nn < 0 || nn > K.cap_nodes) return false;
+      const int* s = K.fv_start + (long long)kf * (K.cap_nodes + 1);
+      bool ok = t > 0 || (s[0] >= 0 && s[nn] <= n);
+      for (int a = t; a < nn; a += stride) ok = ok && s[a] <= s[a + 1];
+      return ok;
+    },
+    [&](int kf, int t, int stride) {
+      const int n = K.n[kf];
+      const int* s = K.fv_start + (long long)kf * (K.cap_nodes + 1);
+      const int* items = K.fv_items + (long long)kf * K.cap;
+      bool ok = true;
+      for (int j = s[0] + t; j < s[K.nn[kf]]; j += stride) ok = ok && items[j] >= 0 && items[j] < n;
+      return ok;
+    });
+  if (tid == 0) A.status[p] = st;
+  if (st) return;
+  const int k1 = Q.kf1[p], k2 = Q.kf2[p], n1 = K.n[k1], nn1 = K.nn[k1], nn2 = K.nn[k2];
+  const long long r1 = (long long)k1 * K.cap, r2 = (long long)k2 * K.cap;
+  const PLKeyPoint* key1 = K.keys_un + r1; const PLKeyPoint* key2 = K.keys_un + r2;
+  const uint8_t* d1 = K.desc + 32 * r1; const uint8_t* d2 = K.desc + 32 * r2;
+  const uint8_t* mp1 = K.has_mp + r1; const uint8_t* mp2 = K.has_mp + r2;
+  const unsigned* nodes1 = K.fv_nodes + (long long)k1 * K.cap_nodes; const unsigned* nodes2 = K.fv_nodes + (long long)k2 * K.cap_nodes;
+  const int* s1 = K.fv_start + (long long)k1 * (K.cap_nodes + 1); const int* s2 = K.fv_start + (long long)k2 * (K.cap_nodes + 1);
+  const int* items1 = K.fv_items + r1; const int* items2 = K.fv_items + r2;
+  int* match = A.match + Q.out_offset[p];
   if (tid < HISTO) hist[tid] = 0;
-  if (tid == 0) s_nm = 0;
-  for (int i = tid; i < A.n1; i += blockDim.x) { A.matches12[i] = -1; A.bins[i] = 255; }
+  if (tid < 9) s_F[tid] = Q.F12[9LL * p + tid];
+  if (tid == 0) {
+    s_nm = 0;
+    // epipole of camera 1 in image 2 (:729-737): C2 = R2w*Cw + t2w in cv::gemm's fp32 order, every operation rounded on its own
+    const float* T = K.Tcw + 16LL * k2; const float* Cw = K.Ow + 3LL * k1; const float* Kc = K.K + 4LL * k2;
+    float C2[3];
+    for (int i = 0; i < 3; i++)
+      C2[i] = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(T[4 * i], Cw[0]), __fmul_rn(T[4 * i + 1], Cw[1])), __fmul_rn(T[4 * i + 2], Cw[2])), T[4 * i + 3]);
+    const float invz = __fdiv_rn(1.0f, C2[2]);
+    s_e[0] = __fadd_rn(__fmul_rn(__fmul_rn(Kc[0], C2[0]), invz), Kc[2]);
+    s_e[1] = __fadd_rn(__fmul_rn(__fmul_rn(Kc[1], C2[1]), invz), Kc[3]);
+  }
+  for (int i = tid; i < n1; i += kTriThreads) match[i] = -1;
   __syncthreads();
-  for (int q = tid; q < A.nq; q += blockDim.x) {
-    const int idx1 = A.q_idx1[q];
-    if (A.mp1[idx1]) continue;
-    const PLKeyPoint kp1 = A.k1[idx1];
+  const float* F = s_F; const float ex = s_e[0], ey = s_e[1];
+  for (int q = s1[0] + tid; q < s1[nn1]; q += kTriThreads) {
+    int lo = 0, hi = nn1 - 1;          // the node of item q: the last a with s1[a] <= q
+    while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (s1[mid] <= q) lo = mid; else hi = mid - 1; }
+    const int b = find_node(nodes2, nn2, nodes1[lo]);
+    if (b < 0) continue;
+    const int idx1 = items1[q];
+    if (mp1[idx1]) continue;
+    const PLKeyPoint kp1 = key1[idx1];
     // epipolar line of kp1 in image 2 (CheckDistEpipolarLine, :155-172): l = x1' F12
-    const float la = __fadd_rn(__fadd_rn(__fmul_rn(kp1.x, A.F[0]), __fmul_rn(kp1.y, A.F[3])), A.F[6]);
-    const float lb = __fadd_rn(__fadd_rn(__fmul_rn(kp1.x, A.F[1]), __fmul_rn(kp1.y, A.F[4])), A.F[7]);
-    const float lc = __fadd_rn(__fadd_rn(__fmul_rn(kp1.x, A.F[2]), __fmul_rn(kp1.y, A.F[5])), A.F[8]);
+    const float la = __fadd_rn(__fadd_rn(__fmul_rn(kp1.x, F[0]), __fmul_rn(kp1.y, F[3])), F[6]);
+    const float lb = __fadd_rn(__fadd_rn(__fmul_rn(kp1.x, F[1]), __fmul_rn(kp1.y, F[4])), F[7]);
+    const float lc = __fadd_rn(__fadd_rn(__fmul_rn(kp1.x, F[2]), __fmul_rn(kp1.y, F[5])), F[8]);
     const float den = __fadd_rn(__fmul_rn(la, la), __fmul_rn(lb, lb));
     int bestDist = 50, bestIdx2 = -1;
-    for (int i2 = A.q_s[q]; i2 < A.q_e[q]; i2++) {
-      const int idx2 = A.fv2_items[i2];
-      if (A.mp2[idx2]) continue;
-      const int dist = hamming256(A.d1 + 32 * idx1, A.d2 + 32 * idx2);
+    for (int i2 = s2[b]; i2 < s2[b + 1]; i2++) {
+      const int idx2 = items2[i2];
+      if (mp2[idx2]) continue;
+      const int dist = hamming256(d1 + 32 * idx1, d2 + 32 * idx2);
       if (dist > 50 || dist > bestDist) continue;
-      const PLKeyPoint kp2 = A.k2[idx2];
-      const float dx = __fsub_rn(A.ex, kp2.x), dy = __fsub_rn(A.ey, kp2.y);
-      if (__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)) < __fmul_rn(100.f, A.scale2[kp2.octave])) continue;
+      const PLKeyPoint kp2 = key2[idx2];
+      const float dx = __fsub_rn(ex, kp2.x), dy = __fsub_rn(ey, kp2.y);
+      if (__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)) < __fmul_rn(100.f, K.scale_factors[kp2.octave])) continue;
       const float num = __fadd_rn(__fadd_rn(__fmul_rn(la, kp2.x), __fmul_rn(lb, kp2.y)), lc);
       if (den == 0.f) continue;
       const float dsqr = __fdiv_rn(__fmul_rn(num, num), den);
-      if ((double)dsqr < 3.84 * (double)A.sigma2_2[kp2.octave]) { bestIdx2 = idx2; bestDist = dist; }
+      if ((double)dsqr < 3.84 * (double)K.level_sigma2[kp2.octave]) { bestIdx2 = idx2; bestDist = dist; }
     }
     if (bestIdx2 >= 0) {
-      A.matches12[idx1] = bestIdx2;
+      match[idx1] = bestIdx2;
       atomicAdd(&s_nm, 1);
-      if (A.checkOri) { const int bin = rot_bin(kp1.angle, A.k2[bestIdx2].angle); A.bins[idx1] = (unsigned char)bin; atomicAdd(&hist[bin], 1); }
+      if (A.checkOri) atomicAdd(&hist[rot_bin(kp1.angle, key2[bestIdx2].angle)], 1);
     }
   }
   __syncthreads();
   if (A.checkOri) {
     if (tid == 0) { int a, b, c; three_maxima(hist, a, b, c); s_keep[0] = a; s_keep[1] = b; s_keep[2] = c; }
     __syncthreads();
-    for (int i = tid; i < A.n1; i += blockDim.x) {
-      const int bin = A.bins[i];
-      if (bin != 255 && bin != s_keep[0] && bin != s_keep[1] && bin != s_keep[2]) { A.matches12[i] = -1; atomicSub(&s_nm, 1); }
+    for (int i = tid; i < n1; i += kTriThreads) {
+      const int j = match[i];
+      if (j < 0) continue;
+      const int bin = rot_bin(key1[i].angle, key2[j].angle);
+      if (bin != s_keep[0] && bin != s_keep[1] && bin != s_keep[2]) { match[i] = -1; atomicSub(&s_nm, 1); }
     }
     __syncthreads();
   }
-  if (tid == 0) *A.nmatches = s_nm;
+  if (tid == 0) A.nmatches[p] = s_nm;
+}
+
+// LSDmatcher::SearchForTriangulation (src/LSDmatcher.cpp:727-776): k_search_double for P (KF1, KF2) problems of a keyframe table,
+// then the pairs whose line already has a MapLine on either side are dropped (:756).  Shared memory is laid out on the problem's
+// own counts, m1[N1], m2[N2], bd0 and bd1[max(N1, N2)], inside what the launch reserves for its largest problem.
+struct LineTriBatch { PLTriLineKeyframes K; PLTriProblems Q; float th, nnratio; int mutual; int *match, *nmatches, *status; };
+__global__ void __launch_bounds__(128) k_lsd_search_triangulation(const __grid_constant__ LineTriBatch A) {
+  extern __shared__ unsigned char smem[];
+  __shared__ int hist[257];
+  __shared__ int total;
+  const PLTriLineKeyframes& K = A.K; const PLTriProblems& Q = A.Q;
+  const int p = blockIdx.x, tid = threadIdx.x;
+  const int st = tri_status(Q, K.n_kf, K.n, [&](int kf, int, int) { return K.n[kf] >= 0 && K.n[kf] <= K.cap; },
+                            [](int, int, int) { return true; });
+  if (tid == 0) A.status[p] = st;
+  if (st) return;
+  const int k1 = Q.kf1[p], k2 = Q.kf2[p], N1 = K.n[k1], N2 = K.n[k2];
+  const uint8_t* a = K.ldesc + 32LL * k1 * K.cap; const uint8_t* c = K.ldesc + 32LL * k2 * K.cap;
+  const uint8_t* ml1 = K.has_ml + (long long)k1 * K.cap; const uint8_t* ml2 = K.has_ml + (long long)k2 * K.cap;
+  int* out = A.match + Q.out_offset[p];
+  if (N1 == 0 || N2 == 0) {     // ldesc.rows == 0 -> return 0 (:738-739)
+    for (int i = tid; i < N1; i += 128) out[i] = -1;
+    if (tid == 0) A.nmatches[p] = 0;
+    return;
+  }
+  short* m1 = reinterpret_cast<short*>(smem);
+  short* m2 = m1 + N1;
+  short* bd0 = m2 + N2;
+  short* bd1 = bd0 + max(N1, N2);
+  frame_bf_match_cta(a, N1, c, N2, A.th, A.nnratio, m1, bd0, bd1, hist);
+  __syncthreads();
+  if (A.mutual) {
+    frame_bf_match_cta(c, N2, a, N1, A.th, A.nnratio, m2, bd0, bd1, hist);
+    __syncthreads();
+  }
+  int cnt = 0;
+  for (int i = tid; i < N1; i += 128) {
+    int j = m1[i];
+    if (j >= 0 && ((A.mutual && m2[j] != i) || ml1[i] || ml2[j])) j = -1;
+    out[i] = j;
+    cnt += (j >= 0);
+  }
+  if (tid == 0) total = 0;
+  __syncthreads();
+  atomicAdd(&total, cnt);
+  __syncthreads();
+  if (tid == 0) A.nmatches[p] = total;
 }
 
 struct SkipChi2 {
@@ -1305,21 +1419,23 @@ extern "C" int pl_match_bf_knn2(const uint8_t* d1, int n1, const uint8_t* d2, in
 
 // m1[cap1], m2[cap2], bd0 and bd1[max(cap1, cap2)] of k_search_double
 static size_t search_double_smem(int cap1, int cap2) { return (size_t)(cap1 + cap2 + 2 * std::max(cap1, cap2)) * sizeof(short); }
-int pl::search_double_fits(int cap1, int cap2) {
+// PL_OK if search_double_smem(cap1, cap2) fits beside `kernel`'s static shared memory
+static int search_double_fits_for(const void* kernel, const char* name, int cap1, int cap2) {
   int dev = 0, optin = 0;
   cudaFuncAttributes fa;
   PL_CUDA(cudaGetDevice(&dev));
   PL_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
-  PL_CUDA(cudaFuncGetAttributes(&fa, k_search_double));
+  PL_CUDA(cudaFuncGetAttributes(&fa, kernel));
   const size_t room = optin > (int)fa.sharedSizeBytes ? (size_t)optin - fa.sharedSizeBytes : 0;
   if (search_double_smem(cap1, cap2) > room) {
-    set_error("line matching of %d against %d lines needs %zu B of shared memory beside k_search_double's %zu static B, over the "
-              "device's %d B per block; at most %zu lines per side fit", cap1, cap2, search_double_smem(cap1, cap2),
+    set_error("line matching of %d against %d lines needs %zu B of shared memory beside %s's %zu static B, over the "
+              "device's %d B per block; at most %zu lines per side fit", cap1, cap2, search_double_smem(cap1, cap2), name,
               (size_t)fa.sharedSizeBytes, optin, room / (4 * sizeof(short)));
     return PL_ERR_ARG;
   }
   return PL_OK;
 }
+int pl::search_double_fits(int cap1, int cap2) { return search_double_fits_for((const void*)k_search_double, "k_search_double", cap1, cap2); }
 
 extern "C" int pl_lsd_search_double_dev(const uint8_t* d1, const int* n1, const uint8_t* d2, const int* n2, int cap1,
                                         int cap2, int B, float th, float nnratio, int mutual, int* matches,
@@ -1356,23 +1472,64 @@ extern "C" int pl_lsd_frame_bf_match(const uint8_t* d1, int n1, const uint8_t* d
 extern "C" int pl_lsd_search_double(const uint8_t* d1, int n1, const uint8_t* d2, int n2, float nnratio, int* matches) {
   return search_double_host(d1, n1, d2, n2, 50.f, nnratio, 1, matches);
 }
+// PL_OK if a triangulation batch's problem table can be read as plslam_b200.h states (PLTriProblems); the rest is checked on the
+// device.  The line call does not read F12.
+static int tri_problems_ok(const PLTriProblems* Q, bool points, int* match, int* nmatches, int* status) {
+  PL_ARG(Q && Q->P >= 0 && Q->n_out >= 0);
+  if (Q->P == 0) return PL_OK;
+  PL_ARG(Q->kf1 && Q->kf2 && Q->out_offset && (Q->F12 || !points) && nmatches && status);
+  PL_ARG(Q->n_out == 0 || match);
+  return PL_OK;
+}
+
+// sm: the dynamic shared memory of the largest problem, search_double_smem(N1, N2)
+static int lsd_tri_launch(const PLTriLineKeyframes& K, const PLTriProblems& Q, float th, float nnratio, int mutual, size_t sm, int* match,
+                          int* nmatches, int* status, void* stream) {
+  PL_CUDA(cudaFuncSetAttribute(k_lsd_search_triangulation, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
+  const LineTriBatch A{K, Q, th, nnratio, mutual, match, nmatches, status};
+  k_lsd_search_triangulation<<<Q.P, 128, sm, (cudaStream_t)stream>>>(A);
+  PL_LAUNCH_CHECK();
+  return PL_OK;
+}
+
+extern "C" int pl_lsd_search_for_triangulation_dev(const PLTriLineKeyframes* kfs, const PLTriProblems* problems, float th, float nnratio,
+                                                   int is_double, int* matched_pairs, int* nmatches, int* status, void* stream) {
+  PL_TRY(tri_problems_ok(problems, false, matched_pairs, nmatches, status));
+  if (problems->P == 0) return PL_OK;
+  PL_ARG(kfs);
+  const PLTriLineKeyframes& K = *kfs;
+  PL_ARG(K.n_kf >= 1 && K.cap >= 1 && K.cap < 32000 && (long long)K.n_kf * K.cap <= INT_MAX && K.ldesc && K.has_ml && K.n);
+  PL_TRY(require_device());
+  PL_TRY(search_double_fits_for((const void*)k_lsd_search_triangulation, "k_lsd_search_triangulation", K.cap, K.cap));
+  return lsd_tri_launch(K, *problems, th, nnratio, is_double ? 1 : 0, search_double_smem(K.cap, K.cap), matched_pairs, nmatches,
+                        status, stream);
+}
+
 // LSDmatcher::SearchForTriangulation(pKF1, pKF2, vMatchedPairs, isDouble) (src/LSDmatcher.cpp:727-776, the variant
 // LocalMapping calls at LocalMapping.cc:961, th = TH_HIGH = 80) and its pair<> twin (:672-725, LocalMapping.cc:679, th = TH_LOW = 50,
-// always mutual): FrameBFMatch both ways at th, optional mutual check, then pairs
-// whose line already has a MapLine on either side are dropped (a few hundred flags: applied on the host).
+// always mutual): the P = 1 case of pl_lsd_search_for_triangulation_dev, a table of the two keyframes.
 extern "C" int pl_lsd_search_for_triangulation(const uint8_t* ldesc1, const uint8_t* has_ml1, int n1, const uint8_t* ldesc2,
                                                const uint8_t* has_ml2, int n2, float th, float nnratio, int is_double, int* matched_pairs) {
   PL_ARG(matched_pairs && n1 >= 0 && n2 >= 0 && (n1 == 0 || (ldesc1 && has_ml1)) && (n2 == 0 || (ldesc2 && has_ml2)));
   for (int i = 0; i < n1; i++) matched_pairs[i] = -1;
   if (n1 == 0 || n2 == 0) { int rc = require_device(); return rc ? rc : 0; }     // ldesc.rows == 0 -> return 0 (:738-739)
-  int rc = search_double_host(ldesc1, n1, ldesc2, n2, th, nnratio, is_double ? 1 : 0, matched_pairs);
-  if (rc < 0) return rc;
-  int nm = 0;
-  for (int i = 0; i < n1; i++) {
-    const int j = matched_pairs[i];
-    if (j < 0) continue;
-    if (has_ml1[i] || has_ml2[j]) matched_pairs[i] = -1; else nm++;
-  }
+  int rc = require_device(); if (rc) return rc;
+  PL_ARG(n1 < 32000 && n2 < 32000);
+  PL_TRY(search_double_fits_for((const void*)k_lsd_search_triangulation, "k_lsd_search_triangulation", n1, n2));
+  const int cap = std::max(n1, n2);
+  std::vector<uint8_t> desc((size_t)2 * cap * 32, 0), ml((size_t)2 * cap, 0);
+  memcpy(desc.data(), ldesc1, (size_t)n1 * 32); memcpy(desc.data() + (size_t)cap * 32, ldesc2, (size_t)n2 * 32);
+  memcpy(ml.data(), has_ml1, n1); memcpy(ml.data() + cap, has_ml2, n2);
+  const int ints[5] = {n1, n2, 0, 1, 0};     // the keyframes' counts; kf1, kf2, out_offset of the one problem
+  Staging s;
+  const int* di = s.in(ints, 5);
+  const PLTriLineKeyframes K{2, cap, s.in(desc.data(), desc.size()), s.in(ml.data(), ml.size()), di};
+  const PLTriProblems Q{1, di + 2, di + 3, nullptr, di + 4, n1};
+  int nm = 0, st = 0;
+  int* dm = s.out(matched_pairs, n1); int* dnm = s.out(&nm, 1); int* dst = s.out(&st, 1);
+  if ((rc = s.status())) return rc;
+  PL_TRY(lsd_tri_launch(K, Q, th, nnratio, is_double ? 1 : 0, search_double_smem(n1, n2), dm, dnm, dst, nullptr));
+  if ((rc = s.fetch())) return rc;
   return nm;
 }
 
@@ -1485,6 +1642,30 @@ extern "C" int pl_lsd_search_by_projection_dev(int variant, const void* keylines
 
 // ------------------------------------------------------------------------------------------------ §8f.2 wrappers
 
+static int orb_tri_launch(const PLTriKeyframes& K, const PLTriProblems& Q, int check_orientation, int* match, int* nmatches, int* status,
+                          void* stream) {
+  const TriBatch A{K, Q, check_orientation ? 1 : 0, match, nmatches, status};
+  k_search_triangulation<<<Q.P, kTriThreads, 0, (cudaStream_t)stream>>>(A);
+  PL_LAUNCH_CHECK();
+  return PL_OK;
+}
+
+extern "C" int pl_orb_search_for_triangulation_dev(const PLTriKeyframes* kfs, const PLTriProblems* problems, int check_orientation,
+                                                   int* matches12, int* nmatches, int* status, void* stream) {
+  PL_TRY(tri_problems_ok(problems, true, matches12, nmatches, status));
+  if (problems->P == 0) return PL_OK;
+  PL_ARG(kfs);
+  const PLTriKeyframes& K = *kfs;
+  PL_ARG(K.n_kf >= 1 && K.cap >= 1 && K.cap <= kMatchMaxKeys && K.cap_nodes >= 1 && K.nlevels >= 1);
+  PL_ARG((long long)K.n_kf * K.cap <= INT_MAX && (long long)K.n_kf * (K.cap_nodes + 1) <= INT_MAX);
+  PL_ARG(K.keys_un && K.desc && K.has_mp && K.n && K.fv_nodes && K.fv_start && K.fv_items && K.nn && K.Tcw && K.Ow && K.K &&
+         K.scale_factors && K.level_sigma2);
+  PL_TRY(require_device());
+  return orb_tri_launch(K, *problems, check_orientation, matches12, nmatches, status, stream);
+}
+
+// The P = 1 case of pl_orb_search_for_triangulation_dev: a table of the two keyframes, KF1 in row 0 (Ow = Cw1) and KF2 in row 1
+// (Tcw from R2w / t2w, K = K2).
 extern "C" int pl_orb_search_for_triangulation(const PLKeyPoint* keys1_un, const uint8_t* desc1, const uint8_t* has_mp1, int n1,
                                                const PLKeyPoint* keys2_un, const uint8_t* desc2, const uint8_t* has_mp2, int n2,
                                                const unsigned* fv1_nodes, const int* fv1_start, const int* fv1_items, int nn1,
@@ -1497,41 +1678,43 @@ extern "C" int pl_orb_search_for_triangulation(const PLKeyPoint* keys1_un, const
   PL_ARG((nn1 == 0 || (fv1_nodes && fv1_start && fv1_items)) && (nn2 == 0 || (fv2_nodes && fv2_start && fv2_items)));
   int rc = require_device(); if (rc) return rc;
   for (int i = 0; i < n1; i++) matches12[i] = -1;
-  // the node merge of :760-884 (std::map order, lower_bound jumps) on the host: one query per keypoint of a shared node
-  std::vector<int> q_idx1, q_s, q_e;
-  for (int a = 0, b = 0; a < nn1 && b < nn2;) {
-    if (fv1_nodes[a] == fv2_nodes[b]) {
-      for (int i1 = fv1_start[a]; i1 < fv1_start[a + 1]; i1++) {
-        PL_ARG(fv1_items[i1] >= 0 && fv1_items[i1] < n1);
-        q_idx1.push_back(fv1_items[i1]); q_s.push_back(fv2_start[b]); q_e.push_back(fv2_start[b + 1]);
-      }
-      a++; b++;
-    } else if (fv1_nodes[a] < fv2_nodes[b]) a++;
-    else b++;
-  }
-  if (q_idx1.empty() || n1 == 0 || n2 == 0) return 0;
-  const int nitems2 = fv2_start[nn2];
-  for (int i = 0; i < nitems2; i++) PL_ARG(fv2_items[i] >= 0 && fv2_items[i] < n2);
+  const int cap = std::max(std::max(n1, n2), 1), capn = std::max(std::max(nn1, nn2), 1);
+  std::vector<PLKeyPoint> keys((size_t)2 * cap);
+  std::vector<uint8_t> desc((size_t)2 * cap * 32, 0), mp((size_t)2 * cap, 0);
+  std::vector<unsigned> nodes((size_t)2 * capn, 0);
+  std::vector<int> start((size_t)2 * (capn + 1), 0), items((size_t)2 * cap, 0);
+  auto put = [&](int r, const PLKeyPoint* k, const uint8_t* d, const uint8_t* m, int n, const unsigned* fn, const int* fs, const int* fi, int nn) {
+    std::copy(k, k + n, keys.begin() + (size_t)r * cap);
+    memcpy(desc.data() + (size_t)r * cap * 32, d, (size_t)n * 32); memcpy(mp.data() + (size_t)r * cap, m, n);
+    if (nn == 0) return;
+    std::copy(fn, fn + nn, nodes.begin() + (size_t)r * capn); std::copy(fs, fs + nn + 1, start.begin() + (size_t)r * (capn + 1));
+    const int ni = std::min(std::max(fs[nn], 0), cap);     // a count past n is reported by the kernel (status 2), not read
+    std::copy(fi, fi + ni, items.begin() + (size_t)r * cap);
+  };
+  put(0, keys1_un, desc1, has_mp1, n1, fv1_nodes, fv1_start, fv1_items, nn1);
+  put(1, keys2_un, desc2, has_mp2, n2, fv2_nodes, fv2_start, fv2_items, nn2);
+  float cam[46] = {0};     // Tcw [2][16], Ow [2][3], K [2][4]: one upload
+  for (int r = 0; r < 3; r++) { memcpy(cam + 16 + 4 * r, R2w + 3 * r, 12); cam[16 + 4 * r + 3] = t2w[r]; }
+  cam[31] = 1.f;
+  memcpy(cam + 32, Cw1, 12); memcpy(cam + 42, K2, 16);
+  float fz[9]; memcpy(fz, F12, 36);
+  const int ints[7] = {n1, n2, nn1, nn2, 0, 1, 0};     // n [2], nn [2]; kf1, kf2, out_offset of the one problem
   Staging s;
-  TriArgs A;
-  A.k1 = s.in(keys1_un, n1); A.k2 = s.in(keys2_un, n2); A.d1 = s.in(desc1, (size_t)n1 * 32); A.d2 = s.in(desc2, (size_t)n2 * 32);
-  A.mp1 = s.in(has_mp1, n1); A.mp2 = s.in(has_mp2, n2);
-  A.q_idx1 = s.in(q_idx1.data(), q_idx1.size()); A.q_s = s.in(q_s.data(), q_s.size()); A.q_e = s.in(q_e.data(), q_e.size());
-  A.fv2_items = s.in(fv2_items, nitems2); A.nq = (int)q_idx1.size(); A.n1 = n1;
-  memcpy(A.F, F12, sizeof(A.F));
-  {  // epipole of camera 1 in image 2 (:729-737): C2 = R2w*Cw + t2w in cv::gemm's fp32 order
-    float C2[3];
-    for (int i = 0; i < 3; i++) C2[i] = ((R2w[3 * i] * Cw1[0] + R2w[3 * i + 1] * Cw1[1]) + R2w[3 * i + 2] * Cw1[2]) + t2w[i];
-    const float invz = 1.0f / C2[2];
-    A.ex = K2[0] * C2[0] * invz + K2[2]; A.ey = K2[1] * C2[1] * invz + K2[3];
-  }
-  A.scale2 = s.in(scale_factors2, nlevels); A.sigma2_2 = s.in(level_sigma2_2, nlevels); A.checkOri = check_orientation;
-  int nm = 0;
-  A.matches12 = s.out(matches12, n1); A.nmatches = s.out(&nm, 1); A.bins = s.out<unsigned char>(n1);
+  const float* dc = s.in(cam, 46); const int* di = s.in(ints, 7);
+  const PLTriKeyframes K{2, cap, capn, s.in(keys.data(), keys.size()), s.in(desc.data(), desc.size()), s.in(mp.data(), mp.size()), di,
+                         s.in(nodes.data(), nodes.size()), s.in(start.data(), start.size()), s.in(items.data(), items.size()), di + 2,
+                         dc, dc + 32, dc + 38, s.in(scale_factors2, nlevels), s.in(level_sigma2_2, nlevels), nlevels};
+  const PLTriProblems Q{1, di + 4, di + 5, s.in(fz, 9), di + 6, n1};
+  int nm = 0, st = 0;
+  int* dm = s.out(matches12, n1); int* dnm = s.out(&nm, 1); int* dst = s.out(&st, 1);
   if ((rc = s.status())) return rc;
-  k_search_triangulation<<<1, 256>>>(A);
-  PL_LAUNCH_CHECK();
+  PL_TRY(orb_tri_launch(K, Q, check_orientation, dm, dnm, dst, nullptr));
   if ((rc = s.fetch())) return rc;
+  if (st) {
+    set_error("pl_orb_search_for_triangulation: a feature vector is malformed (%s)",
+              st == 2 ? "fv_start not monotone, or past the keypoint count" : "an fv_items entry outside 0 .. n - 1");
+    return PL_ERR_ARG;
+  }
   return nm;
 }
 
