@@ -608,6 +608,7 @@ typedef struct PLTriProblems {
  * (GetMapPoint(i) != NULL at the snapshot), n [n_kf]; mFeatVec as CSR per keyframe: fv_nodes [n_kf][cap_nodes] (ascending and
  * unique, as std::map keeps them), fv_start [n_kf][cap_nodes + 1], fv_items [n_kf][cap], nn [n_kf] nodes; the camera Tcw [n_kf][16]
  * (row-major; R2w and t2w of a KF2), Ow [n_kf][3] (GetCameraCenter() as stored; Cw of a KF1), K [n_kf][4] (fx fy cx cy of a KF2);
+ * pl_orb_triangulate_dev reads Tcw, Ow and K of KF1 and of KF2;
  * scale_factors / level_sigma2 [nlevels] (mvScaleFactors, mvLevelSigma2) shared by every keyframe. */
 typedef struct PLTriKeyframes {
   int n_kf, cap, cap_nodes;
@@ -637,6 +638,35 @@ int pl_orb_search_for_triangulation_dev(const PLTriKeyframes* kfs, const PLTriPr
                                         int* matches12, int* nmatches, int* status, void* stream);
 int pl_lsd_search_for_triangulation_dev(const PLTriLineKeyframes* kfs, const PLTriProblems* problems, float th, float nnratio,
                                         int is_double, int* matched_pairs, int* nmatches, int* status, void* stream);
+
+/* The triangulation of LocalMapping::CreateNewMapPoints (src/LocalMapping.cc:417-574, monocular) for the pairs that
+ * pl_orb_search_for_triangulation_dev found, with the neighbour-order commit, on the same keyframe table and problem list, enqueued
+ * on `stream`: kernels only, no allocation, copy or synchronisation, so the call can be captured into a CUDA graph together with
+ * the search.  matches12 and search_status are the search's outputs, read on the device.  It reads keys_un, n, Tcw, Ow, K (of KF1
+ * and KF2), scale_factors, level_sigma2 and nlevels of the table, never the descriptors, has_mp or the feature vector.
+ * scale_factor is KF1's mfScaleFactor (ratioFactor = 1.5f * scale_factor); scale_factors[1] does not exist when nlevels == 1.
+ * The caller guarantees 0 <= octave < nlevels for every keypoint of KF1 and KF2 in a pair (ORBextractor's keypoints satisfy it):
+ * scale_factors and level_sigma2 are read at both keypoints' octaves unchecked, as the search reads them at KF2's.
+ *
+ * Per slot out_offset[p] + idx1, idx1 < n[kf1[p]]: code -1 no pair (matches12 = -1); 0 committed; 1 dropped at commit (the pair
+ * passed the gates, but an earlier problem with the same kf1 committed or dropped a pair at the same idx1: the reference searched
+ * that neighbour later, when idx1 already held a map point); 2 .. 8 the first gate that rejected it: 2 parallax (cosParallaxRays
+ * not in (0, 0.9998)), 3 vt.row(3)[3] == 0, 4 behind camera 1, 5 behind camera 2, 6 reprojection in KF1, 7 reprojection in KF2
+ * (5.991 sigma^2 at the keypoint's octave), 8 scale consistency (a zero distance, or the distance ratio off the octave ratio by
+ * more than ratioFactor).  x3D [n_out][3] is the triangulated point (world) for codes 0 and 1, bit for bit the reference's.
+ * Per problem: nnew[p] = the number of committed slots; status[p] = search_status[p] when that is nonzero, else 1: kf1[p] or
+ * kf2[p] outside the table or the output range outside n_out, 2: n[kf1] or n[kf2] negative or over cap, 4: a matches12 entry of
+ * the problem outside -1 .. n[kf2] - 1, or 0.  A problem with a nonzero status writes nothing but status[p].
+ *
+ * A caller applies the committed slots in problem order, then in ascending idx1: that is the reference's creation order when the
+ * problems of a kf1 are its neighbours in the reference's order.  Two committed slots of one problem may share an idx2 (the search
+ * never marks KF2's keypoints as taken); the reference creates both points, and KF2's slot ends up with the later one
+ * (AddMapPoint overwrites it).  Problems with different kf1 are independent.
+ * PL_ERR_ARG before anything is enqueued: the argument and capacity rules of pl_orb_search_for_triangulation_dev on kfs, problems
+ * and (matches12, nnew, status) in the places of (matches12, nmatches, status), and a NULL search_status, or a NULL x3D or code
+ * when n_out > 0.  P = 0 enqueues nothing. */
+int pl_orb_triangulate_dev(const PLTriKeyframes* kfs, const PLTriProblems* problems, const int* matches12, const int* search_status,
+                           float scale_factor, float* x3D, int8_t* code, int* nnew, int* status, void* stream);
 
 /* ------------------------------------------------------------------ tracking a batch of frames against a fixed map
  * Tracking::TrackLocalMapWithLines (src/Tracking.cc:1491-1562) with SearchLocalPoints (:1751-1801) and SearchLocalLines

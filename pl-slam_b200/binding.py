@@ -1241,6 +1241,7 @@ def _tri_lib():
         L.pl_orb_search_for_triangulation_dev.argtypes = [C.POINTER(PLTriKeyframes), C.POINTER(PLTriProblems), C.c_int] + [vp] * 4
         L.pl_lsd_search_for_triangulation_dev.argtypes = ([C.POINTER(PLTriLineKeyframes), C.POINTER(PLTriProblems), C.c_float, C.c_float,
                                                             C.c_int] + [vp] * 4)
+        L.pl_orb_triangulate_dev.argtypes = [C.POINTER(PLTriKeyframes), C.POINTER(PLTriProblems), vp, vp, C.c_float] + [vp] * 5
         L._tri_types = True
     return L
 
@@ -1283,7 +1284,12 @@ class TriangulationProblems:
     pack_tri_problems) into torch CUDA tensors and allocates the outputs once; run() only enqueues the launch, so it can be captured
     into a CUDA graph; results() waits for it and returns one dict per problem: matches (numpy [n[kf1]]: idx2 or -1), nmatches and
     status.  Points: scales = (scale_factors, level_sigma2), options = check_orientation; lines: options = (th, nnratio, is_double).
-    Outputs are pre-filled with `out_fill`."""
+    Outputs are pre-filled with `out_fill` (x3D with NaN).
+
+    Points also triangulate (LocalMapping::CreateNewMapPoints): triangulate() enqueues pl_orb_triangulate_dev on the search's device
+    outputs, which it reads where run() left them, and triangulated() returns one dict per problem: code (numpy int8 [n[kf1]]: -1 no
+    pair, 0 committed, 1 dropped at commit, 2 .. 8 the gate that rejected it), x3D ([n[kf1]][3], written for codes 0 and 1), nnew and
+    status."""
 
     def __init__(self, keyframes, problems, scales=None, lines=False, options=0, out_fill=-7):
         import torch
@@ -1300,6 +1306,13 @@ class TriangulationProblems:
         self.outputs = dict(matches=torch.full((max(q["n_out"], 1),), out_fill, dtype=torch.int32, device="cuda"),
                             nmatches=torch.full((max(self.P, 1),), out_fill, dtype=torch.int32, device="cuda"),
                             status=torch.full((max(self.P, 1),), out_fill, dtype=torch.int32, device="cuda"))
+        if not lines:
+            n_out = max(q["n_out"], 1)
+            self.outputs.update(code=torch.full((n_out,), out_fill, dtype=torch.int8, device="cuda"),
+                                x3D=torch.full((n_out, 3), float("nan"), dtype=torch.float32, device="cuda"),
+                                nnew=torch.full((max(self.P, 1),), out_fill, dtype=torch.int32, device="cuda"),
+                                tri_status=torch.full((max(self.P, 1),), out_fill, dtype=torch.int32, device="cuda"))
+            self.scale_factors = np.asarray(scales[0], np.float32)
         i = lambda n: self.inputs[n].data_ptr()
         self._q = PLTriProblems(self.P, i("q_kf1"), i("q_kf2"), None if lines else i("q_F12"), i("q_out_offset"), q["n_out"])
         n_kf = len(keyframes)
@@ -1323,6 +1336,27 @@ class TriangulationProblems:
         else:
             check(L.pl_orb_search_for_triangulation_dev(C.byref(self._k), C.byref(self._q), int(self.options), o["matches"],
                                                         o["nmatches"], o["status"], s))
+
+    def triangulate(self, stream=None, scale_factor=None):
+        """pl_orb_triangulate_dev on `stream` after run(): enqueues, does not wait.  scale_factor: KF1's mfScaleFactor (default
+        scale_factors[1], which a single-level table does not have)."""
+        assert not self.lines, "the line searches have no triangulation here"
+        if scale_factor is None:
+            assert len(self.scale_factors) > 1, "nlevels == 1: pass the keyframe's mfScaleFactor"
+            scale_factor = float(self.scale_factors[1])
+        s = None if stream is None else stream.cuda_stream
+        o = {n: t.data_ptr() for n, t in self.outputs.items()}
+        check(_tri_lib().pl_orb_triangulate_dev(C.byref(self._k), C.byref(self._q), o["matches"], o["status"], float(scale_factor),
+                                                o["x3D"], o["code"], o["nnew"], o["tri_status"], s))
+
+    def triangulated(self):
+        import torch
+        torch.cuda.synchronize()
+        h = {n: t.cpu().numpy() for n, t in self.outputs.items()}
+        q = self.host["q"]
+        sl = lambda p: slice(q["out_offset"][p], q["out_offset"][p] + q["count"][p])
+        return [dict(code=h["code"][sl(p)].copy(), x3D=h["x3D"][sl(p)].copy(), nnew=int(h["nnew"][p]), status=int(h["tri_status"][p]))
+                for p in range(self.P)]
 
     def results(self):
         import torch

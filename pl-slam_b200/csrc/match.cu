@@ -1474,7 +1474,7 @@ extern "C" int pl_lsd_search_double(const uint8_t* d1, int n1, const uint8_t* d2
 }
 // PL_OK if a triangulation batch's problem table can be read as plslam_b200.h states (PLTriProblems); the rest is checked on the
 // device.  The line call does not read F12.
-static int tri_problems_ok(const PLTriProblems* Q, bool points, int* match, int* nmatches, int* status) {
+static int tri_problems_ok(const PLTriProblems* Q, bool points, const void* match, const void* nmatches, const void* status) {
   PL_ARG(Q && Q->P >= 0 && Q->n_out >= 0);
   if (Q->P == 0) return PL_OK;
   PL_ARG(Q->kf1 && Q->kf2 && Q->out_offset && (Q->F12 || !points) && nmatches && status);
@@ -1650,9 +1650,9 @@ static int orb_tri_launch(const PLTriKeyframes& K, const PLTriProblems& Q, int c
   return PL_OK;
 }
 
-extern "C" int pl_orb_search_for_triangulation_dev(const PLTriKeyframes* kfs, const PLTriProblems* problems, int check_orientation,
-                                                   int* matches12, int* nmatches, int* status, void* stream) {
-  PL_TRY(tri_problems_ok(problems, true, matches12, nmatches, status));
+int pl::orb_tri_args_ok(const PLTriKeyframes* kfs, const PLTriProblems* problems, const void* match, const void* nmatches,
+                        const void* status) {
+  PL_TRY(tri_problems_ok(problems, true, match, nmatches, status));
   if (problems->P == 0) return PL_OK;
   PL_ARG(kfs);
   const PLTriKeyframes& K = *kfs;
@@ -1660,6 +1660,14 @@ extern "C" int pl_orb_search_for_triangulation_dev(const PLTriKeyframes* kfs, co
   PL_ARG((long long)K.n_kf * K.cap <= INT_MAX && (long long)K.n_kf * (K.cap_nodes + 1) <= INT_MAX);
   PL_ARG(K.keys_un && K.desc && K.has_mp && K.n && K.fv_nodes && K.fv_start && K.fv_items && K.nn && K.Tcw && K.Ow && K.K &&
          K.scale_factors && K.level_sigma2);
+  return PL_OK;
+}
+
+extern "C" int pl_orb_search_for_triangulation_dev(const PLTriKeyframes* kfs, const PLTriProblems* problems, int check_orientation,
+                                                   int* matches12, int* nmatches, int* status, void* stream) {
+  PL_TRY(orb_tri_args_ok(kfs, problems, matches12, nmatches, status));
+  if (problems->P == 0) return PL_OK;
+  const PLTriKeyframes& K = *kfs;
   PL_TRY(require_device());
   return orb_tri_launch(K, *problems, check_orientation, matches12, nmatches, status, stream);
 }

@@ -15,6 +15,11 @@ constexpr int kMatchMaxKeys = 6144;
 // PL_OK if k_search_double's shared memory for line capacities cap1 and cap2 fits the device's opt-in limit per block beside the
 // kernel's static shared memory, else PL_ERR_ARG with a message naming the largest equal capacity that fits.
 int search_double_fits(int cap1, int cap2);
+// The argument and capacity rules of pl_orb_search_for_triangulation_dev (plslam_b200.h), which pl_orb_triangulate_dev applies to
+// the same tables: PL_OK or PL_ERR_ARG, nothing enqueued.  `match` is the per-slot array of n_out entries, nmatches / status the
+// per-problem outputs.  P = 0 passes without looking at the keyframe table.
+int orb_tri_args_ok(const PLTriKeyframes* kfs, const PLTriProblems* problems, const void* match, const void* nmatches,
+                    const void* status);
 int search_by_projection_last_launch(const PLKeyPoint* keys_cur, const uint8_t* desc_cur, const int* n_cur, int cap, int B,
                                      const float* bounds, const float* Tcw, const float* K, const float* scale_factors, int nlevels,
                                      const int* n_last, int cap_last, const uint8_t* last_valid, const float* last_pos,

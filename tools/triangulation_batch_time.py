@@ -7,7 +7,11 @@ against its 20 best covisible neighbours for points (CreateNewMapPoints, ORBmatc
           synchronises);
   device: pl_orb_search_for_triangulation_dev with the 20 problems and pl_lsd_search_for_triangulation_dev with the 10 (two launches
           on one stream, CUDA events around them);
-  batched keyframes: the searches of --keyframes such keyframes in one launch per kind.
+  batched keyframes: the searches of --keyframes such keyframes in one launch per kind;
+  point search + triangulation: pl_orb_search_for_triangulation_dev then pl_orb_triangulate_dev (the gates and the neighbour-order
+          commit) for one keyframe's 20 problems and for --keyframes keyframes', three launches on one stream, CUDA events around
+          them; the triangulation launches alone as well;
+  CPU oracle: tests/cnmp_oracle.py's triangulate (numpy, vectorised over the pairs) on the same search outputs, a CPU time.
 After --warmup calls, --rounds rounds alternate the forms; each number is the median over the timed calls.  Prints one JSON line,
 with the card's name and power limit read in the same run.
 
@@ -105,8 +109,33 @@ def main():
     nm, m = L.SearchForTriangulation(lkf[k1]["ldesc"], lkf[k1]["has_ml"], lkf[k2]["ldesc"], lkf[k2]["has_ml"], True)
     assert rl[3]["nmatches"] == nm > 10 and np.array_equal(rl[3]["matches"], m)
 
+    # the triangulation computes what the oracle computes, on the same search outputs
+    import cnmp_oracle as co
+    sfac = float(s["scale_factors"][1])
+    dev[0].triangulate(scale_factor=sfac)
+    tri = dev[0].triangulated()
+    m12 = dev[0].outputs["matches"].cpu().numpy()[:dev[0].host["q"]["n_out"]]
+    st = dev[0].outputs["status"].cpu().numpy()[:dev[0].P]
+    oc = co.triangulate(dev[0].host["k"], dev[0].host["q"], m12, st, sfac, *scales)
+    assert np.array_equal(np.concatenate([t["code"] for t in tri]), oc[0]) and sum(t["nnew"] for t in tri) == oc[2].sum() > 100
+
+    class SearchTri:                     # search + triangulation of one TriangulationProblems, as one timed object
+        def __init__(self, b, only_tri=False):
+            self.b, self.only_tri = b, only_tri
+
+        def run(self, stream):
+            if not self.only_tri:
+                self.b.run(stream)
+            self.b.triangulate(stream, scale_factor=sfac)
+    st1, stK, tri1, triK = SearchTri(dev[0]), SearchTri(devK[0]), SearchTri(dev[0], True), SearchTri(devK[0], True)
+
+    def oracle_loop():
+        t0 = time.perf_counter()
+        co.triangulate(dev[0].host["k"], dev[0].host["q"], m12, st, sfac, *scales)
+        return (time.perf_counter() - t0) * 1e3
+
     for _ in range(args.warmup):
-        host_loop(); timed(dev); timed(devK)
+        host_loop(); timed(dev); timed(devK); timed([st1]); timed([stK]); oracle_loop()
     host, one, many, per = [], [], [], {}
     for _ in range(args.rounds):
         host += [host_loop() for _ in range(args.iters)]
@@ -114,11 +143,18 @@ def main():
         many += [timed(devK) for _ in range(args.iters)]
         for i, nm in enumerate(("points", "lines")):
             per.setdefault(nm, []).extend(timed([dev[i]]) for _ in range(args.iters))
+        for nm, o in (("search_triangulate_1kf", st1), ("search_triangulate_kfs", stK), ("triangulate_1kf", tri1), ("triangulate_kfs", triK)):
+            per.setdefault(nm, []).extend(timed([o]) for _ in range(args.iters))
+        per.setdefault("cpu_oracle_1kf", []).extend(oracle_loop() for _ in range(args.iters))
     med = lambda a: round(float(np.median(a)), 4)
     print(json.dumps(dict(tool="triangulation_batch_time", card=name, power_limit=plim, keypoints=len(pkf[0]["keys"]), keylines=N_LINES,
                           point_neighbours=N_POINT_NEIGH, line_neighbours=N_LINE_NEIGH, host_loop_ms=med(host), device_ms=med(one),
-                          device_launch_ms={k: med(v) for k, v in per.items()}, keyframes=args.keyframes,
-                          batched_keyframes_ms=med(many), speedup=round(med(host) / med(one), 1))))
+                          device_launch_ms={k: med(per[k]) for k in ("points", "lines")}, keyframes=args.keyframes,
+                          batched_keyframes_ms=med(many), speedup=round(med(host) / med(one), 1),
+                          point_pairs_1kf=int((m12 >= 0).sum()), new_points_1kf=int(oc[2].sum()),
+                          search_triangulate_1kf_ms=med(per["search_triangulate_1kf"]), search_triangulate_kfs_ms=med(per["search_triangulate_kfs"]),
+                          triangulate_1kf_ms=med(per["triangulate_1kf"]), triangulate_kfs_ms=med(per["triangulate_kfs"]),
+                          cpu_oracle_triangulate_1kf_ms=med(per["cpu_oracle_1kf"]))))
 
 
 if __name__ == "__main__":
