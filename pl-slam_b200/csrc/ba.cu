@@ -16,7 +16,7 @@
 
 #include "common.cuh"
 #include <mutex>
-#include "se3.cuh"
+#include "g2o.cuh"
 #include <algorithm>
 #include <climits>
 
@@ -110,6 +110,7 @@ struct BAArgs {
   __device__ __forceinline__ double* Xb() const { return ws<double>(B.L.Xb); }
   __device__ __forceinline__ double* err() const { return ws<double>(B.L.err); }
   __device__ __forceinline__ uint8_t* lvl() const { return ws<uint8_t>(B.L.lvl); }
+  __device__ __forceinline__ uint8_t& edge_lvl(int c) const { return lvl()[c < n_pe() ? c : n_pe() + ((c - n_pe()) >> 1)]; }   // by edge code
   __device__ __forceinline__ double* JA() const { return ws<double>(B.L.JA); }
   __device__ __forceinline__ double* JB() const { return ws<double>(B.L.JB); }
   __device__ __forceinline__ double* omr() const { return ws<double>(B.L.omr); }
@@ -156,15 +157,6 @@ __device__ __forceinline__ double block_max(BAShared& S, double v, int tid) {
   __syncthreads();
   return s;
 }
-__device__ __forceinline__ void inv3(const double* D, double lambda, double* Di) {
-  const double a = D[0] + lambda, b = D[1], c = D[2], d = D[3], e = D[4] + lambda, f = D[5], g = D[6], h = D[7], i = D[8] + lambda;
-  const double A = e * i - f * h, B = -(d * i - f * g), C = d * h - e * g;
-  const double id = 1.0 / (a * A + b * B + c * C);
-  Di[0] = A * id; Di[1] = -(b * i - c * h) * id; Di[2] = (b * f - c * e) * id;
-  Di[3] = B * id; Di[4] = (a * i - c * g) * id; Di[5] = -(a * f - c * d) * id;
-  Di[6] = C * id; Di[7] = -(a * h - b * g) * id; Di[8] = (a * e - b * d) * id;
-}
-
 __device__ __forceinline__ void edge_decode(const BAArgs& A, int code, int& kf, int& lm, int& dim, int& e, int& end) {
   if (code < A.n_pe()) { e = code; end = 0; dim = 2; kf = A.pe_kf()[e]; lm = A.pe_pt()[e]; }
   else { const int c = code - A.n_pe(); e = c >> 1; end = c & 1; dim = 1; kf = A.le_kf()[e]; lm = A.n_pt() + 2 * A.le_ln()[e] + end; }
@@ -173,30 +165,29 @@ __device__ __forceinline__ void cam_K(const BAArgs& A, int kf, int end_edge, dou
   if (end_edge) { for (int i = 0; i < 4; i++) k[i] = (double)A.K_end()[i]; }
   else { for (int i = 0; i < 4; i++) k[i] = (double)A.kf_K()[4 * kf + i]; }
 }
-__device__ __forceinline__ double line_err_at(const BAArgs& A, const SE3& T, const double* X, int e, int end) {
-  double c[3], k[4];
-  se3_map(T, X, c);
-  cam_K(A, A.le_kf()[e], end, k);
-  const double u = c[0] / c[2] * k[0] + k[2], v = c[1] / c[2] * k[1] + k[3];
-  return A.le_f()[3 * e] * u + A.le_f()[3 * e + 1] * v + A.le_f()[3 * e + 2];
+
+__device__ __forceinline__ int edge_lm(const BAArgs& A, int c) {
+  return c < A.n_pe() ? A.pe_pt()[c] : A.n_pt() + 2 * A.le_ln()[(c - A.n_pe()) >> 1] + ((c - A.n_pe()) & 1);
 }
+__device__ __forceinline__ int edge_kf(const BAArgs& A, int c) { return c < A.n_pe() ? A.pe_kf()[c] : A.le_kf()[(c - A.n_pe()) >> 1]; }
 
 // computeActiveErrors + activeRobustChi2
 __device__ double errors_and_chi2(const BAArgs& A, BAShared& S, bool p_robust, bool l_robust, int tid) {
-  const double kDeltaMono = (double)(float)sqrt(5.991), kDeltaLine = (double)(float)sqrt(3.84);
+  const double kDeltaMono = huber_delta_mono(), kDeltaLine = huber_delta_line();
   double chi = 0, r0, r1;
   for (int e = tid; e < A.n_pe(); e += BA_THREADS) if (!A.lvl()[e]) {
-    double c[3], k[4];
-    se3_map(A.T()[A.pe_kf()[e]], A.X() + 3 * A.pe_pt()[e], c);
+    double k[4], e0, e1;
     cam_K(A, A.pe_kf()[e], 0, k);
-    const double e0 = (double)A.pe_obs()[2 * e] - (c[0] / c[2] * k[0] + k[2]), e1 = (double)A.pe_obs()[2 * e + 1] - (c[1] / c[2] * k[1] + k[3]);
+    proj_error(A.T()[A.pe_kf()[e]], A.X() + 3 * A.pe_pt()[e], k, (double)A.pe_obs()[2 * e], (double)A.pe_obs()[2 * e + 1], e0, e1);
     A.err()[2 * e] = e0; A.err()[2 * e + 1] = e1;
     const double w = (double)A.pe_w()[e], c2 = e0 * (w * e0) + e1 * (w * e1);
     if (p_robust) { huber(c2, kDeltaMono, r0, r1); chi += r0; } else chi += c2;
   }
   for (int e = tid; e < A.n_le(); e += BA_THREADS) if (!A.lvl()[A.n_pe() + e])
     for (int end = 0; end < 2; end++) {
-      const double er = line_err_at(A, A.T()[A.le_kf()[e]], A.X() + 3 * (A.n_pt() + 2 * A.le_ln()[e] + end), e, end);
+      double k[4];
+      cam_K(A, A.le_kf()[e], end, k);
+      const double er = line_error(A.T()[A.le_kf()[e]], A.X() + 3 * (A.n_pt() + 2 * A.le_ln()[e] + end), k, A.le_f() + 3 * e);
       A.err()[2 * A.n_pe() + 2 * e + end] = er;
       const double c2 = er * (0.5 * er);
       if (l_robust) { huber(c2, kDeltaLine, r0, r1); chi += r0; } else chi += c2;
@@ -208,17 +199,17 @@ __device__ double errors_and_chi2(const BAArgs& A, BAShared& S, bool p_robust, b
 // to itself: keeping the LM loops rolled and this function out of line shrinks it from 81 k to 21 k SASS instructions but makes
 // the 20+40-keyframe window markedly slower, so the inlined, unrolled form stays.)
 __device__ int ba_optimize(const BAArgs& A, BAShared& S, int iterations, bool p_robust, bool l_robust, int tid) {
-  const double kDeltaMono = (double)(float)sqrt(5.991), kDeltaLine = (double)(float)sqrt(3.84);
+  const double kDeltaMono = huber_delta_mono(), kDeltaLine = huber_delta_line();
   const int n_lm = A.n_pt() + 2 * A.n_ln(), n_edges = A.n_pe() + 2 * A.n_le();
   // ---- active sets and slots (initializeOptimization)
   for (int k = tid; k < A.n_kf(); k += BA_THREADS) {
     int act = 0;
-    for (int j = A.kf_start()[k]; j < A.kf_start()[k + 1] && !act; j++) { int c = A.kf_edges()[j]; act = !A.lvl()[c < A.n_pe() ? c : A.n_pe() + ((c - A.n_pe()) >> 1)]; }
+    for (int j = A.kf_start()[k]; j < A.kf_start()[k + 1] && !act; j++) act = !A.edge_lvl(A.kf_edges()[j]);
     A.pose_slot()[k] = (act && !A.kf_fixed()[k]) ? 1 : -1;
   }
   for (int l = tid; l < n_lm; l += BA_THREADS) {
     int act = 0;
-    for (int j = A.lm_start()[l]; j < A.lm_start()[l + 1] && !act; j++) { int c = A.lm_edges()[j]; act = !A.lvl()[c < A.n_pe() ? c : A.n_pe() + ((c - A.n_pe()) >> 1)]; }
+    for (int j = A.lm_start()[l]; j < A.lm_start()[l + 1] && !act; j++) act = !A.edge_lvl(A.lm_edges()[j]);
     A.lm_slot()[l] = act ? 1 : -1;
   }
   __syncthreads();
@@ -241,49 +232,28 @@ __device__ int ba_optimize(const BAArgs& A, BAShared& S, int iterations, bool p_
     // ---- perturbed poses for the numeric (line) Jacobians
     if (A.n_le() > 0)
       for (int i = tid; i < A.n_kf() * 12; i += BA_THREADS) {
-        const int k = i / 12, r = i - k * 12, d = r >> 1;
-        double add[6] = {0, 0, 0, 0, 0, 0};
-        add[d] = (r & 1) ? -1e-9 : 1e-9;
-        const SE3 Tn = se3_mul(se3_exp(add), A.T()[k]);
-        if (r & 1) A.Tm()[k * 6 + d] = Tn; else A.Tp()[k * 6 + d] = Tn;
+        const int k = i / 12, r = i - k * 12;
+        const SE3 Tn = perturbed_pose(A.T()[k], r);
+        if (r & 1) A.Tm()[k * 6 + (r >> 1)] = Tn; else A.Tp()[k * 6 + (r >> 1)] = Tn;
       }
     __syncthreads();
     // ---- per-edge linearisation
     for (int code = tid; code < n_edges; code += BA_THREADS) {
       int kf, lm, dim, e, end;
       edge_decode(A, code, kf, lm, dim, e, end);
-      if (A.lvl()[code < A.n_pe() ? e : A.n_pe() + e]) continue;
+      if (A.edge_lvl(code)) continue;
       double* JA = A.JA() + 6 * (size_t)code; double* JB = A.JB() + 12 * (size_t)code;
-      double r0, r1 = 1.0;
+      double k[4], omr[2], wg;
+      cam_K(A, kf, end, k);
       if (dim == 2) {
-        const SE3 T = A.T()[kf];
-        double c[3], k[4], R[3][3];
-        se3_map(T, A.X() + 3 * lm, c); cam_K(A, kf, 0, k); quat_to_matrix(T.r, R);
-        const double x = c[0], y = c[1], z = c[2], z_2 = z * z, fx = k[0], fy = k[1];
-        const double t00 = fx, t02 = -x / z * fx, t11 = fy, t12 = -y / z * fy;
-        for (int j = 0; j < 3; j++) {
-          JA[j] = -1. / z * (t00 * R[0][j] + t02 * R[2][j]);
-          JA[3 + j] = -1. / z * (t11 * R[1][j] + t12 * R[2][j]);
-        }
-        JB[0] = x * y / z_2 * fx; JB[1] = -(1 + (x * x / z_2)) * fx; JB[2] = y / z * fx; JB[3] = -1. / z * fx; JB[4] = 0; JB[5] = x / z_2 * fx;
-        JB[6] = (1 + y * y / z_2) * fy; JB[7] = -x * y / z_2 * fy; JB[8] = -x / z * fy; JB[9] = 0; JB[10] = -1. / z * fy; JB[11] = y / z_2 * fy;
-        const double w = (double)A.pe_w()[e], e0 = A.err()[2 * e], e1 = A.err()[2 * e + 1];
-        double o0 = -(w * e0), o1 = -(w * e1), wg = w;
-        if (p_robust) { huber(e0 * (w * e0) + e1 * (w * e1), kDeltaMono, r0, r1); o0 *= r1; o1 *= r1; wg = r1 * w; }
-        A.omr()[2 * (size_t)code] = o0; A.omr()[2 * (size_t)code + 1] = o1; A.wgt()[code] = wg;
+        proj_jacobians(A.T()[kf], A.X() + 3 * lm, k, JA, JB);
+        edge_weights(2, (double)A.pe_w()[e], A.err() + 2 * e, p_robust, kDeltaMono, omr, wg);
       } else {
-        const double* X = A.X() + 3 * lm;
-        for (int d = 0; d < 3; d++) {
-          double Xp[3] = {X[0], X[1], X[2]}, Xm[3] = {X[0], X[1], X[2]};
-          Xp[d] += 1e-9; Xm[d] += -1e-9;
-          JA[d] = 5e8 * (line_err_at(A, A.T()[kf], Xp, e, end) - line_err_at(A, A.T()[kf], Xm, e, end));
-        }
-        for (int d = 0; d < 6; d++) JB[d] = 5e8 * (line_err_at(A, A.Tp()[kf * 6 + d], X, e, end) - line_err_at(A, A.Tm()[kf * 6 + d], X, e, end));
-        const double er = A.err()[2 * A.n_pe() + 2 * e + end], w = 0.5;
-        double o0 = -(w * er), wg = w;
-        if (l_robust) { huber(er * (w * er), kDeltaLine, r0, r1); o0 *= r1; wg = r1 * w; }
-        A.omr()[2 * (size_t)code] = o0; A.omr()[2 * (size_t)code + 1] = 0; A.wgt()[code] = wg;
+        line_point_jacobian(A.T()[kf], A.X() + 3 * lm, k, A.le_f() + 3 * e, JA);
+        line_pose_jacobian(A.Tp() + kf * 6, A.Tm() + kf * 6, A.X() + 3 * lm, k, A.le_f() + 3 * e, JB);
+        edge_weights(1, 0.5, A.err() + 2 * A.n_pe() + 2 * e + end, l_robust, kDeltaLine, omr, wg);
       }
+      A.omr()[2 * (size_t)code] = omr[0]; A.omr()[2 * (size_t)code + 1] = omr[1]; A.wgt()[code] = wg;
     }
     __syncthreads();
     // ---- landmark blocks (thread per landmark, edges in CSR order)
@@ -293,16 +263,8 @@ __device__ int ba_optimize(const BAArgs& A, BAShared& S, int iterations, bool p_
       double H[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0}, b[3] = {0, 0, 0};
       for (int j = A.lm_start()[l]; j < A.lm_start()[l + 1]; j++) {
         const int code = A.lm_edges()[j];
-        if (A.lvl()[code < A.n_pe() ? code : A.n_pe() + ((code - A.n_pe()) >> 1)]) continue;
-        const int dim = code < A.n_pe() ? 2 : 1;
-        const double* JA = A.JA() + 6 * (size_t)code;
-        const double wg = A.wgt()[code];
-        for (int a = 0; a < 3; a++) {
-          double s = 0;
-          for (int d = 0; d < dim; d++) s += JA[d * 3 + a] * A.omr()[2 * (size_t)code + d];
-          b[a] += s;
-          for (int c = 0; c < 3; c++) { double h = 0; for (int d = 0; d < dim; d++) h += JA[d * 3 + a] * wg * JA[d * 3 + c]; H[a * 3 + c] += h; }
-        }
+        if (A.edge_lvl(code)) continue;
+        add_landmark_block(code < A.n_pe() ? 2 : 1, A.JA() + 6 * (size_t)code, A.omr() + 2 * (size_t)code, A.wgt()[code], H, b);
       }
       for (int i = 0; i < 9; i++) A.Hll()[(size_t)ls * 9 + i] = H[i];
       for (int i = 0; i < 3; i++) A.bl()[(size_t)ls * 3 + i] = b[i];
@@ -317,14 +279,8 @@ __device__ int ba_optimize(const BAArgs& A, BAShared& S, int iterations, bool p_
       for (int i = 0; i < 27; i++) acc[i] = 0;
       for (int j = A.kf_start()[k] + lane; j < A.kf_start()[k + 1]; j += 32) {
         const int code = A.kf_edges()[j];
-        if (A.lvl()[code < A.n_pe() ? code : A.n_pe() + ((code - A.n_pe()) >> 1)]) continue;
-        const int dim = code < A.n_pe() ? 2 : 1;
-        const double* JB = A.JB() + 12 * (size_t)code;
-        const double wg = A.wgt()[code];
-        int q = 0;
-        for (int a = 0; a < 6; a++)
-          for (int c = a; c < 6; c++) { double h = 0; for (int d = 0; d < dim; d++) h += JB[d * 6 + a] * wg * JB[d * 6 + c]; acc[q++] += h; }
-        for (int a = 0; a < 6; a++) { double s = 0; for (int d = 0; d < dim; d++) s += JB[d * 6 + a] * A.omr()[2 * (size_t)code + d]; acc[21 + a] += s; }
+        if (A.edge_lvl(code)) continue;
+        add_pose_block(code < A.n_pe() ? 2 : 1, A.JB() + 12 * (size_t)code, A.omr() + 2 * (size_t)code, A.wgt()[code], acc);
       }
 #pragma unroll
       for (int i = 0; i < 27; i++) acc[i] = warp_sum(acc[i]);
@@ -340,7 +296,7 @@ __device__ int ba_optimize(const BAArgs& A, BAShared& S, int iterations, bool p_
       for (int i = tid; i < np * 6; i += BA_THREADS) md = fmax(md, fabs(A.Hpp()[(size_t)(i / 6) * 36 + (i % 6) * 7]));
       for (int i = tid; i < nl * 3; i += BA_THREADS) md = fmax(md, fabs(A.Hll()[(size_t)(i / 3) * 9 + (i % 3) * 4]));
       md = block_max(S, md, tid);
-      if (tid == 0) { S.lambda = 1e-5 * md; S.ni = 2; S.nBad = 0; }
+      if (tid == 0) lm_init(md, S.lambda, S.ni, S.nBad);
     }
     if (tid == 0) { S.rho = 0; S.qmax = 0; }
     __syncthreads();
@@ -371,22 +327,17 @@ __device__ int ba_optimize(const BAArgs& A, BAShared& S, int iterations, bool p_
         const double* Db = A.Dinvb() + (size_t)ls * 3;
         for (int j1 = A.lm_start()[l]; j1 < A.lm_start()[l + 1]; j1++) {
           const int c1 = A.lm_edges()[j1];
-          if (A.lvl()[c1 < A.n_pe() ? c1 : A.n_pe() + ((c1 - A.n_pe()) >> 1)]) continue;
-          const int k1 = c1 < A.n_pe() ? A.pe_kf()[c1] : A.le_kf()[(c1 - A.n_pe()) >> 1];
-          const int p1 = A.pose_slot()[k1];
+          if (A.edge_lvl(c1)) continue;
+          const int p1 = A.pose_slot()[edge_kf(A, c1)];
           if (p1 < 0) continue;
-          const int d1 = c1 < A.n_pe() ? 2 : 1;
-          const double *JA1 = A.JA() + 6 * (size_t)c1, *JB1 = A.JB() + 12 * (size_t)c1;
-          const double w1 = A.wgt()[c1];
-          double B1[18], BD[18];   // Hpl block = B^T w A (6x3); BD = Hpl * Dinv
-          for (int a = 0; a < 6; a++) for (int c = 0; c < 3; c++) { double h = 0; for (int d = 0; d < d1; d++) h += JB1[d * 6 + a] * w1 * JA1[d * 3 + c]; B1[a * 3 + c] = h; }
+          double B1[18], BD[18];   // Hpl block (6x3); BD = Hpl * Dinv
+          hpl_block(c1 < A.n_pe() ? 2 : 1, A.JA() + 6 * (size_t)c1, A.JB() + 12 * (size_t)c1, A.wgt()[c1], B1);
           for (int a = 0; a < 6; a++) for (int c = 0; c < 3; c++) BD[a * 3 + c] = B1[a * 3] * Di[c] + B1[a * 3 + 1] * Di[3 + c] + B1[a * 3 + 2] * Di[6 + c];
           for (int a = 0; a < 6; a++) atomicAdd(&A.bs()[p1 * 6 + a], -(B1[a * 3] * Db[0] + B1[a * 3 + 1] * Db[1] + B1[a * 3 + 2] * Db[2]));
           for (int j2 = A.lm_start()[l]; j2 < A.lm_start()[l + 1]; j2++) {
             const int c2 = A.lm_edges()[j2];
-            if (A.lvl()[c2 < A.n_pe() ? c2 : A.n_pe() + ((c2 - A.n_pe()) >> 1)]) continue;
-            const int k2 = c2 < A.n_pe() ? A.pe_kf()[c2] : A.le_kf()[(c2 - A.n_pe()) >> 1];
-            const int p2 = A.pose_slot()[k2];
+            if (A.edge_lvl(c2)) continue;
+            const int p2 = A.pose_slot()[edge_kf(A, c2)];
             if (p2 < 0) continue;
             const int d2 = c2 < A.n_pe() ? 2 : 1;
             const double *JA2 = A.JA() + 6 * (size_t)c2, *JB2 = A.JB() + 12 * (size_t)c2;
@@ -394,7 +345,7 @@ __device__ int ba_optimize(const BAArgs& A, BAShared& S, int iterations, bool p_
             for (int a = 0; a < 6; a++)
               for (int c = 0; c < 6; c++) {
                 double s = 0;
-                for (int m = 0; m < 3; m++) { double b2 = 0; for (int d = 0; d < d2; d++) b2 += JB2[d * 6 + c] * w2 * JA2[d * 3 + m]; s += BD[a * 3 + m] * b2; }
+                for (int m = 0; m < 3; m++) s += BD[a * 3 + m] * hpl_entry(d2, JA2, JB2, w2, c, m);
                 atomicAdd(&A.Hs()[(size_t)(p1 * 6 + a) * n + p2 * 6 + c], -s);
               }
           }
@@ -435,16 +386,15 @@ __device__ int ba_optimize(const BAArgs& A, BAShared& S, int iterations, bool p_
           double cl[3] = {A.bl()[(size_t)ls * 3], A.bl()[(size_t)ls * 3 + 1], A.bl()[(size_t)ls * 3 + 2]};
           for (int j1 = A.lm_start()[l]; j1 < A.lm_start()[l + 1]; j1++) {
             const int c1 = A.lm_edges()[j1];
-            if (A.lvl()[c1 < A.n_pe() ? c1 : A.n_pe() + ((c1 - A.n_pe()) >> 1)]) continue;
-            const int k1 = c1 < A.n_pe() ? A.pe_kf()[c1] : A.le_kf()[(c1 - A.n_pe()) >> 1];
-            const int p1 = A.pose_slot()[k1];
+            if (A.edge_lvl(c1)) continue;
+            const int p1 = A.pose_slot()[edge_kf(A, c1)];
             if (p1 < 0) continue;
             const int d1 = c1 < A.n_pe() ? 2 : 1;
             const double *JA1 = A.JA() + 6 * (size_t)c1, *JB1 = A.JB() + 12 * (size_t)c1;
             const double w1 = A.wgt()[c1];
             for (int c = 0; c < 3; c++) {
               double s = 0;
-              for (int a = 0; a < 6; a++) { double h = 0; for (int d = 0; d < d1; d++) h += JB1[d * 6 + a] * w1 * JA1[d * 3 + c]; s += h * A.x()[p1 * 6 + a]; }
+              for (int a = 0; a < 6; a++) s += hpl_entry(d1, JA1, JB1, w1, a, c) * A.x()[p1 * 6 + a];
               cl[c] -= s;
             }
           }
@@ -457,20 +407,15 @@ __device__ int ba_optimize(const BAArgs& A, BAShared& S, int iterations, bool p_
       for (int k = tid; k < A.n_kf(); k += BA_THREADS) if (A.pose_slot()[k] >= 0) A.T()[k] = se3_mul(se3_exp(A.x() + (size_t)A.pose_slot()[k] * 6), A.T()[k]);
       for (int l = tid; l < n_lm; l += BA_THREADS) if (A.lm_slot()[l] >= 0) for (int a = 0; a < 3; a++) A.X()[3 * l + a] += A.x()[n + A.lm_slot()[l] * 3 + a];
       __syncthreads();
-      double tempChi = errors_and_chi2(A, S, p_robust, l_robust, tid);
+      const double tempChi = errors_and_chi2(A, S, p_robust, l_robust, tid);
       double sc = 0;
       for (int i = tid; i < n; i += BA_THREADS) sc += A.x()[i] * (lambda * A.x()[i] + A.bp()[i]);
       for (int i = tid; i < nl * 3; i += BA_THREADS) sc += A.x()[n + i] * (lambda * A.x()[n + i] + A.bl()[i]);
       sc = block_sum(S, sc, tid);
       if (tid == 0) {
-        if (!S.ok2) tempChi = 1.7976931348623157e308;
-        double rho = (S.currentChi - tempChi) / (sc + 1e-3);
-        if (rho > 0 && isfinite(tempChi)) {
-          double alpha = 1. - pow((2 * rho - 1), 3.0);
-          alpha = fmin(alpha, 2. / 3.);
-          S.lambda *= fmax(1. / 3., alpha); S.ni = 2; S.currentChi = tempChi; S.flag = 0;
-        } else { S.lambda *= S.ni; S.ni *= 2; S.flag = 1; }
-        S.rho = rho; S.qmax++;
+        bool kept;
+        S.rho = lm_trial(S.ok2, tempChi, sc, S.lambda, S.ni, S.currentChi, kept);
+        S.flag = !kept; S.qmax++;
       }
       __syncthreads();
       if (S.flag) {   // rejected: restore the state
@@ -482,22 +427,20 @@ __device__ int ba_optimize(const BAArgs& A, BAShared& S, int iterations, bool p_
       __syncthreads();
       if (!again) break;
     }
-    if (tid == 0) {
-      int stop = 0;
-      if (S.qmax == 10 || S.rho == 0) stop = 1;
-      else { if ((S.iniChi - S.currentChi) * 1e3 < S.iniChi) S.nBad++; else S.nBad = 0; if (S.nBad >= 3) stop = 1; }
-      S.stop_it = stop;
-    }
+    if (tid == 0) S.stop_it = lm_stop(S.qmax, S.rho, S.iniChi, S.currentChi, S.nBad);
     __syncthreads();
     if (S.stop_it) break;
   }
   return done;
 }
 
-__device__ __forceinline__ int edge_lm(const BAArgs& A, int c) {
-  return c < A.n_pe() ? A.pe_pt()[c] : A.n_pt() + 2 * A.le_ln()[(c - A.n_pe()) >> 1] + ((c - A.n_pe()) & 1);
+// The reference's point gate (Optimizer.cc:1957-1964 marks level 1, :2010-2016 erases): chi2 over 5.991 or not in front of the camera
+__device__ __forceinline__ bool point_gated(const BAArgs& A, int e) {
+  const double w = (double)A.pe_w()[e], c2 = A.err()[2 * e] * (w * A.err()[2 * e]) + A.err()[2 * e + 1] * (w * A.err()[2 * e + 1]);
+  double c[3];
+  se3_map(A.T()[A.pe_kf()[e]], A.X() + 3 * A.pe_pt()[e], c);
+  return c2 > 5.991 || !(c[2] > 0.0);
 }
-__device__ __forceinline__ int edge_kf(const BAArgs& A, int c) { return c < A.n_pe() ? A.pe_kf()[c] : A.le_kf()[(c - A.n_pe()) >> 1]; }
 
 // a[0 .. n) -> its exclusive prefix sums, a contiguous chunk per thread
 __device__ void block_exclusive_scan(BAShared& S, int* a, int n, int tid) {
@@ -615,12 +558,7 @@ __global__ void __launch_bounds__(BA_THREADS) k_local_ba(const __grid_constant__
     __syncthreads();
     const bool more = !(A.stop() && *A.stop());
     if (more) {
-      for (int e = tid; e < A.n_pe(); e += BA_THREADS) {
-        const double w = (double)A.pe_w()[e], c2 = A.err()[2 * e] * (w * A.err()[2 * e]) + A.err()[2 * e + 1] * (w * A.err()[2 * e + 1]);
-        double c[3];
-        se3_map(A.T()[A.pe_kf()[e]], A.X() + 3 * A.pe_pt()[e], c);
-        if (c2 > 5.991 || !(c[2] > 0.0)) A.lvl()[e] = 1;
-      }
+      for (int e = tid; e < A.n_pe(); e += BA_THREADS) if (point_gated(A, e)) A.lvl()[e] = 1;
       for (int e = tid; e < A.n_le(); e += BA_THREADS) {
         const double a = A.err()[2 * A.n_pe() + 2 * e], b = A.err()[2 * A.n_pe() + 2 * e + 1];
         if (a * (0.5 * a) > 3.84 || b * (0.5 * b) > 3.84) A.lvl()[A.n_pe() + e] = 1;
@@ -629,12 +567,7 @@ __global__ void __launch_bounds__(BA_THREADS) k_local_ba(const __grid_constant__
       its += ba_optimize(A, S, 10, false, false, tid);
       __syncthreads();
     }
-    for (int e = tid; e < A.n_pe(); e += BA_THREADS) {
-      const double w = (double)A.pe_w()[e], c2 = A.err()[2 * e] * (w * A.err()[2 * e]) + A.err()[2 * e + 1] * (w * A.err()[2 * e + 1]);
-      double c[3];
-      se3_map(A.T()[A.pe_kf()[e]], A.X() + 3 * A.pe_pt()[e], c);
-      A.pe_erase()[e] = (c2 > 5.991 || !(c[2] > 0.0)) ? 1 : 0;
-    }
+    for (int e = tid; e < A.n_pe(); e += BA_THREADS) A.pe_erase()[e] = point_gated(A, e) ? 1 : 0;
     for (int e = tid; e < A.n_le(); e += BA_THREADS) {
       const double a = A.err()[2 * A.n_pe() + 2 * e];
       A.le_erase()[e] = (a * (0.5 * a) > 3.84) ? 1 : 0;           // START-point edge read twice (Optimizer.cc:2030-2031)

@@ -22,10 +22,9 @@
 // Sums over edges (chi2, the gain ratio's scale) are two-stage reductions with a fixed grid: deterministic as well.
 
 #include "common.cuh"
-#include "se3.cuh"
+#include "g2o.cuh"
 #include <algorithm>
 #include <cmath>
-#include <limits>
 #include <vector>
 
 namespace pl {
@@ -63,13 +62,6 @@ __device__ __forceinline__ double block_sum256(double v, double* red) {
 }
 
 __device__ __forceinline__ void cam_K(const G& A, int kf, double* k) { for (int i = 0; i < 4; i++) k[i] = (double)A.kf_K[4 * kf + i]; }
-__device__ __forceinline__ double line_err_at(const G& A, const SE3& T, const double* X, int kf, int e) {
-  double c[3], k[4];
-  se3_map(T, X, c);
-  cam_K(A, kf, k);
-  const double u = c[0] / c[2] * k[0] + k[2], v = c[1] / c[2] * k[1] + k[3];
-  return A.le_f[3 * e] * u + A.le_f[3 * e + 1] * v + A.le_f[3 * e + 2];
-}
 
 __global__ void k_gba_init(G A) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -84,18 +76,17 @@ __global__ void __launch_bounds__(RED_THREADS) k_gba_errors(G A) {
   double chi = 0, r0, r1;
   for (int code = blockIdx.x * RED_THREADS + threadIdx.x; code < A.n_edges; code += RED_BLOCKS * RED_THREADS) {
     const int kf = A.ed_kf[code], lm = A.ed_lm[code];
-    double c2;
+    double c2, k[4];
+    cam_K(A, kf, k);
     if (code < A.n_pe) {
-      double c[3], k[4];
-      se3_map(A.T[kf], A.X + 3 * lm, c);
-      cam_K(A, kf, k);
-      const double e0 = (double)A.pe_obs[2 * code] - (c[0] / c[2] * k[0] + k[2]), e1 = (double)A.pe_obs[2 * code + 1] - (c[1] / c[2] * k[1] + k[3]);
+      double e0, e1;
+      proj_error(A.T[kf], A.X + 3 * lm, k, (double)A.pe_obs[2 * code], (double)A.pe_obs[2 * code + 1], e0, e1);
       A.err[2 * (size_t)code] = e0; A.err[2 * (size_t)code + 1] = e1;
       const double w = (double)A.pe_w[code];
       c2 = e0 * (w * e0) + e1 * (w * e1);
       if (A.robust) { huber(c2, A.delta_p, r0, r1); c2 = r0; }
     } else {
-      const double er = line_err_at(A, A.T[kf], A.X + 3 * lm, kf, (code - A.n_pe) % A.n_le);
+      const double er = line_error(A.T[kf], A.X + 3 * lm, k, A.le_f + 3 * ((code - A.n_pe) % A.n_le));
       A.err[2 * (size_t)code] = er; A.err[2 * (size_t)code + 1] = 0;
       c2 = er * (A.info_line * er);
       if (A.robust) { huber(c2, A.delta_l, r0, r1); c2 = r0; }
@@ -137,11 +128,9 @@ __global__ void k_gba_reduce(G A, int slot, int is_max) {     // one thread: RED
 __global__ void k_gba_perturb(G A) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= A.n_kf * 12) return;
-  const int k = i / 12, r = i - k * 12, d = r >> 1;
-  double add[6] = {0, 0, 0, 0, 0, 0};
-  add[d] = (r & 1) ? -1e-9 : 1e-9;
-  const SE3 Tn = se3_mul(se3_exp(add), A.T[k]);
-  if (r & 1) A.Tm[k * 6 + d] = Tn; else A.Tp[k * 6 + d] = Tn;
+  const int k = i / 12, r = i - k * 12;
+  const SE3 Tn = perturbed_pose(A.T[k], r);
+  if (r & 1) A.Tm[k * 6 + (r >> 1)] = Tn; else A.Tp[k * 6 + (r >> 1)] = Tn;
 }
 
 __global__ void k_gba_linearize(G A) {
@@ -149,37 +138,18 @@ __global__ void k_gba_linearize(G A) {
   if (code >= A.n_edges) return;
   const int kf = A.ed_kf[code], lm = A.ed_lm[code];
   double* JA = A.JA + 6 * (size_t)code; double* JB = A.JB + 12 * (size_t)code;
-  double r0, r1 = 1.0;
+  double k[4], omr[2], wg;
+  cam_K(A, kf, k);
   if (code < A.n_pe) {
-    const SE3 T = A.T[kf];
-    double c[3], k[4], R[3][3];
-    se3_map(T, A.X + 3 * lm, c); cam_K(A, kf, k); quat_to_matrix(T.r, R);
-    const double x = c[0], y = c[1], z = c[2], z_2 = z * z, fx = k[0], fy = k[1];
-    const double t00 = fx, t02 = -x / z * fx, t11 = fy, t12 = -y / z * fy;
-    for (int j = 0; j < 3; j++) {
-      JA[j] = -1. / z * (t00 * R[0][j] + t02 * R[2][j]);
-      JA[3 + j] = -1. / z * (t11 * R[1][j] + t12 * R[2][j]);
-    }
-    JB[0] = x * y / z_2 * fx; JB[1] = -(1 + (x * x / z_2)) * fx; JB[2] = y / z * fx; JB[3] = -1. / z * fx; JB[4] = 0; JB[5] = x / z_2 * fx;
-    JB[6] = (1 + y * y / z_2) * fy; JB[7] = -x * y / z_2 * fy; JB[8] = -x / z * fy; JB[9] = 0; JB[10] = -1. / z * fy; JB[11] = y / z_2 * fy;
-    const double w = (double)A.pe_w[code], e0 = A.err[2 * (size_t)code], e1 = A.err[2 * (size_t)code + 1];
-    double o0 = -(w * e0), o1 = -(w * e1), wg = w;
-    if (A.robust) { huber(e0 * (w * e0) + e1 * (w * e1), A.delta_p, r0, r1); o0 *= r1; o1 *= r1; wg = r1 * w; }
-    A.omr[2 * (size_t)code] = o0; A.omr[2 * (size_t)code + 1] = o1; A.wgt[code] = wg;
+    proj_jacobians(A.T[kf], A.X + 3 * lm, k, JA, JB);
+    edge_weights(2, (double)A.pe_w[code], A.err + 2 * (size_t)code, A.robust, A.delta_p, omr, wg);
   } else {
-    const int e = (code - A.n_pe) % A.n_le;
-    const double* X = A.X + 3 * lm;
-    for (int d = 0; d < 3; d++) {
-      double Xp[3] = {X[0], X[1], X[2]}, Xm[3] = {X[0], X[1], X[2]};
-      Xp[d] += 1e-9; Xm[d] += -1e-9;
-      JA[d] = 5e8 * (line_err_at(A, A.T[kf], Xp, kf, e) - line_err_at(A, A.T[kf], Xm, kf, e));
-    }
-    for (int d = 0; d < 6; d++) JB[d] = 5e8 * (line_err_at(A, A.Tp[kf * 6 + d], X, kf, e) - line_err_at(A, A.Tm[kf * 6 + d], X, kf, e));
-    const double er = A.err[2 * (size_t)code], w = A.info_line;
-    double o0 = -(w * er), wg = w;
-    if (A.robust) { huber(er * (w * er), A.delta_l, r0, r1); o0 *= r1; wg = r1 * w; }
-    A.omr[2 * (size_t)code] = o0; A.omr[2 * (size_t)code + 1] = 0; A.wgt[code] = wg;
+    const double* f = A.le_f + 3 * ((code - A.n_pe) % A.n_le);
+    line_point_jacobian(A.T[kf], A.X + 3 * lm, k, f, JA);
+    line_pose_jacobian(A.Tp + kf * 6, A.Tm + kf * 6, A.X + 3 * lm, k, f, JB);
+    edge_weights(1, A.info_line, A.err + 2 * (size_t)code, A.robust, A.delta_l, omr, wg);
   }
+  A.omr[2 * (size_t)code] = omr[0]; A.omr[2 * (size_t)code + 1] = omr[1]; A.wgt[code] = wg;
 }
 
 __global__ void k_gba_lm_blocks(G A) {
@@ -189,15 +159,8 @@ __global__ void k_gba_lm_blocks(G A) {
   if (ls < 0) return;
   double H[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0}, b[3] = {0, 0, 0};
   for (int j = A.lm_start[l]; j < A.lm_start[l + 1]; j++) {
-    const int code = A.lm_edges[j], dim = code < A.n_pe ? 2 : 1;
-    const double* JA = A.JA + 6 * (size_t)code;
-    const double wg = A.wgt[code];
-    for (int a = 0; a < 3; a++) {
-      double s = 0;
-      for (int d = 0; d < dim; d++) s += JA[d * 3 + a] * A.omr[2 * (size_t)code + d];
-      b[a] += s;
-      for (int c = 0; c < 3; c++) { double h = 0; for (int d = 0; d < dim; d++) h += JA[d * 3 + a] * wg * JA[d * 3 + c]; H[a * 3 + c] += h; }
-    }
+    const int code = A.lm_edges[j];
+    add_landmark_block(code < A.n_pe ? 2 : 1, A.JA + 6 * (size_t)code, A.omr + 2 * (size_t)code, A.wgt[code], H, b);
   }
   for (int i = 0; i < 9; i++) A.Hll[(size_t)ls * 9 + i] = H[i];
   for (int i = 0; i < 3; i++) A.bl[(size_t)ls * 3 + i] = b[i];
@@ -212,13 +175,8 @@ __global__ void k_gba_pose_blocks(G A) {     // warp per keyframe
 #pragma unroll
   for (int i = 0; i < 27; i++) acc[i] = 0;
   for (int j = A.kf_start[k] + lane; j < A.kf_start[k + 1]; j += 32) {
-    const int code = A.kf_edges[j], dim = code < A.n_pe ? 2 : 1;
-    const double* JB = A.JB + 12 * (size_t)code;
-    const double wg = A.wgt[code];
-    int q = 0;
-    for (int a = 0; a < 6; a++)
-      for (int c = a; c < 6; c++) { double h = 0; for (int d = 0; d < dim; d++) h += JB[d * 6 + a] * wg * JB[d * 6 + c]; acc[q++] += h; }
-    for (int a = 0; a < 6; a++) { double s = 0; for (int d = 0; d < dim; d++) s += JB[d * 6 + a] * A.omr[2 * (size_t)code + d]; acc[21 + a] += s; }
+    const int code = A.kf_edges[j];
+    add_pose_block(code < A.n_pe ? 2 : 1, A.JB + 12 * (size_t)code, A.omr + 2 * (size_t)code, A.wgt[code], acc);
   }
 #pragma unroll
   for (int i = 0; i < 27; i++) acc[i] = warp_sum(acc[i]);
@@ -236,22 +194,14 @@ __global__ void k_gba_hpl(G A) {
   double W[18];
   for (int i = 0; i < 18; i++) W[i] = 0;
   for (int j = A.plb_start[b]; j < A.plb_start[b + 1]; j++) {
-    const int code = A.plb_edges[j], dim = code < A.n_pe ? 2 : 1;
-    const double *JA = A.JA + 6 * (size_t)code, *JB = A.JB + 12 * (size_t)code;
-    const double wg = A.wgt[code];
-    for (int a = 0; a < 6; a++) for (int c = 0; c < 3; c++) { double h = 0; for (int d = 0; d < dim; d++) h += JB[d * 6 + a] * wg * JA[d * 3 + c]; W[a * 3 + c] += h; }
+    const int code = A.plb_edges[j];
+    double We[18];
+    hpl_block(code < A.n_pe ? 2 : 1, A.JA + 6 * (size_t)code, A.JB + 12 * (size_t)code, A.wgt[code], We);
+    for (int i = 0; i < 18; i++) W[i] += We[i];
   }
   for (int i = 0; i < 18; i++) A.W[(size_t)b * 18 + i] = W[i];
 }
 
-__device__ __forceinline__ void inv3(const double* D, double lambda, double* Di) {
-  const double a = D[0] + lambda, b = D[1], c = D[2], d = D[3], e = D[4] + lambda, f = D[5], g = D[6], h = D[7], i = D[8] + lambda;
-  const double A = e * i - f * h, B = -(d * i - f * g), C = d * h - e * g;
-  const double id = 1.0 / (a * A + b * B + c * C);
-  Di[0] = A * id; Di[1] = -(b * i - c * h) * id; Di[2] = (b * f - c * e) * id;
-  Di[3] = B * id; Di[4] = (a * i - c * g) * id; Di[5] = -(a * f - c * d) * id;
-  Di[6] = C * id; Di[7] = -(a * h - b * g) * id; Di[8] = (a * e - b * d) * id;
-}
 __global__ void k_gba_dinv(G A, double lambda) {
   const int l = blockIdx.x * blockDim.x + threadIdx.x;
   if (l >= A.nl) return;
@@ -550,7 +500,7 @@ extern "C" int pl_global_ba(const PLBAProblem* p, int n_iterations, int robust, 
   float* d_pt_out = pt_Xw_out ? s.out(pt_Xw_out, 3 * (size_t)n_pt) : s.out<float>(3 * (size_t)n_pt);
   double* d_ln_out = ln_Xw_out ? s.out(ln_Xw_out, 6 * (size_t)n_ln) : s.out<double>(6 * (size_t)n_ln);
   A.robust = robust ? 1 : 0; A.info_line = 1.0;
-  A.delta_p = (double)(float)std::sqrt(5.99); A.delta_l = (double)(float)std::sqrt(3.84);
+  A.delta_p = huber_delta_gba(); A.delta_l = huber_delta_line();
   int ret = s.status(), done = 0;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   auto terminate = [&]() { return stop_flag_host && *(volatile const int*)stop_flag_host; };
@@ -574,7 +524,6 @@ extern "C" int pl_global_ba(const PLBAProblem* p, int n_iterations, int robust, 
       e = chi2(currentChi);
       if (e != cudaSuccess) break;
       const double iniChi = currentChi;
-      double tempChi = currentChi;
       if (n_le > 0) { k_gba_perturb<<<cdiv(n_kf * 12, 128), 128>>>(A); count_launch(); }
       k_gba_linearize<<<cdiv(n_edges, 128), 128>>>(A);
       k_gba_lm_blocks<<<cdiv(n_lm, 128), 128>>>(A);
@@ -586,7 +535,7 @@ extern "C" int pl_global_ba(const PLBAProblem* p, int n_iterations, int robust, 
         double md = 0;
         e = cudaMemcpy(&md, A.scal + 2, 8, cudaMemcpyDeviceToHost);
         if (e != cudaSuccess) break;
-        lambda = 1e-5 * md; ni = 2; nBad = 0;
+        lm_init(md, lambda, ni, nBad);
       }
       double rho = 0;
       int qmax = 0;
@@ -621,23 +570,15 @@ extern "C" int pl_global_ba(const PLBAProblem* p, int n_iterations, int robust, 
         e = cudaMemcpy(sc, A.scal, 16, cudaMemcpyDeviceToHost);
         if (e == cudaSuccess) e = cudaMemcpy(&bad, A.flag, 4, cudaMemcpyDeviceToHost);
         if (e != cudaSuccess) break;
-        tempChi = bad ? std::numeric_limits<double>::max() : sc[0];
-        rho = (currentChi - tempChi) / (sc[1] + 1e-3);
-        if (rho > 0 && std::isfinite(tempChi)) {
-          double alpha = 1. - std::pow((2 * rho - 1), 3);
-          alpha = std::min(alpha, 2. / 3.);
-          lambda *= std::max(1. / 3., alpha); ni = 2; currentChi = tempChi;
-        } else {
-          lambda *= ni; ni *= 2;
+        bool kept;
+        rho = lm_trial(!bad, sc[0], sc[1], lambda, ni, currentChi, kept);
+        if (!kept) {
           cudaMemcpyAsync(A.T, Tb, sizeof(SE3) * n_kf, cudaMemcpyDeviceToDevice, 0);
           cudaMemcpyAsync(A.X, Xb, 24 * (size_t)n_lm, cudaMemcpyDeviceToDevice, 0);
         }
         qmax++;
       } while (rho < 0 && qmax < 10 && !terminate());
-      if (e != cudaSuccess) break;
-      if (qmax == 10 || rho == 0) break;
-      if ((iniChi - currentChi) * 1e3 < iniChi) nBad++; else nBad = 0;
-      if (nBad >= 3) break;
+      if (e != cudaSuccess || lm_stop(qmax, rho, iniChi, currentChi, nBad)) break;
     }
     if (e == cudaSuccess) {
       k_gba_finish<<<cdiv(std::max(std::max(n_kf, n_pt), 6 * n_ln), 128), 128>>>(A, d_kf_out, d_pt_out, d_ln_out); count_launch();

@@ -16,7 +16,7 @@
 // step-control logic and broadcasts the decision.  No graph objects, no per-edge allocation, no virtual calls.
 
 #include "common.cuh"
-#include "se3.cuh"
+#include "g2o.cuh"
 #include <vector>
 
 namespace pl {
@@ -90,11 +90,11 @@ __device__ __forceinline__ void block_reduce(LmShared& S, double* v, int tid) {
 __global__ void __launch_bounds__(LM_THREADS) k_pose_opt(PoseArgs A) {
   __shared__ LmShared S;
   const int b = blockIdx.x, tid = threadIdx.x;
-  const double kDeltaMono = (double)(float)sqrt(5.991), kDeltaLine = (double)(float)sqrt(3.84);
+  const double kDeltaMono = huber_delta_mono(), kDeltaLine = huber_delta_line();
   int np = min(A.np[b], A.capP), nl = min(A.nl[b], A.capL);
   if (A.mode == 1) nl = 0;
   if (A.mode == 2) np = 0;
-  const double fx = A.K[4 * b], fy = A.K[4 * b + 1], cx = A.K[4 * b + 2], cy = A.K[4 * b + 3];
+  const double cam[4] = {A.K[4 * b], A.K[4 * b + 1], A.K[4 * b + 2], A.K[4 * b + 3]};
   const float* obs = A.pt_obs + (long long)b * A.capP * 2;
   const float* pw = A.pt_w + (long long)b * A.capP;
   const float* pX = A.pt_X + (long long)b * A.capP * 3;
@@ -115,17 +115,10 @@ __global__ void __launch_bounds__(LM_THREADS) k_pose_opt(PoseArgs A) {
   __syncthreads();
 
   auto point_err = [&](const SE3& T, int i, double& e0, double& e1) {
-    double X[3] = {(double)pX[3 * i], (double)pX[3 * i + 1], (double)pX[3 * i + 2]}, c[3];
-    se3_map(T, X, c);
-    e0 = (double)obs[2 * i] - (c[0] / c[2] * fx + cx);
-    e1 = (double)obs[2 * i + 1] - (c[1] / c[2] * fy + cy);
+    const double X[3] = {(double)pX[3 * i], (double)pX[3 * i + 1], (double)pX[3 * i + 2]};
+    proj_error(T, X, cam, (double)obs[2 * i], (double)obs[2 * i + 1], e0, e1);
   };
-  auto line_err = [&](const SE3& T, int i, int e) -> double {
-    double c[3];
-    se3_map(T, lX + 6 * i + 3 * e, c);
-    double u = c[0] / c[2] * fx + cx, v = c[1] / c[2] * fy + cy;
-    return lf[3 * i] * u + lf[3 * i + 1] * v + lf[3 * i + 2];
-  };
+  auto line_err = [&](const SE3& T, int i, int e) { return line_error(T, lX + 6 * i + 3 * e, cam, lf + 3 * i); };
   bool p_robust = true, l_robust = true;
   // computeActiveErrors + activeRobustChi2 at pose S.T; result in S.red[0][0]
   auto errors_and_chi2 = [&]() {
@@ -168,11 +161,8 @@ __global__ void __launch_bounds__(LM_THREADS) k_pose_opt(PoseArgs A) {
         errors_and_chi2();
         if (tid == 0) { S.currentChi = S.red[0][0]; S.iniChi = S.currentChi; }
         if (nl > 0 && tid < 12) {  // perturbed poses for the numeric Jacobian
-          double add[6] = {0, 0, 0, 0, 0, 0};
-          const int d = tid >> 1;
-          add[d] = (tid & 1) ? -1e-9 : 1e-9;
-          SE3 Tn = se3_mul(se3_exp(add), S.T);
-          if (tid & 1) S.Tm[d] = Tn; else S.Tp[d] = Tn;
+          const SE3 Tn = perturbed_pose(S.T, tid);
+          if (tid & 1) S.Tm[tid >> 1] = Tn; else S.Tp[tid >> 1] = Tn;
         }
         __syncthreads();
         // ---- buildSystem
@@ -183,9 +173,11 @@ __global__ void __launch_bounds__(LM_THREADS) k_pose_opt(PoseArgs A) {
           const SE3 T = S.T;
           double r0, r1;
           for (int i = tid; i < np; i += LM_THREADS) if (!pout[i]) {
+            // EdgeSE3ProjectXYZOnlyPose::linearizeOplus (types_six_dof_expmap.cpp:266-296) multiplies by invz and invz_2 where
+            // EdgeSE3ProjectXYZ (proj_jacobians, :103-139) divides by z and z_2; the two round differently, so this one stays.
             double X[3] = {(double)pX[3 * i], (double)pX[3 * i + 1], (double)pX[3 * i + 2]}, c[3];
             se3_map(T, X, c);
-            const double x = c[0], y = c[1], invz = 1.0 / c[2], invz_2 = invz * invz;
+            const double x = c[0], y = c[1], invz = 1.0 / c[2], invz_2 = invz * invz, fx = cam[0], fy = cam[1];
             double J0[6], J1[6];
             J0[0] = x * y * invz_2 * fx; J0[1] = -(1 + (x * x * invz_2)) * fx; J0[2] = y * invz * fx;
             J0[3] = -invz * fx; J0[4] = 0; J0[5] = x * invz_2 * fx;
@@ -206,8 +198,7 @@ __global__ void __launch_bounds__(LM_THREADS) k_pose_opt(PoseArgs A) {
           for (int i = tid; i < nl; i += LM_THREADS) if (!lout[i])
             for (int e = 0; e < 2; e++) {
               double J[6];
-#pragma unroll 1
-              for (int d = 0; d < 6; d++) J[d] = 5e8 * (line_err(S.Tp[d], i, e) - line_err(S.Tm[d], i, e));
+              line_pose_jacobian(S.Tp, S.Tm, lX + 6 * i + 3 * e, cam, lf + 3 * i, J);
               const double err = le[2 * i + e];
               r1 = 1.0;
               if (l_robust) huber(err * err, kDeltaLine, r0, r1);
@@ -229,7 +220,7 @@ __global__ void __launch_bounds__(LM_THREADS) k_pose_opt(PoseArgs A) {
           if (it == 0) {
             double md = 0;
             for (int j = 0; j < 6; j++) md = fmax(fabs(S.H[j * 6 + j]), md);
-            S.lambda = 1e-5 * md; S.ni = 2; S.nBad = 0;
+            lm_init(md, S.lambda, S.ni, S.nBad);
           }
           S.rho = 0; S.qmax = 0;
         }
@@ -245,36 +236,18 @@ __global__ void __launch_bounds__(LM_THREADS) k_pose_opt(PoseArgs A) {
           __syncthreads();
           errors_and_chi2();
           if (tid == 0) {
-            double tempChi = S.red[0][0];
-            if (!S.flag) tempChi = 1.7976931348623157e308;
-            double rho = S.currentChi - tempChi, scale = 0;
+            double scale = 0;
             for (int j = 0; j < 6; j++) scale += S.x[j] * (S.lambda * S.x[j] + S.b[j]);
-            scale += 1e-3;
-            rho /= scale;
-            if (rho > 0 && isfinite(tempChi)) {
-              double alpha = 1. - pow((2 * rho - 1), 3.0);
-              alpha = fmin(alpha, 2. / 3.);
-              double scaleFactor = fmax(1. / 3., alpha);
-              S.lambda *= scaleFactor; S.ni = 2; S.currentChi = tempChi;
-            } else {
-              S.lambda *= S.ni; S.ni *= 2; S.T = S.backup;
-            }
-            S.rho = rho;
+            bool kept;
+            S.rho = lm_trial(S.flag, S.red[0][0], scale, S.lambda, S.ni, S.currentChi, kept);
+            if (!kept) S.T = S.backup;
             S.qmax++;
-            S.flag = (rho < 0 && S.qmax < 10) ? 1 : 0;  // repeat?
+            S.flag = (S.rho < 0 && S.qmax < 10) ? 1 : 0;  // repeat?
           }
           __syncthreads();
           if (!S.flag) break;
         }
-        if (tid == 0) {
-          int stop = 0;
-          if (S.qmax == 10 || S.rho == 0) stop = 1;
-          else {
-            if ((S.iniChi - S.currentChi) * 1e3 < S.iniChi) S.nBad++; else S.nBad = 0;
-            if (S.nBad >= 3) stop = 1;
-          }
-          S.any = stop;
-        }
+        if (tid == 0) S.any = lm_stop(S.qmax, S.rho, S.iniChi, S.currentChi, S.nBad);
         __syncthreads();
         if (S.any) break;
       }

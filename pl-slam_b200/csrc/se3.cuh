@@ -1,5 +1,5 @@
 // SE3Quat arithmetic on the device (fp64): restated from Thirdparty/g2o/g2o/types/se3quat.h and the Eigen quaternion
-// routines it calls.  Shared by lm.cu (pose-only LM) and ba.cu (local bundle adjustment).
+// routines it calls.  Used by the optimisers: lm.cu, ba.cu and gba.cu, through g2o.cuh.
 #pragma once
 #include "common.cuh"
 namespace pl {
@@ -115,10 +115,5 @@ static __device__ void se3_to_cv(const SE3& s, float* T) {
   quat_to_matrix(s.r, R);
   for (int i = 0; i < 3; i++) { for (int j = 0; j < 3; j++) T[4 * i + j] = (float)R[i][j]; T[4 * i + 3] = (float)s.t[i]; }
   T[12] = 0; T[13] = 0; T[14] = 0; T[15] = 1;
-}
-__device__ __forceinline__ void huber(double e, double delta, double& rho0, double& rho1) {
-  double dsqr = delta * delta;
-  if (e <= dsqr) { rho0 = e; rho1 = 1.; }
-  else { double s = sqrt(e); rho0 = 2 * s * delta - dsqr; rho1 = delta / s; }
 }
 }  // namespace pl
