@@ -668,6 +668,61 @@ int pl_lsd_search_for_triangulation_dev(const PLTriLineKeyframes* kfs, const PLT
 int pl_orb_triangulate_dev(const PLTriKeyframes* kfs, const PLTriProblems* problems, const int* matches12, const int* search_status,
                            float scale_factor, float* x3D, int8_t* code, int* nnew, int* status, void* stream);
 
+/* The three-view triangulation of LocalMapping::CreateNewMapLinesConstraint (src/LocalMapping.cc:966-1439, monocular) for the
+ * matches of a pl_lsd_search_for_triangulation_dev batch, with the commit, enqueued on `stream`: kernels only, no allocation, copy
+ * or synchronisation, so the call can be captured into a CUDA graph together with the search.
+ *
+ * The geometry of the rows of the PLTriLineKeyframes table (same n_kf and cap): keylines [n_kf][cap] 68 B KeyLine records
+ * (KeyFrame::mvKeyLines), line_func [n_kf][cap][3] (mvKeyLineFunctions), Tcw [n_kf][16] (row-major), Ow [n_kf][3]
+ * (GetCameraCenter()), K [n_kf][4] (fx fy cx cy), and level_sigma2_line [nlevels] (mvLevelSigma2Line) shared by every keyframe.
+ * The caller guarantees 0 <= octave < nlevels for every keyline a triple reads. */
+typedef struct PLTriLineGeometry {
+  int n_kf, cap;
+  const void* keylines; const double* line_func;
+  const float* Tcw; const float* Ow; const float* K;
+  const float* level_sigma2_line; int nlevels;
+} PLTriLineGeometry;
+/* Most entries (vpNeighKFs) of one group; the commit keeps its taken state for kf_cur and each entry in shared memory. */
+#define PL_TRI_LINE_MAX_ENTRIES 16
+/* One group per current keyframe: kf_cur [G], entries entry_start[g] .. entry_start[g] + n_entries[g] - 1 of the entry list, and
+ * out_offset [G].  Entry e (TotalvMatchedIndices[e]) names its search problem entry_problem[e] (a problem of the search batch with
+ * kf1 = kf_cur), the POSITIONAL keyframe row entry_kf[e] (vpNeighKFs[e], which the reference pairs with entry e even when an
+ * earlier neighbour failed the baseline test and the entry holds another neighbour's matches) and entry_median_depth[e]
+ * (ComputeSceneMedianDepth(2) of vpNeighKFs[e], INTEGRATION.md).  n_out is the length of the slot outputs. */
+typedef struct PLTriLineGroups {
+  int G;
+  const int* kf_cur; const int* entry_start; const int* n_entries; const int* out_offset;   /* [G] */
+  int n_entry_list;
+  const int* entry_problem; const int* entry_kf; const float* entry_median_depth;          /* [n_entry_list] */
+  int n_out;
+} PLTriLineGroups;
+/* Group g with E entries and N = n[kf_cur[g]] keylines owns the slots out_offset[g] + pair(i, j) * N + ikl for the E (E - 1) / 2
+ * entry pairs i < j in the reference's order (pair(i, j) = i (2E - i - 1) / 2 + j - i - 1) and ikl < N.  code [n_out] gets the
+ * first reason in the reference's order: -1 no triple (idx1 or idx2 = -1, idx1 >= n[entry_kf[i]], idx2 >= n[entry_kf[j]], or an
+ * entry whose nmatches is 0); 1 one of the three slots (kf_cur: ikl, entry_kf[i]: idx1, entry_kf[j]: idx2) holds a map line at
+ * the snapshot has_ml; 2 one of them was taken by a line this call committed at an earlier slot; 3 the epipolar-plane test
+ * (|Result| > 0.996); 4 a zero norm; 5 CosSita > 0.0087; 6 vt(3,3) == 0; 7 parallax (>= 0.99998); 8 an end point too close
+ * (distance / median depth < 0.3); 9 too long (> 1); 10 behind a camera; 11, 12, 13 reprojection in view 1, 2, 3 (3.84 sigma^2 at
+ * the keyline's octave); 14, 15, 16 overlap in view 1, 2, 3 (0.85); 0 committed.  line3D [n_out][6] (start, end; world) is
+ * written for every slot whose triple passed all gates (code 0, and code 2 where the slots were taken); other slots keep theirs.
+ * Per group: nnew[g] = the number of committed slots; status[g], the first that applies: 2 an entry count negative or over
+ * PL_TRI_LINE_MAX_ENTRIES; 1 the entry range or an entry's problem index outside its table; the first nonzero search status of
+ * the entries' problems (passed through); 1 kf_cur, an entry's keyframe row or its problem's kf1 / kf2 outside the table; 2 one of
+ * their counts negative or over cap; 1 the group's output range outside n_out or a problem's match range outside the search's
+ * n_out; 3 an entry's problem has kf1 != kf_cur; 4 a matches entry outside -1 .. n[kf2] - 1 of its problem's kf2; else 0.  A
+ * group with a nonzero status writes nothing but status[g].
+ * The commit applies a group's slots in slot order (pairs in order, ikl ascending within a pair): a passed slot commits iff none of
+ * its three slots is taken, and takes them.  A caller creates the committed lines in slot order (INTEGRATION.md).  Groups are
+ * independent; their output ranges must not overlap.
+ * PL_ERR_ARG before anything is enqueued: the argument rules of pl_lsd_search_for_triangulation_dev on kfs and problems with
+ * (matches, nmatches, search_status) in the places of (matched_pairs, nmatches, status); and a NULL group list, G < 0,
+ * n_entry_list < 0 or n_out < 0; and, when G > 0, a NULL group or entry array, geometry, keylines, line_func, Tcw, Ow, K or
+ * level_sigma2_line, nlevels < 1, geometry rows other than the table's, a NULL nnew or status, or a NULL code or line3D when
+ * n_out > 0.  G = 0 enqueues nothing. */
+int pl_lsd_triangulate_dev(const PLTriLineKeyframes* kfs, const PLTriLineGeometry* geom, const PLTriProblems* problems,
+                           const int* matches, const int* nmatches, const int* search_status, const PLTriLineGroups* groups,
+                           int8_t* code, float* line3D, int* nnew, int* status, void* stream);
+
 /* ------------------------------------------------------------------ tracking a batch of frames against a fixed map
  * Tracking::TrackLocalMapWithLines (src/Tracking.cc:1491-1562) with SearchLocalPoints (:1751-1801) and SearchLocalLines
  * (:1803-1855), in localisation mode (mbOnlyTracking), for B frames at once; every intermediate stays on the device.

@@ -1235,6 +1235,19 @@ class PLTriLineKeyframes(C.Structure):
     _fields_ = [("n_kf", C.c_int), ("cap", C.c_int), ("ldesc", vp), ("has_ml", vp), ("n", vp)]
 
 
+class PLTriLineGeometry(C.Structure):
+    _fields_ = [("n_kf", C.c_int), ("cap", C.c_int), ("keylines", vp), ("line_func", vp), ("Tcw", vp), ("Ow", vp), ("K", vp),
+                ("level_sigma2_line", vp), ("nlevels", C.c_int)]
+
+
+class PLTriLineGroups(C.Structure):
+    _fields_ = [("G", C.c_int), ("kf_cur", vp), ("entry_start", vp), ("n_entries", vp), ("out_offset", vp), ("n_entry_list", C.c_int),
+                ("entry_problem", vp), ("entry_kf", vp), ("entry_median_depth", vp), ("n_out", C.c_int)]
+
+
+TRI_LINE_MAX_ENTRIES = 16     # PL_TRI_LINE_MAX_ENTRIES
+
+
 def _tri_lib():
     L = lib()
     if not getattr(L, "_tri_types", False):
@@ -1242,18 +1255,27 @@ def _tri_lib():
         L.pl_lsd_search_for_triangulation_dev.argtypes = ([C.POINTER(PLTriLineKeyframes), C.POINTER(PLTriProblems), C.c_float, C.c_float,
                                                             C.c_int] + [vp] * 4)
         L.pl_orb_triangulate_dev.argtypes = [C.POINTER(PLTriKeyframes), C.POINTER(PLTriProblems), vp, vp, C.c_float] + [vp] * 5
+        L.pl_lsd_triangulate_dev.argtypes = ([C.POINTER(PLTriLineKeyframes), C.POINTER(PLTriLineGeometry), C.POINTER(PLTriProblems)]
+                                             + [vp] * 3 + [C.POINTER(PLTriLineGroups)] + [vp] * 5)
         L._tri_types = True
     return L
 
 
 def pack_tri_keyframes(keyframes, lines=False, cap=None, cap_nodes=None):
     """Keyframes (dicts: keys [n] KP_DTYPE, desc [n][32], has_mp [n], fv (DBoW2 FeatureVector: dict node -> feature indices), Tcw
-    [16], Ow [3], K [4] for points; ldesc [n][32], has_ml [n] for lines) -> host arrays in the [n_kf][cap] layouts of PLTriKeyframes /
-    PLTriLineKeyframes.  cap / cap_nodes default to the largest count (at least 1); rows past a keyframe's count are zero."""
+    [16], Ow [3], K [4] for points; ldesc [n][32], has_ml [n] for lines, and for the line triangulation keylines [n] KEYLINE_DTYPE,
+    line_func [n][3], Tcw, Ow, K) -> host arrays in the [n_kf][cap] layouts of PLTriKeyframes / PLTriLineKeyframes (and
+    PLTriLineGeometry when every keyframe carries keylines).  cap / cap_nodes default to the largest count (at least 1); rows past a
+    keyframe's count are zero."""
     if lines:
         ldesc, n, cap = _pad_rows([k["ldesc"] for k in keyframes], np.uint8, (32,), cap, "keylines")
         has_ml, _, _ = _pad_rows([k["has_ml"] for k in keyframes], np.uint8, (), cap, "keylines")
-        return dict(ldesc=ldesc, has_ml=has_ml, n=n, cap=cap)
+        out = dict(ldesc=ldesc, has_ml=has_ml, n=n, cap=cap)
+        if keyframes and all("keylines" in k for k in keyframes):
+            out["keylines"], _, _ = _pad_rows([k["keylines"] for k in keyframes], KEYLINE_DTYPE, (), cap, "keylines")
+            out["line_func"], _, _ = _pad_rows([k["line_func"] for k in keyframes], np.float64, (3,), cap, "keylines")
+            out.update(_camera_rows(keyframes, Tcw=16, Ow=3, K=4))
+        return out
     keys, n, cap = _pad_rows([k["keys"] for k in keyframes], KP_DTYPE, (), cap, "keypoints")
     desc, _, _ = _pad_rows([k["desc"] for k in keyframes], np.uint8, (32,), cap, "keypoints")
     has_mp, _, _ = _pad_rows([k["has_mp"] for k in keyframes], np.uint8, (), cap, "keypoints")
@@ -1278,6 +1300,23 @@ def pack_tri_problems(problems, counts):
     return dict(P=P, kf1=kf1, kf2=kf2, F12=F12, out_offset=out_offset, n_out=int(n.sum()), count=n)
 
 
+def pack_tri_line_groups(groups, counts):
+    """Line triangulation groups (dicts: kf_cur, entries = [(problem, keyframe row, median depth), ...] in TotalvMatchedIndices'
+    order) -> host arrays of PLTriLineGroups; counts [n_kf] = the keyframes' n.  The groups' entries and outputs are packed end to
+    end: group g owns E (E - 1) / 2 * n[kf_cur] slots after those of group g - 1 (none when kf_cur lies outside the table)."""
+    G = len(groups)
+    kf_cur = np.array([int(g["kf_cur"]) for g in groups], np.int32)
+    n_entries = np.array([len(g["entries"]) for g in groups], np.int32)
+    entry_start = np.concatenate([[0], np.cumsum(n_entries)[:-1]]).astype(np.int32) if G else np.zeros(0, np.int32)
+    ent = [e for g in groups for e in g["entries"]]
+    n = np.array([(counts[k] if 0 <= k < len(counts) else 0) * (E * (E - 1) // 2) for k, E in zip(kf_cur, n_entries)], np.int64)
+    out_offset = np.concatenate([[0], np.cumsum(n)[:-1]]).astype(np.int32) if G else np.zeros(0, np.int32)
+    return dict(G=G, kf_cur=kf_cur, entry_start=entry_start, n_entries=n_entries, out_offset=out_offset,
+                entry_problem=np.array([int(e[0]) for e in ent], np.int32), entry_kf=np.array([int(e[1]) for e in ent], np.int32),
+                entry_median_depth=np.array([float(e[2]) for e in ent], np.float32), n_out=int(n.sum()),
+                count=n.astype(np.int32), n_cur=np.array([counts[k] if 0 <= k < len(counts) else 0 for k in kf_cur], np.int32))
+
+
 class TriangulationProblems:
     """A batch of triangulation searches on the device for pl_orb_search_for_triangulation_dev (lines=False) or
     pl_lsd_search_for_triangulation_dev (lines=True): the constructor packs the keyframe table and the problems (pack_tri_keyframes,
@@ -1289,9 +1328,15 @@ class TriangulationProblems:
     Points also triangulate (LocalMapping::CreateNewMapPoints): triangulate() enqueues pl_orb_triangulate_dev on the search's device
     outputs, which it reads where run() left them, and triangulated() returns one dict per problem: code (numpy int8 [n[kf1]]: -1 no
     pair, 0 committed, 1 dropped at commit, 2 .. 8 the gate that rejected it), x3D ([n[kf1]][3], written for codes 0 and 1), nnew and
-    status."""
+    status.
 
-    def __init__(self, keyframes, problems, scales=None, lines=False, options=0, out_fill=-7):
+    Lines triangulate too (LocalMapping::CreateNewMapLinesConstraint) when the keyframes carry keylines, line_func, Tcw, Ow and K
+    and `groups` are given (see pack_tri_line_groups; scales = level_sigma2_line): triangulate() enqueues pl_lsd_triangulate_dev and
+    triangulated() returns one dict per group: code (numpy int8 [E (E - 1) / 2][n[kf_cur]], one row per entry pair in the
+    reference's order, -1 .. 16 as plslam_b200.h lists them), line3D ([pairs][n[kf_cur]][6], written where the triple passed every
+    gate), pairs [(i, j)], nnew and status."""
+
+    def __init__(self, keyframes, problems, scales=None, lines=False, options=0, out_fill=-7, groups=None):
         import torch
         self.lines, self.options = lines, options
         k = pack_tri_keyframes(keyframes, lines)
@@ -1313,11 +1358,29 @@ class TriangulationProblems:
                                 nnew=torch.full((max(self.P, 1),), out_fill, dtype=torch.int32, device="cuda"),
                                 tri_status=torch.full((max(self.P, 1),), out_fill, dtype=torch.int32, device="cuda"))
             self.scale_factors = np.asarray(scales[0], np.float32)
+        if lines and groups is not None:
+            assert scales is not None, "the line triangulation needs scales = level_sigma2_line (mvLevelSigma2Line)"
+            gr = pack_tri_line_groups(groups, k["n"])
+            self.host["g"] = gr
+            self.inputs.update({f"g_{n}": _to_device(v) for n, v in gr.items() if isinstance(v, np.ndarray)})
+            self.inputs["level_sigma2_line"] = _to_device(np.asarray(scales, np.float32).reshape(-1))
+            n_out, G = max(gr["n_out"], 1), max(gr["G"], 1)
+            self.outputs.update(code=torch.full((n_out,), out_fill, dtype=torch.int8, device="cuda"),
+                                line3D=torch.full((n_out, 6), float("nan"), dtype=torch.float32, device="cuda"),
+                                nnew=torch.full((G,), out_fill, dtype=torch.int32, device="cuda"),
+                                tri_status=torch.full((G,), out_fill, dtype=torch.int32, device="cuda"))
         i = lambda n: self.inputs[n].data_ptr()
         self._q = PLTriProblems(self.P, i("q_kf1"), i("q_kf2"), None if lines else i("q_F12"), i("q_out_offset"), q["n_out"])
         n_kf = len(keyframes)
         if lines:
             self._k = PLTriLineKeyframes(n_kf, k["cap"], i("k_ldesc"), i("k_has_ml"), i("k_n"))
+            if "g_kf_cur" in self.inputs:
+                gr = self.host["g"]
+                self._geom = PLTriLineGeometry(n_kf, k["cap"], i("k_keylines"), i("k_line_func"), i("k_Tcw"), i("k_Ow"), i("k_K"),
+                                               i("level_sigma2_line"), int(self.inputs["level_sigma2_line"].numel()))
+                self._g = PLTriLineGroups(gr["G"], i("g_kf_cur"), i("g_entry_start"), i("g_n_entries"), i("g_out_offset"),
+                                          len(gr["entry_kf"]), i("g_entry_problem"), i("g_entry_kf"), i("g_entry_median_depth"),
+                                          gr["n_out"])
         else:
             self._k = PLTriKeyframes(n_kf, k["cap"], k["cap_nodes"], i("k_keys_un"), i("k_desc"), i("k_has_mp"), i("k_n"), i("k_fv_nodes"),
                                      i("k_fv_start"), i("k_fv_items"), i("k_nn"), i("k_Tcw"), i("k_Ow"), i("k_K"), i("scale_factors"),
@@ -1338,9 +1401,16 @@ class TriangulationProblems:
                                                         o["nmatches"], o["status"], s))
 
     def triangulate(self, stream=None, scale_factor=None):
-        """pl_orb_triangulate_dev on `stream` after run(): enqueues, does not wait.  scale_factor: KF1's mfScaleFactor (default
-        scale_factors[1], which a single-level table does not have)."""
-        assert not self.lines, "the line searches have no triangulation here"
+        """pl_orb_triangulate_dev (points) or pl_lsd_triangulate_dev (lines) on `stream` after run(): enqueues, does not wait.
+        scale_factor (points): KF1's mfScaleFactor (default scale_factors[1], which a single-level table does not have)."""
+        if self.lines:
+            assert "g_kf_cur" in self.inputs, "the line triangulation needs groups and the keyframes' geometry"
+            s = None if stream is None else stream.cuda_stream
+            o = {n: t.data_ptr() for n, t in self.outputs.items()}
+            check(_tri_lib().pl_lsd_triangulate_dev(C.byref(self._k), C.byref(self._geom), C.byref(self._q), o["matches"],
+                                                    o["nmatches"], o["status"], C.byref(self._g), o["code"], o["line3D"], o["nnew"],
+                                                    o["tri_status"], s))
+            return
         if scale_factor is None:
             assert len(self.scale_factors) > 1, "nlevels == 1: pass the keyframe's mfScaleFactor"
             scale_factor = float(self.scale_factors[1])
@@ -1353,6 +1423,18 @@ class TriangulationProblems:
         import torch
         torch.cuda.synchronize()
         h = {n: t.cpu().numpy() for n, t in self.outputs.items()}
+        if self.lines:
+            gr = self.host["g"]
+            res = []
+            for g in range(gr["G"]):
+                E, n = int(gr["n_entries"][g]), int(gr["n_cur"][g])
+                a, c = int(gr["out_offset"][g]), int(gr["count"][g])
+                np_ = E * (E - 1) // 2
+                res.append(dict(code=h["code"][a:a + c].reshape(np_, n).copy() if c else np.zeros((np_, n), np.int8),
+                                line3D=h["line3D"][a:a + c].reshape(np_, n, 6).copy() if c else np.zeros((np_, n, 6), np.float32),
+                                pairs=[(i, j) for i in range(E) for j in range(i + 1, E)] if np_ else [],
+                                nnew=int(h["nnew"][g]), status=int(h["tri_status"][g])))
+            return res
         q = self.host["q"]
         sl = lambda p: slice(q["out_offset"][p], q["out_offset"][p] + q["count"][p])
         return [dict(code=h["code"][sl(p)].copy(), x3D=h["x3D"][sl(p)].copy(), nnew=int(h["nnew"][p]), status=int(h["tri_status"][p]))

@@ -1492,13 +1492,25 @@ static int lsd_tri_launch(const PLTriLineKeyframes& K, const PLTriProblems& Q, f
   return PL_OK;
 }
 
-extern "C" int pl_lsd_search_for_triangulation_dev(const PLTriLineKeyframes* kfs, const PLTriProblems* problems, float th, float nnratio,
-                                                   int is_double, int* matched_pairs, int* nmatches, int* status, void* stream) {
-  PL_TRY(tri_problems_ok(problems, false, matched_pairs, nmatches, status));
-  if (problems->P == 0) return PL_OK;
+int pl::lsd_tri_table_ok(const PLTriLineKeyframes* kfs) {
   PL_ARG(kfs);
   const PLTriLineKeyframes& K = *kfs;
   PL_ARG(K.n_kf >= 1 && K.cap >= 1 && K.cap < 32000 && (long long)K.n_kf * K.cap <= INT_MAX && K.ldesc && K.has_ml && K.n);
+  return PL_OK;
+}
+
+int pl::lsd_tri_args_ok(const PLTriLineKeyframes* kfs, const PLTriProblems* problems, const void* match, const void* nmatches,
+                        const void* status) {
+  PL_TRY(tri_problems_ok(problems, false, match, nmatches, status));
+  if (problems->P == 0) return PL_OK;
+  return lsd_tri_table_ok(kfs);
+}
+
+extern "C" int pl_lsd_search_for_triangulation_dev(const PLTriLineKeyframes* kfs, const PLTriProblems* problems, float th, float nnratio,
+                                                   int is_double, int* matched_pairs, int* nmatches, int* status, void* stream) {
+  PL_TRY(lsd_tri_args_ok(kfs, problems, matched_pairs, nmatches, status));
+  if (problems->P == 0) return PL_OK;
+  const PLTriLineKeyframes& K = *kfs;
   PL_TRY(require_device());
   PL_TRY(search_double_fits_for((const void*)k_lsd_search_triangulation, "k_lsd_search_triangulation", K.cap, K.cap));
   return lsd_tri_launch(K, *problems, th, nnratio, is_double ? 1 : 0, search_double_smem(K.cap, K.cap), matched_pairs, nmatches,

@@ -20,6 +20,11 @@ int search_double_fits(int cap1, int cap2);
 // per-problem outputs.  P = 0 passes without looking at the keyframe table.
 int orb_tri_args_ok(const PLTriKeyframes* kfs, const PLTriProblems* problems, const void* match, const void* nmatches,
                     const void* status);
+// The same for pl_lsd_search_for_triangulation_dev, which pl_lsd_triangulate_dev applies to its table and problems;
+// lsd_tri_table_ok is its part on the keyframe table alone.
+int lsd_tri_table_ok(const PLTriLineKeyframes* kfs);
+int lsd_tri_args_ok(const PLTriLineKeyframes* kfs, const PLTriProblems* problems, const void* match, const void* nmatches,
+                    const void* status);
 int search_by_projection_last_launch(const PLKeyPoint* keys_cur, const uint8_t* desc_cur, const int* n_cur, int cap, int B,
                                      const float* bounds, const float* Tcw, const float* K, const float* scale_factors, int nlevels,
                                      const int* n_last, int cap_last, const uint8_t* last_valid, const float* last_pos,

@@ -11,7 +11,10 @@ against its 20 best covisible neighbours for points (CreateNewMapPoints, ORBmatc
   point search + triangulation: pl_orb_search_for_triangulation_dev then pl_orb_triangulate_dev (the gates and the neighbour-order
           commit) for one keyframe's 20 problems and for --keyframes keyframes', three launches on one stream, CUDA events around
           them; the triangulation launches alone as well;
-  CPU oracle: tests/cnmp_oracle.py's triangulate (numpy, vectorised over the pairs) on the same search outputs, a CPU time.
+  CPU oracle: tests/cnmp_oracle.py's triangulate (numpy, vectorised over the pairs) on the same search outputs, a CPU time;
+  line search + triangulation: pl_lsd_search_for_triangulation_dev then pl_lsd_triangulate_dev (CreateNewMapLinesConstraint's
+          three-view gates and commit, 45 entry pairs) for one current keyframe of about 230 keylines against 10 neighbours of the
+          tests/cnml_scene.py geometry, and for --keyframes such keyframes in one call; the triangulation launches alone as well.
 After --warmup calls, --rounds rounds alternate the forms; each number is the median over the timed calls.  Prints one JSON line,
 with the card's name and power limit read in the same run.
 
@@ -134,8 +137,37 @@ def main():
         co.triangulate(dev[0].host["k"], dev[0].host["q"], m12, st, sfac, *scales)
         return (time.perf_counter() - t0) * 1e3
 
+    # lines: current keyframes 0 .. K-1 of a scene with 10 neighbours after them, one group each, entries in neighbour order
+    import cnml_oracle as cno
+    import cnml_scene as cs
+    lsc = cs.scene(seed=7, n_seg=300, n_clutter=30, n_kf=args.keyframes + N_LINE_NEIGH)
+    nb = list(range(args.keyframes, args.keyframes + N_LINE_NEIGH))
+    lgroup = lambda c, p0: dict(kf_cur=c, entries=[(p0 + e, j, lsc["medians"][j]) for e, j in enumerate(nb)])
+    ltri = [pl.TriangulationProblems(lsc["kfs"], [(0, j) for j in nb], lsc["level_sigma2_line"], lines=True, options=lopt,
+                                     groups=[lgroup(0, 0)]),
+            pl.TriangulationProblems(lsc["kfs"], [(c, j) for c in range(args.keyframes) for j in nb], lsc["level_sigma2_line"],
+                                     lines=True, options=lopt, groups=[lgroup(c, c * N_LINE_NEIGH) for c in range(args.keyframes)])]
+    ltri[0].run(); ltri[0].triangulate()
+    lt = ltri[0].triangulated()
+    h = {k: v.cpu().numpy() for k, v in ltri[0].outputs.items()}
+    q0 = ltri[0].host["q"]
+    lo = cno.triangulate_lines(ltri[0].host["k"], q0, ltri[0].host["g"], h["matches"][:q0["n_out"]], h["nmatches"][:ltri[0].P],
+                               h["status"][:ltri[0].P], lsc["level_sigma2_line"])
+    assert np.array_equal(lt[0]["code"].ravel(), lo[0]) and lt[0]["nnew"] == lo[2][0]
+
+    class LineTri:
+        def __init__(self, b, only_tri=False):
+            self.b, self.only_tri = b, only_tri
+
+        def run(self, stream):
+            if not self.only_tri:
+                self.b.run(stream)
+            self.b.triangulate(stream)
+    lst1, lstK, ltri1, ltriK = LineTri(ltri[0]), LineTri(ltri[1]), LineTri(ltri[0], True), LineTri(ltri[1], True)
+
     for _ in range(args.warmup):
         host_loop(); timed(dev); timed(devK); timed([st1]); timed([stK]); oracle_loop()
+        timed([lst1]); timed([lstK])
     host, one, many, per = [], [], [], {}
     for _ in range(args.rounds):
         host += [host_loop() for _ in range(args.iters)]
@@ -146,6 +178,9 @@ def main():
         for nm, o in (("search_triangulate_1kf", st1), ("search_triangulate_kfs", stK), ("triangulate_1kf", tri1), ("triangulate_kfs", triK)):
             per.setdefault(nm, []).extend(timed([o]) for _ in range(args.iters))
         per.setdefault("cpu_oracle_1kf", []).extend(oracle_loop() for _ in range(args.iters))
+        for nm, o in (("line_search_triangulate_1kf", lst1), ("line_search_triangulate_kfs", lstK), ("line_triangulate_1kf", ltri1),
+                      ("line_triangulate_kfs", ltriK)):
+            per.setdefault(nm, []).extend(timed([o]) for _ in range(args.iters))
     med = lambda a: round(float(np.median(a)), 4)
     print(json.dumps(dict(tool="triangulation_batch_time", card=name, power_limit=plim, keypoints=len(pkf[0]["keys"]), keylines=N_LINES,
                           point_neighbours=N_POINT_NEIGH, line_neighbours=N_LINE_NEIGH, host_loop_ms=med(host), device_ms=med(one),
@@ -154,7 +189,11 @@ def main():
                           point_pairs_1kf=int((m12 >= 0).sum()), new_points_1kf=int(oc[2].sum()),
                           search_triangulate_1kf_ms=med(per["search_triangulate_1kf"]), search_triangulate_kfs_ms=med(per["search_triangulate_kfs"]),
                           triangulate_1kf_ms=med(per["triangulate_1kf"]), triangulate_kfs_ms=med(per["triangulate_kfs"]),
-                          cpu_oracle_triangulate_1kf_ms=med(per["cpu_oracle_1kf"]))))
+                          cpu_oracle_triangulate_1kf_ms=med(per["cpu_oracle_1kf"]),
+                          line_keylines_1kf=len(lsc["kfs"][0]["keylines"]), new_lines_1kf=int(lo[2][0]),
+                          line_search_triangulate_1kf_ms=med(per["line_search_triangulate_1kf"]),
+                          line_search_triangulate_kfs_ms=med(per["line_search_triangulate_kfs"]),
+                          line_triangulate_1kf_ms=med(per["line_triangulate_1kf"]), line_triangulate_kfs_ms=med(per["line_triangulate_kfs"]))))
 
 
 if __name__ == "__main__":
