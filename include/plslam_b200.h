@@ -723,6 +723,50 @@ int pl_lsd_triangulate_dev(const PLTriLineKeyframes* kfs, const PLTriLineGeometr
                            const int* matches, const int* nmatches, const int* search_status, const PLTriLineGroups* groups,
                            int8_t* code, float* line3D, int* nnew, int* status, void* stream);
 
+/* ------------------------------------------------------------------ redundant keyframes (LocalMapping::KeyFrameCulling)
+ * The loop of LocalMapping::KeyFrameCulling (src/LocalMapping.cc:1835-1899, monocular) for G current keyframes at once, on device
+ * pointers, enqueued on `stream` (NULL = the legacy default stream): kernels only, no allocation, copy or synchronisation, so the
+ * call can be captured into a CUDA graph.
+ *
+ * Keyframe rows of capacity cap, the layout of PLTriKeyframes.keys_un / n: keys_un [n_kf][cap] (mvKeysUn; only the octave is read),
+ * n [n_kf], mp [n_kf][cap] (GetMapPointMatches(): a map-point index or -1 for NULL), origin [n_kf] (mnId == 0) and not_erase [n_kf]
+ * (mbNotErase).  Every keyframe that observes a point held by a listed keyframe must be a row; the numbering of the rows is free. */
+typedef struct PLCullKeyframes {
+  int n_kf, cap;
+  const PLKeyPoint* keys_un; const int* n; const int* mp; const uint8_t* origin; const uint8_t* not_erase;
+} PLCullKeyframes;
+/* Map points: bad [n_mp] (isBad()) and GetObservations() as CSR: point p's observations are (obs_kf[e], obs_idx[e]) for
+ * obs_offset[p] <= e < obs_offset[p + 1], one per observing keyframe (monocular: Observations() is their number). */
+typedef struct PLCullPoints {
+  int n_mp, n_obs;
+  const uint8_t* bad; const int* obs_offset /* [n_mp + 1] */; const int* obs_kf; const int* obs_idx;   /* [n_obs] */
+} PLCullPoints;
+/* Group g walks list[offset[g]] .. list[offset[g] + count[g] - 1] (keyframe rows, GetVectorCovisibleKeyFrames() of its current
+ * keyframe, in order).  Groups are independent evaluations of the same snapshot; their list ranges must not overlap. */
+typedef struct PLCullGroups {
+  int G;
+  const int* offset; const int* count;   /* [G] */
+  int n_list; const int* list;           /* [n_list] */
+} PLCullGroups;
+/* Per list entry j: code[j] = -1 skipped (origin), 0 kept, 1 culled (nRedundantObservations > 0.9 * nMPs in double; its
+ * observations are erased for the entries after it), 2 redundant but not_erase (SetBadFlag only sets mbToBeErased); n_mps[j],
+ * n_redundant[j] = the reference's nMPs and nRedundantObservations (0 for a skipped entry).  An entry is judged on the state the
+ * culls of the entries before it leave: a point p with obs observers of which culled(p) were culled earlier has Observations() =
+ * obs - culled(p), those observers are gone, and it is bad when it was bad on input or when culled(p) >= 1 and obs - culled(p) <= 2
+ * (MapPoint::EraseObservation).  A slot counts in nMPs when its point is not bad; it is redundant when the point's Observations()
+ * > 3 and at least 3 other remaining observers see it at an octave <= the slot's octave + 1.  The caller calls SetBadFlag() on
+ * the entries with codes 1 and 2 in list order, which reproduces the reference.
+ * status[g], the first that applies: 1 the list range outside n_list or a list entry outside the table; 2 a listed keyframe's n
+ * negative or over cap; 3 a keyframe listed twice; 4 a slot of a listed keyframe naming a point outside -1 .. n_mp - 1; 5 such a
+ * point's obs_offset decreasing or outside 0 .. n_obs; 6 one of its observations naming a keyframe outside the table, an idx
+ * outside 0 .. min(n, cap) - 1 of that keyframe, or a slot that does not hold the point; else 0.  A group with a nonzero status
+ * writes nothing but status[g].
+ * PL_ERR_ARG before anything is enqueued for a NULL groups, G < 0 or n_list < 0; and, when G > 0, for a NULL kfs, points, array or
+ * output, n_mp or n_obs < 0, n_kf outside 1 .. 65536 (the culled set is one bit per row in shared memory), cap outside 1 .. 6144
+ * or n_kf * cap beyond an int.  G = 0 enqueues nothing. */
+int pl_keyframe_culling_dev(const PLCullKeyframes* kfs, const PLCullPoints* points, const PLCullGroups* groups, int8_t* code,
+                            int* n_mps, int* n_redundant, int* status, void* stream);
+
 /* ------------------------------------------------------------------ tracking a batch of frames against a fixed map
  * Tracking::TrackLocalMapWithLines (src/Tracking.cc:1491-1562) with SearchLocalPoints (:1751-1801) and SearchLocalLines
  * (:1803-1855), in localisation mode (mbOnlyTracking), for B frames at once; every intermediate stays on the device.

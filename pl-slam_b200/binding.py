@@ -1470,6 +1470,111 @@ ORBmatcher.SearchForTriangulationBatch = _search_for_triangulation_batch
 LSDmatcher.SearchForTriangulationBatch = _lsd_search_for_triangulation_batch
 
 
+# ---------------------------------------------------------------------------------------------- redundant keyframes (KeyFrameCulling)
+class PLCullKeyframes(C.Structure):
+    _fields_ = [("n_kf", C.c_int), ("cap", C.c_int), ("keys_un", vp), ("n", vp), ("mp", vp), ("origin", vp), ("not_erase", vp)]
+
+
+class PLCullPoints(C.Structure):
+    _fields_ = [("n_mp", C.c_int), ("n_obs", C.c_int), ("bad", vp), ("obs_offset", vp), ("obs_kf", vp), ("obs_idx", vp)]
+
+
+class PLCullGroups(C.Structure):
+    _fields_ = [("G", C.c_int), ("offset", vp), ("count", vp), ("n_list", C.c_int), ("list", vp)]
+
+
+def _cull_lib():
+    L = lib()
+    if not getattr(L, "_cull_types", False):
+        L.pl_keyframe_culling_dev.argtypes = [C.POINTER(PLCullKeyframes), C.POINTER(PLCullPoints), C.POINTER(PLCullGroups)] + [vp] * 5
+        L._cull_types = True
+    return L
+
+
+def pack_cull_keyframes(keyframes, cap=None):
+    """Keyframes (dicts: keys [n] KP_DTYPE (mvKeysUn; the octave is read), mp [n] (GetMapPointMatches(): map-point index or -1),
+    origin (mnId == 0), not_erase (mbNotErase)) -> host arrays in the [n_kf][cap] layout of PLCullKeyframes.  cap defaults to the
+    largest count (at least 1); slots past a keyframe's count are -1."""
+    keys, n, cap = _pad_rows([k["keys"] for k in keyframes], KP_DTYPE, (), cap, "keypoints")
+    mp, _, _ = _pad_rows([np.asarray(k["mp"], np.int32) + 1 for k in keyframes], np.int32, (), cap, "keypoints")
+    return dict(keys_un=keys, n=n, mp=mp - 1, origin=np.array([bool(k["origin"]) for k in keyframes], np.uint8),
+                not_erase=np.array([bool(k["not_erase"]) for k in keyframes], np.uint8), cap=cap)
+
+
+def pack_cull_points(points):
+    """Map points (dict: bad [n_mp], observations = per point the (keyframe row, idx) pairs of GetObservations(), in any order) ->
+    host arrays of PLCullPoints (the observations as CSR)."""
+    obs = points["observations"]
+    offset = np.zeros(len(obs) + 1, np.int32)
+    offset[1:] = np.cumsum([len(o) for o in obs])
+    flat = np.array([e for o in obs for e in o], np.int32).reshape(-1, 2)
+    return dict(bad=np.asarray(points["bad"], np.uint8).reshape(-1), obs_offset=offset, obs_kf=flat[:, 0].copy(),
+                obs_idx=flat[:, 1].copy())
+
+
+def pack_cull_groups(groups):
+    """Groups (one list of keyframe rows per current keyframe, GetVectorCovisibleKeyFrames() order) -> host arrays of PLCullGroups,
+    the lists packed end to end."""
+    count = np.array([len(g) for g in groups], np.int32)
+    offset = np.concatenate([[0], np.cumsum(count)[:-1]]).astype(np.int32) if len(groups) else np.zeros(0, np.int32)
+    return dict(offset=offset, count=count, list=np.array([int(k) for g in groups for k in g], np.int32))
+
+
+class KeyFrameCullingProblems:
+    """A batch of KeyFrameCulling groups on the device for pl_keyframe_culling_dev: the constructor takes the packed host arrays
+    (pack_cull_keyframes, pack_cull_points, pack_cull_groups; one dict each, any of their arrays may be replaced), uploads them as
+    torch CUDA tensors and allocates the outputs once; run() only enqueues the launch, so it can be captured into a CUDA graph;
+    results() waits for it and returns one dict per group: code (numpy int8, one per list entry: -1 skipped, 0 kept, 1 culled,
+    2 redundant but mbNotErase), n_mps, n_redundant (numpy int32, per entry) and status.  Outputs are pre-filled with `out_fill`."""
+
+    def __init__(self, keyframes, points, groups, out_fill=-7):
+        import torch
+        self.host = dict(k=keyframes, m=points, g=groups)
+        self.inputs = {f"k_{n}": _to_device(keyframes[n]) for n in ("keys_un", "n", "mp", "origin", "not_erase")}
+        self.inputs.update({f"m_{n}": _to_device(points[n]) for n in ("bad", "obs_offset", "obs_kf", "obs_idx")})
+        self.inputs.update({f"g_{n}": _to_device(groups[n]) for n in ("offset", "count", "list")})
+        self.G, n_list = len(groups["offset"]), len(groups["list"])
+        self.outputs = dict(code=torch.full((max(n_list, 1),), out_fill, dtype=torch.int8, device="cuda"),
+                            n_mps=torch.full((max(n_list, 1),), out_fill, dtype=torch.int32, device="cuda"),
+                            n_redundant=torch.full((max(n_list, 1),), out_fill, dtype=torch.int32, device="cuda"),
+                            status=torch.full((max(self.G, 1),), out_fill, dtype=torch.int32, device="cuda"))
+        i = lambda n: self.inputs[n].data_ptr()
+        self._k = PLCullKeyframes(len(keyframes["n"]), int(keyframes["mp"].shape[1]), i("k_keys_un"), i("k_n"), i("k_mp"), i("k_origin"),
+                                  i("k_not_erase"))
+        self._m = PLCullPoints(len(points["bad"]), len(points["obs_kf"]), i("m_bad"), i("m_obs_offset"), i("m_obs_kf"), i("m_obs_idx"))
+        self._g = PLCullGroups(self.G, i("g_offset"), i("g_count"), n_list, i("g_list"))
+        torch.cuda.synchronize()        # the uploads ran on the current stream; run() may use another one
+
+    def run(self, stream=None):
+        """The launch on `stream` (a torch.cuda.Stream; None = the legacy default stream): enqueues, does not wait."""
+        s = None if stream is None else stream.cuda_stream
+        o = {n: t.data_ptr() for n, t in self.outputs.items()}
+        check(_cull_lib().pl_keyframe_culling_dev(C.byref(self._k), C.byref(self._m), C.byref(self._g), o["code"], o["n_mps"],
+                                                  o["n_redundant"], o["status"], s))
+
+    def results(self):
+        import torch
+        torch.cuda.synchronize()
+        h = {n: t.cpu().numpy() for n, t in self.outputs.items()}
+        g = self.host["g"]
+        out = []
+        for q in range(self.G):
+            a, c = int(g["offset"][q]), int(g["count"][q])
+            sl = slice(a, a + c) if a >= 0 and c >= 0 else slice(0, 0)
+            out.append(dict(code=h["code"][sl].copy(), n_mps=h["n_mps"][sl].copy(), n_redundant=h["n_redundant"][sl].copy(),
+                            status=int(h["status"][q])))
+        return out
+
+
+def KeyFrameCullingBatch(keyframes, points, groups, stream=None):
+    """LocalMapping::KeyFrameCulling for many current keyframes in one pl_keyframe_culling_dev launch: keyframes, points and groups
+    as pack_cull_keyframes, pack_cull_points and pack_cull_groups take them.  Returns one dict per group (code, n_mps, n_redundant,
+    status); the caller calls SetBadFlag() on the entries with codes 1 and 2, in list order."""
+    b = KeyFrameCullingProblems(pack_cull_keyframes(keyframes), pack_cull_points(points), pack_cull_groups(groups))
+    b.run(stream)
+    return b.results()
+
+
 # ---------------------------------------------------------------------------------------------- tracking against a fixed map
 class PLMapDesc(C.Structure):
     _fields_ = [("n_points", C.c_int), ("pt_pos", vp), ("pt_normal", vp), ("pt_min_dist", vp), ("pt_max_dist", vp), ("pt_desc", vp),
