@@ -214,6 +214,12 @@ int pl_line_debug_order(PLLine* h, int frame, unsigned* out, int cap);
 int pl_line_debug_seed_path(PLLine* h);
 /* fill every byte of the seed order and of its lengths with `byte` (tests: a later call must rewrite all it reports) */
 int pl_line_debug_fill_order(PLLine* h, int byte);
+/* Test-only: the library's own device build of the float libm restatements and of the 4x4 SVD, one thread per argument on
+ * `stream`, all arrays DEVICE pointers of n entries.  fn 0: out0 = atan2f(a, b); fn 1: out0, out1 = sinf(a), cosf(a) (|a| < 120);
+ * fn 2: out0 = logf(a) (positive normal a); b and out1 are read / written only where fn uses them.  pl_debug_svd4_dev: w [n][4]
+ * and vt [n][4][4] of cv::SVD::compute(A [n][4][4] row-major CV_32F, MODIFY_A | FULL_UV). */
+int pl_debug_float_math_dev(int fn, const float* a, const float* b, int n, float* out0, float* out1, void* stream);
+int pl_debug_svd4_dev(const float* A, int n, float* w, float* vt, void* stream);
 
 /* ------------------------------------------------------------------ per-frame front-end pipeline (batch of frames)
  * The hot-path calls Tracking makes for one frame (SURVEY.md §3.1), chained on one stream with all intermediates in

@@ -27,6 +27,11 @@ __device__ __forceinline__ bool project(const FrustumArgs& A, const float* Pc, f
   if (v < A.bounds[1] || v > A.bounds[3]) return false;
   return true;
 }
+// MapPoint / MapLine::PredictScale before any clamp (MapPoint.cc:413-428, MapLine.cpp:395-404): ceil(log(maxDist / dist) /
+// logScaleFactor) with fp32 operands and glibc's logf, so a ratio on a level boundary lands on the reference's side of it
+__device__ __forceinline__ int predict_scale_level(float maxDist, float dist, float logScaleFactor) {
+  return (int)ceilf(__fdiv_rn(glibc::logf_(__fdiv_rn(maxDist, dist)), logScaleFactor));
+}
 // true = mbTrackInView; then {u, v} = {mTrackProjX, mTrackProjY}, level = mnTrackScaleLevel, viewCos = mTrackViewCos
 __device__ __forceinline__ bool frustum_point(const FrustumArgs& A, const float* pos, const float* normal, float minDist, float maxDist,
                                               float& u, float& v, int& level, float& viewCos) {
@@ -39,8 +44,7 @@ __device__ __forceinline__ bool frustum_point(const FrustumArgs& A, const float*
   if (dist < __fmul_rn(0.8f, minDist) || dist > __fmul_rn(1.2f, maxDist)) return false;   // Get{Min,Max}DistanceInvariance (MapPoint.cc:384-394)
   viewCos = (float)(((double)PO[0] * normal[0] + (double)PO[1] * normal[1] + (double)PO[2] * normal[2]) / dist);
   if (viewCos < A.viewingCosLimit) return false;
-  const float ratio = __fdiv_rn(maxDist, dist);
-  int nScale = (int)ceilf(__fdiv_rn(glibc::logf_(ratio), A.logScaleFactor));
+  int nScale = predict_scale_level(maxDist, dist, A.logScaleFactor);
   if (nScale < 0) nScale = 0; else if (nScale >= A.nScaleLevels) nScale = A.nScaleLevels - 1;
   level = nScale;
   return true;
@@ -62,9 +66,8 @@ __device__ __forceinline__ bool frustum_line(const FrustumArgs& A, const double*
   const float pn[3] = {(float)normal[0], (float)normal[1], (float)normal[2]};
   viewCos = (float)(((double)OM[0] * pn[0] + (double)OM[1] * pn[1] + (double)OM[2] * pn[2]) / dist);
   if (viewCos < A.viewingCosLimit) return false;
-  const float ratio = __fdiv_rn(maxDist, dist);
   proj[0] = u1; proj[1] = v1; proj[2] = u2; proj[3] = v2;
-  level = (int)ceilf(__fdiv_rn(glibc::logf_(ratio), A.logScaleFactor));
+  level = predict_scale_level(maxDist, dist, A.logScaleFactor);
   return true;
 }
 }  // namespace pl

@@ -15,7 +15,8 @@
 //                    lies within 1e-16 of an fp32 rounding boundary: a 1e-8 event).
 // tests/test_libm_glibc.py compiles this header for the host and compares it with the running libm on 2e7 random arguments plus
 // the special values: zero mismatches.  Only the argument ranges the path produces are covered (finite, |x| < 120 for sincosf);
-// the device build relies on -fmad=false (pl-slam_b200/csrc/Makefile) so that no other product is contracted.
+// the device build relies on -fmad=false (pl-slam_b200/csrc/Makefile) so that no other product is contracted, and
+// tests/test_float_math_gpu.py compares it with the host build and the running libm on the same arguments.
 #pragma once
 #include <math.h>
 #include <stdint.h>

@@ -18,7 +18,7 @@
 
 #include "common.cuh"
 #include "search.cuh"
-#include "libm_glibc.cuh"
+#include "frustum.cuh"
 #include <climits>
 #include <vector>
 
@@ -364,8 +364,7 @@ __global__ void __launch_bounds__(32) k_search_proj_last(ProjLastArgs A) {
       const float p0 = __fsub_rn(X[0], A.Ow[0]), p1 = __fsub_rn(X[1], A.Ow[1]), p2 = __fsub_rn(X[2], A.Ow[2]);
       const float dist3D = (float)sqrt((double)p0 * p0 + (double)p1 * p1 + (double)p2 * p2);
       if (dist3D < __fmul_rn(0.8f, A.min_dist[lb + i]) || dist3D > __fmul_rn(1.2f, A.max_dist[lb + i])) continue;   // invariance range; PredictScale below uses the raw mfMaxDistance
-      const float ratio = __fdiv_rn(A.max_dist[lb + i], dist3D);
-      oct = (int)ceilf(__fdiv_rn(glibc::logf_(ratio), A.logSF));
+      oct = predict_scale_level(A.max_dist[lb + i], dist3D, A.logSF);
       if (oct < 0) oct = 0; else if (oct >= A.nlevels) oct = A.nlevels - 1;
     } else oct = A.last_octave[lb + i];
     const float radius = __fmul_rn(A.th, A.scaleFactors[oct]);
@@ -998,8 +997,7 @@ __global__ void __launch_bounds__(32 * kFuseWarps) k_fuse_search(const __grid_co
         if (go) {
           const double dot = (double)PO[0] * L.normal[3 * i] + (double)PO[1] * L.normal[3 * i + 1] + (double)PO[2] * L.normal[3 * i + 2];
           go = !(dot < 0.5 * (double)dist3D);
-          const float ratio = __fdiv_rn(L.max_dist[i], dist3D);
-          lvl = (int)ceilf(__fdiv_rn(glibc::logf_(ratio), K.log_scale_factor));
+          lvl = predict_scale_level(L.max_dist[i], dist3D, K.log_scale_factor);
           if (lvl < 0) lvl = 0; else if (lvl >= K.nlevels) lvl = K.nlevels - 1;
         }
       }
@@ -1152,8 +1150,7 @@ __device__ void line_fuse_one(const FuseCam& cam, const KeyLine68* kls, int nl, 
   const float pn[3] = {(float)L.normal[3 * i], (float)L.normal[3 * i + 1], (float)L.normal[3 * i + 2]};
   const double dot = (double)OM[0] * pn[0] + (double)OM[1] * pn[1] + (double)OM[2] * pn[2];
   if (dot < 0.5 * (double)dist) return;
-  const float ratio = __fdiv_rn(L.max_dist[i], dist);
-  const int lvl = (int)ceilf(__fdiv_rn(glibc::logf_(ratio), logScaleFactorLine));
+  const int lvl = predict_scale_level(L.max_dist[i], dist, logScaleFactorLine);
   float sf = 1.0f;
   if (lvl >= 0) { for (int k = 0; k < lvl; k++) sf = __fmul_rn(sf, scale_line); }
   else { for (int k = 0; k < -lvl; k++) sf = __fmul_rn(sf, scale_line); sf = __fdiv_rn(1.0f, sf); }

@@ -17,7 +17,8 @@
 // U (the normalised At rows, and FULL_UV's completion of the rows that belong to zero singular values) is not formed: no input
 // to w or V depends on it.  tests/test_triangulate_svd.py compiles this header for the host and compares w and the whole of vt
 // with cv2.SVDecomp, stored in tests/golden/orb_cv2_svd4.npz (and live where cv2 imports).
-// On the device every operation is the _rn intrinsic, so no product is contracted whatever -fmad says.
+// On the device every operation is the _rn intrinsic, so no product is contracted whatever -fmad says; tests/test_float_math_gpu.py
+// compares the device build with cv2 on the fixture and with the host build on fresh matrices.
 #pragma once
 #include "libm_glibc.cuh"
 

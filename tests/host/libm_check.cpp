@@ -2,50 +2,22 @@
 // Prints "mismatches <atan2f> <sinf> <cosf> <logf> of <n>"; exit code 0 only when all four are zero.
 #include <cstdio>
 #include <cstdlib>
-#include <cmath>
-#include <cstdint>
-#include "../../pl-slam_b200/csrc/libm_glibc.cuh"
-static uint64_t st = 0x9E3779B97F4A7C15ull;
-static inline uint64_t rnd() { st ^= st << 13; st ^= st >> 7; st ^= st << 17; return st; }
-static inline float urand(float lo, float hi) { return lo + (hi - lo) * (float)((rnd() >> 40) * (1.0 / 16777216.0)); }
+#include "libm_args.h"
 int main(int argc, char** argv) {
   const long n = argc > 1 ? atol(argv[1]) : 20000000;
   long bad_a = 0, bad_s = 0, bad_c = 0, bad_l = 0;
-  volatile float vy, vx;   // volatile: the compiler must call libm, not fold
+  LibmArgs args;
+  LibmCase c;
   for (long i = 0; i < n; i++) {
-    float y, x;
-    switch (i & 7) {
-      case 0: y = urand(-640.f, 640.f); x = urand(-640.f, 640.f); break;                 // end-point differences of a KeyLine
-      case 1: y = (float)((int)(rnd() % 1281) - 640); x = (float)((int)(rnd() % 1281) - 640); break;   // integers, zeros, axes
-      case 2: y = urand(-1.f, 1.f); x = urand(-1e-3f, 1e-3f); break;
-      case 3: y = urand(-1e-3f, 1e-3f); x = urand(-1.f, 1.f); break;
-      case 4: y = urand(-2000.f, 2000.f) * 0.25f; x = urand(-2000.f, 2000.f) * 0.25f; break;
-      case 5: y = pl::glibc::u2f((uint32_t)rnd() & 0xbfffffffu); x = pl::glibc::u2f((uint32_t)rnd() & 0xbfffffffu); break;   // any finite bit pattern below 2
-      default: y = urand(-10.f, 10.f); x = urand(-10.f, 10.f); break;
-    }
-    if (!std::isfinite(y) || !std::isfinite(x)) continue;
-    vy = y; vx = x;
-    const float a = atan2f(vy, vx), b = pl::glibc::atan2f_(y, x);
-    if (pl::glibc::f2u(a) != pl::glibc::f2u(b)) { if (bad_a < 5) fprintf(stderr, "atan2f(%a, %a): libm %a here %a\n", y, x, a, b); bad_a++; }
-    // angles: atan2f results, degrees * pi/180 in [0, 2 pi), and anything below 120
-    float t = (i & 1) ? a : ((i & 2) ? urand(0.f, 360.f) * (float)(3.14159265358979323846 / 180.f) : urand(-119.f, 119.f));
-    vy = t;
-    float s0, c0, s1, c1;
-    sincosf(vy, &s0, &c0);
-    pl::glibc::sincosf_(t, &s1, &c1);
-    if (pl::glibc::f2u(s0) != pl::glibc::f2u(s1)) { if (bad_s < 5) fprintf(stderr, "sinf(%a): libm %a here %a\n", t, s0, s1); bad_s++; }
-    if (pl::glibc::f2u(c0) != pl::glibc::f2u(c1)) { if (bad_c < 5) fprintf(stderr, "cosf(%a): libm %a here %a\n", t, c0, c1); bad_c++; }
-    // logf: distance ratios around 1 (PredictScale), powers of the scale factor, and any positive normal float
-    float q;
-    switch (i & 3) {
-      case 0: q = urand(0.05f, 20.f); break;
-      case 1: q = powf(1.2f, (float)((int)(rnd() % 17) - 8)) * (1.0f + urand(-2e-6f, 2e-6f)); break;
-      case 2: q = pl::glibc::u2f(0x00800000u + (uint32_t)(rnd() % (0x7f800000u - 0x00800000u))); break;
-      default: q = urand(0.5f, 2.f); break;
-    }
-    vy = q;
-    const float l0 = logf(vy), l1 = pl::glibc::logf_(q);
-    if (pl::glibc::f2u(l0) != pl::glibc::f2u(l1)) { if (bad_l < 5) fprintf(stderr, "logf(%a): libm %a here %a\n", q, l0, l1); bad_l++; }
+    if (!args.next(i, c)) continue;
+    const float b = pl::glibc::atan2f_(c.y, c.x);
+    if (pl::glibc::f2u(c.atan2) != pl::glibc::f2u(b)) { if (bad_a < 5) fprintf(stderr, "atan2f(%a, %a): libm %a here %a\n", c.y, c.x, c.atan2, b); bad_a++; }
+    float s1, c1;
+    pl::glibc::sincosf_(c.t, &s1, &c1);
+    if (pl::glibc::f2u(c.sin) != pl::glibc::f2u(s1)) { if (bad_s < 5) fprintf(stderr, "sinf(%a): libm %a here %a\n", c.t, c.sin, s1); bad_s++; }
+    if (pl::glibc::f2u(c.cos) != pl::glibc::f2u(c1)) { if (bad_c < 5) fprintf(stderr, "cosf(%a): libm %a here %a\n", c.t, c.cos, c1); bad_c++; }
+    const float l1 = pl::glibc::logf_(c.q);
+    if (pl::glibc::f2u(c.log) != pl::glibc::f2u(l1)) { if (bad_l < 5) fprintf(stderr, "logf(%a): libm %a here %a\n", c.q, c.log, l1); bad_l++; }
   }
   printf("mismatches %ld %ld %ld %ld of %ld\n", bad_a, bad_s, bad_c, bad_l, n);
   return (bad_a || bad_s || bad_c || bad_l) ? 1 : 0;

@@ -7,6 +7,7 @@ import torch
 import oracle
 import plslam_b200 as pl
 from plslam_b200 import synth
+from predict_scale_cases import boundary_set
 
 pytestmark = pytest.mark.gpu
 G = np.load(os.path.join(os.path.dirname(__file__), "golden", "frame_cv2.npz"))
@@ -131,3 +132,28 @@ def test_is_in_frustum_predicted_level_on_boundaries():
     f64 = np.clip(np.ceil(np.log(ratio.astype(np.float64)) / np.float64(np.float32(log_sf))), 0, 7).astype(np.int32)
     inv = want[0].astype(bool)
     assert (f64[inv] != want[2][inv]).sum() > 0        # the fp64 formula of round 1 would have failed here
+
+
+def test_is_in_frustum_lines_predicted_level_on_boundaries():
+    """MapLine::PredictScale on the boundary set the reference's own PredictScale is checked on (tests/predict_scale_cases.py):
+    segments of 2 mm across the optical axis at depth d, seen from Tcw = I, so the midpoint distance is d exactly.
+    MapLine::PredictScale does not clamp (MapLine.cpp:395-404); clamped to the 8 levels, its level must be MapPoint's answer."""
+    dist, mx, log_sf = boundary_set()
+    n = len(dist)
+    pos = np.zeros((n, 6)); pos[:, 0], pos[:, 3] = -1e-3, 1e-3; pos[:, 2] = pos[:, 5] = dist
+    normal = np.zeros((n, 3)); normal[:, 2] = 1.0
+    mn = (mx / np.float32(1.2) ** 10).astype(np.float32)
+    b = oracle.image_bounds(synth.TUM1_K, synth.TUM1_DIST, 640, 480)
+    a = (np.eye(4, dtype=np.float32), np.zeros(3, np.float32), synth.TUM1_K, b, float(log_sf), 0.5, pos, normal, mn, mx)
+    want = oracle.is_in_frustum_lines(*a); got = pl.isInFrustumLines(*a)
+    for name, g, w_ in zip(("in view", "projection", "level", "viewing cosine"), got, want):
+        assert np.array_equal(g, w_), f"{name}: {(g != w_).reshape(n, -1).any(1).sum()} of {n} segments differ from the oracle"
+    inv = want[0].astype(bool)
+    assert inv[:n // 2].all() and inv.sum() > 150000
+    level = got[2]
+    assert (level[inv] > 7).any(), "raw levels beyond the last one: the clamp is the caller's"
+    ref = oracle.ref_predict_scale(dist, mx, log_sf, 8)
+    assert np.array_equal(np.clip(level, 0, 7)[inv], ref[inv])
+    ratio = (mx / dist).astype(np.float32)
+    f64 = np.clip(np.ceil(np.log(ratio.astype(np.float64)) / np.float64(log_sf)), 0, 7).astype(np.int32)
+    assert (f64[inv] != ref[inv]).sum() > 0

@@ -11,6 +11,7 @@ from plslam_b200 import synth
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 from test_localmap2 import _mp_lists  # noqa: E402
+from predict_scale_cases import boundary_set  # noqa: E402
 
 pytestmark = pytest.mark.skipif(not oracle.ref_match_available(), reason="oracle/_ref/libref_match.so not built (needs /root/reference)")
 BOUNDS = [0.0, 0.0, 640.0, 480.0]
@@ -142,15 +143,8 @@ def test_distinctive_descriptors():
 
 
 def test_predict_scale():
-    rng = np.random.default_rng(1)
-    n = 200000
-    max_dist = rng.uniform(2.0, 12.0, n).astype(np.float32)
-    dist = (max_dist / rng.uniform(0.5, 6.0, n)).astype(np.float32)
     # exact level boundaries and their fp32 neighbours: where logf / the fp32 quotient decide the level
-    k = np.arange(n // 2) % 9
-    edge = (max_dist[:n // 2] / (np.float32(1.2) ** k.astype(np.float32))).astype(np.float32)
-    dist[:n // 2] = np.nextafter(edge, np.where(np.arange(n // 2) % 3 == 0, np.float32(0), np.where(np.arange(n // 2) % 3 == 1, np.float32(1e9), edge)).astype(np.float32))
-    log_sf = np.float32(np.log(np.float32(1.2)))
+    dist, max_dist, log_sf = boundary_set()
     ref = oracle.ref_predict_scale(dist, max_dist, log_sf, 8)
     got = oracle.predict_scale(dist, max_dist, log_sf, 8)
     assert np.array_equal(ref, got)
