@@ -220,6 +220,18 @@ int pl_line_debug_fill_order(PLLine* h, int byte);
  * and vt [n][4][4] of cv::SVD::compute(A [n][4][4] row-major CV_32F, MODIFY_A | FULL_UV). */
 int pl_debug_float_math_dev(int fn, const float* a, const float* b, int n, float* out0, float* out1, void* stream);
 int pl_debug_svd4_dev(const float* A, int n, float* w, float* vt, void* stream);
+/* Test-only: LSD region growing's tables and alignment decisions, as a line handle's frames use them.
+ * pl_line_debug_tables copies the handle's tables to host arrays (NULL = skip): gtab [1021 * 1021][4] floats {deg, cos, sin, 0}
+ * and gtab_seed [1021 * 1021][2] {cos, sin} for the gradient (gx, gy) at (gx + 510) * 1021 + gy + 510, wtab [2 * 510^2 + 1]
+ * doubles sqrt(i / 4).  pl_debug_lsd_align_dev (DEVICE arrays of n): out[i] bit 0 = the shortcut's "surely aligned", bit 1 its
+ * "maybe aligned", bit 2 the exact test, bit 3 the generic isAligned, for the region sum (sumdx, sumdy) and the candidate of
+ * gradient (gx, gy); bit 4 flags |gx| or |gy| > 510 (the decisions then use the clamped gradient).  pl_debug_lsd_fold_dev:
+ * bit 0 the exact test, bit 1 the generic isAligned, for the region angle reg_deg and the candidate angle deg in degrees.
+ * NULL stream = the handle's stream. */
+int pl_line_debug_tables(PLLine* h, float* gtab, float* gtab_seed, double* wtab);
+int pl_debug_lsd_align_dev(PLLine* h, int n, const float* sumdx, const float* sumdy, const int* gx, const int* gy, uint8_t* out,
+                           void* stream);
+int pl_debug_lsd_fold_dev(PLLine* h, int n, const float* reg_deg, const float* deg, uint8_t* out, void* stream);
 
 /* ------------------------------------------------------------------ per-frame front-end pipeline (batch of frames)
  * The hot-path calls Tracking makes for one frame (SURVEY.md §3.1), chained on one stream with all intermediates in

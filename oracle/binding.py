@@ -540,6 +540,22 @@ def lsd_detect(img, order_mode=1):
     return out[:n].copy()
 
 
+LSD_ADDENDS = {"cosf": 0, "cos_rounded": 1, "cos_double": 2}
+
+
+def lsd_detect_scale1(img, addend="cosf"):
+    """cv::createLineSegmentDetector(LSD_REFINE_STD, 1.0)->detect(img): regions grown on the image itself, no blur or resize,
+    so every gradient in [-510, 510]^2 a 2x2 window can have is reachable.  addend: what region_grow adds to its float sums per
+    pixel - libm's cosf / sinf of float(angle) (lsd.cpp's cos(float), the default), the fp64 functions rounded to fp32, or the
+    fp64 functions added in fp64 to the float sum"""
+    img = np.ascontiguousarray(img, np.uint8)
+    cap = 20000
+    out = np.zeros((cap, 4), np.float32)
+    n = lib().oracle_lsd_detect_scale1(_p(img), img.shape[1], img.shape[0], LSD_ADDENDS[addend], _p(out), cap)
+    assert n >= 0
+    return out[:n].copy()
+
+
 def lsd_stages(img):
     img = np.ascontiguousarray(img, np.uint8)
     sw, sh = C.c_int(), C.c_int()

@@ -104,8 +104,11 @@ struct NormPoint { int px, py, norm; };
 
 thread_local long g_stat[8] = {0};  // debug statistics: region_grow calls, points added, regions >= min size, refine regrows, ...
 
+// what region_grow adds to its float sums per pixel: lsd.cpp's  sumdx += cos(float(angle))  read three ways
+enum { kAddCosf = 0, kAddCosRounded = 1, kAddCosDouble = 2 };
+
 struct Lsd {
-  int w = 0, h = 0, order_mode = 0;
+  int w = 0, h = 0, order_mode = 0, addend = kAddCosf;
   std::vector<uint8_t> scaled, used;
   std::vector<double> angles, modgrad;
   std::vector<NormPoint> ordered;
@@ -186,8 +189,14 @@ struct Lsd {
             rp.x = xx; rp.y = yy; rp.modgrad = modgrad[(size_t)yy * w + xx]; rp.angle = angle;
             reg.push_back(rp);
             g_stat[1]++;
-            sumdx += cosf(float(angle));
-            sumdy += sinf(float(angle));
+            // lsd.cpp adds cos(float(angle)), sin(float(angle)).  kAddCosf (the default): <cmath>'s float overloads, libm's cosf /
+            // sinf; kAddCosRounded: the fp64 functions rounded to fp32; kAddCosDouble: ::cos(double) added in fp64 to the float sum.
+            // They differ in the last bit on 1.3 % of the gradients; tests/test_oracle_lsd_knife_edge.py holds cv2 to kAddCosf on
+            // images where the three give different segment lists (tools/gen_lsd_knife_edge.py)
+            const float af = float(angle);
+            if (addend == kAddCosf) { sumdx += cosf(af); sumdy += sinf(af); }
+            else if (addend == kAddCosRounded) { sumdx += float(std::cos(double(af))); sumdy += float(std::sin(double(af))); }
+            else { sumdx = float(double(sumdx) + std::cos(double(af))); sumdy = float(double(sumdy) + std::sin(double(af))); }
             reg_angle = fast_atan2(sumdy, sumdx) * DEG_TO_RADS;
           }
         }
@@ -284,15 +293,20 @@ struct Lsd {
     return true;
   }
 
-  // cv::LineSegmentDetector::detect on an 8-bit image -> Vec4f list
-  void detect(const uint8_t* img, int iw, int ih, std::vector<float>& lines) {
-    const double ANG_TH = 22.5, QUANT = 2.0, SCALE = 0.8, DENSITY_TH = 0.7;
+  // cv::LineSegmentDetector::detect on an 8-bit image -> Vec4f list.  scale1: the detector made with scale 1.0, which grows
+  // regions on the image itself (no blur, no resize)
+  void detect(const uint8_t* img, int iw, int ih, std::vector<float>& lines, bool scale1 = false) {
+    const double ANG_TH = 22.5, QUANT = 2.0, SCALE = scale1 ? 1.0 : 0.8, DENSITY_TH = 0.7;
     const unsigned N_BINS = 1024;
     const double prec = PI_ * ANG_TH / 180, p = ANG_TH / 180, rho = QUANT / std::sin(prec);
-    std::vector<uint8_t> g((size_t)iw * ih);
-    static const int taps[7] = {0, 4, 56, 136, 56, 4, 0};  // GaussianBlur 7x7, sigma 0.6/0.8 = 0.75, 8.8 fixed point
-    blur_sep_u8(img, iw, ih, g.data(), taps, 7);
-    resize_08_exact(g.data(), iw, ih, scaled, w, h);
+    if (scale1) {
+      scaled.assign(img, img + (size_t)iw * ih); w = iw; h = ih;
+    } else {
+      std::vector<uint8_t> g((size_t)iw * ih);
+      static const int taps[7] = {0, 4, 56, 136, 56, 4, 0};  // GaussianBlur 7x7, sigma 0.6/0.8 = 0.75, 8.8 fixed point
+      blur_sep_u8(img, iw, ih, g.data(), taps, 7);
+      resize_08_exact(g.data(), iw, ih, scaled, w, h);
+    }
     ll_angle(rho, N_BINS);
     const double LOG_NT = 5 * (std::log10(double(w)) + std::log10(double(h))) / 2 + std::log10(11.0);
     const size_t min_reg_size = size_t(-LOG_NT / std::log10(p));
@@ -506,6 +520,19 @@ int oracle_lsd_detect(const uint8_t* img, int w, int h, int order_mode, float* l
   l.order_mode = order_mode;
   std::vector<float> v;
   l.detect(img, w, h, v);
+  int n = (int)v.size() / 4;
+  memcpy(lines, v.data(), sizeof(float) * 4 * std::min(n, cap));
+  return n;
+}
+// the same with scale 1.0 (cv::createLineSegmentDetector(LSD_REFINE_STD, 1.0)): regions grown on the image itself; addend:
+// what region_grow adds to its sums (kAddCosf, the default, kAddCosRounded or kAddCosDouble)
+int oracle_lsd_detect_scale1(const uint8_t* img, int w, int h, int addend, float* lines, int cap) {
+  if (addend < kAddCosf || addend > kAddCosDouble) return -1;
+  Lsd l;
+  l.order_mode = 1;
+  l.addend = addend;
+  std::vector<float> v;
+  l.detect(img, w, h, v, true);
   int n = (int)v.size() / 4;
   memcpy(lines, v.data(), sizeof(float) * 4 * std::min(n, cap));
   return n;

@@ -96,20 +96,23 @@ __device__ __forceinline__ double dist_sq(double x1, double y1, double x2, doubl
 constexpr float kNotDefDeg = -1024.f;
 // The level-line record of a pixel depends only on its integer gradient (gx, gy) in [-510, 510]^2: the angle in degrees
 // (cv::fastAtan2(gx, -gy)), cos/sin of that angle as region_grow adds them, and the cos/sin a region SEEDED there starts
-// from.  The fp64 sincos behind them is the whole cost of the gradient pass, so it is evaluated once per (gx, gy) into a
+// from.  The trigonometry behind them is the whole cost of the gradient pass, so it is evaluated once per (gx, gy) into a
 // 25 MB table at handle creation (L2-resident, the hot entries are the small gradients) and the per-frame kernel is loads.
 constexpr int kGradR = 510, kGradN = 2 * kGradR + 1;
 struct GradRec { float deg, c, s, pad; };
 __device__ __forceinline__ void grad_record(int gx, int gy, GradRec& rec, float2& scs) {
   const float deg = fast_atan2_deg((float)gx, (float)(-gy));
-  const double af = (double)(float)((double)deg * kDegToRads);
-  double sn, cs;
-  sincos(af, &sn, &cs);
-  rec.deg = deg; rec.c = (float)cs; rec.s = (float)sn; rec.pad = 0.f;
-  // a region SEEDED here starts from cos/sin of the fp64 angle ad = af + dl, |dl| <= half an fp32 ulp (< 4e-7):
-  // angle-addition with cos(dl) = 1 - dl^2/2, sin(dl) = dl is exact to ~1e-27, far below fp64 rounding
-  const double ad = (double)deg * kDegToRads, dl = ad - af, h2 = 1.0 - 0.5 * dl * dl;
-  scs = make_float2((float)(cs * h2 - sn * dl), (float)(sn * h2 + cs * dl));
+  const double ad = (double)deg * kDegToRads;
+  // region_grow adds cos(float(angle)), sin(float(angle)): <cmath>'s float overloads, libm's cosf / sinf (not correctly rounded:
+  // they differ from the rounded fp64 functions on about 1.3 % of the gradients; tests/test_oracle_lsd_knife_edge.py pins cv2 to
+  // cosf on images where the readings give different segments)
+  float sn, cs;
+  glibc::sincosf_((float)ad, &sn, &cs);
+  rec.deg = deg; rec.c = cs; rec.s = sn; rec.pad = 0.f;
+  // a region SEEDED here starts from float(std::cos(ad)), float(std::sin(ad)) of the fp64 angle
+  double sd, cd;
+  sincos(ad, &sd, &cd);
+  scs = make_float2((float)cd, (float)sd);
 }
 __global__ void __launch_bounds__(256) k_lsd_grad_table(GradRec* __restrict__ T, float2* __restrict__ TS) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1085,3 +1088,59 @@ extern "C" int pl_line_grow_stats(unsigned long long* out, int reset) {
   return 0;
 }
 #endif
+
+// ------------------------------------------------------------------------------------------------ test-only entry points
+// the handle's own tables, what every frame reads: the level-line records and seed cos/sin of (gx, gy) at index
+// (gx + 510) * 1021 + (gy + 510), and the gradient magnitudes sqrt(s / 4), s = 0 .. 2 * 510^2
+extern "C" int pl_line_debug_tables(PLLine* h, float* gtab, float* gtab_seed, double* wtab) {
+  PL_ARG(h);
+  PL_CUDA(cudaStreamSynchronize(h->stream));
+  const size_t n = (size_t)kGradN * kGradN;
+  if (gtab) PL_CUDA(cudaMemcpy(gtab, h->d_gtab, n * sizeof(GradRec), cudaMemcpyDeviceToHost));
+  if (gtab_seed) PL_CUDA(cudaMemcpy(gtab_seed, h->d_gtab_seed, n * sizeof(float2), cudaMemcpyDeviceToHost));
+  if (wtab) PL_CUDA(cudaMemcpy(wtab, h->d_wtab, (size_t)(2 * kGradR * kGradR + 1) * sizeof(double), cudaMemcpyDeviceToHost));
+  return PL_OK;
+}
+namespace pl {
+namespace {
+// region_grow's decisions for a region sum (sumdx, sumdy) and the candidate whose gradient is (gx, gy), its record read from
+// the handle's table: bit 0 sure, bit 1 maybe (ord::align_shortcut), bit 2 the exact test (ord::aligned_fold of the angle
+// fastAtan2(sumdy, sumdx)), bit 3 the generic isAligned of the same two angles, bit 4 (gx, gy) outside [-510, 510]^2
+__global__ void k_debug_lsd_align(LineParams P, const GradRec* __restrict__ T, const float* sx, const float* sy, const int* gx,
+                                  const int* gy, int n, uint8_t* out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  // a gradient outside the table reads a clamped entry and is flagged (bit 4) instead of reading past the allocation
+  const bool out_of_range = gx[i] < -kGradR || gx[i] > kGradR || gy[i] < -kGradR || gy[i] > kGradR;
+  const GradRec r = T[(min(max(gx[i], -kGradR), kGradR) + kGradR) * kGradN + min(max(gy[i], -kGradR), kGradR) + kGradR];
+  bool sure, maybe;
+  ord::align_shortcut(sx[i], sy[i], make_float2(r.c, r.s), ord::Sure{P.sure_ca2, P.sure_cn2}, sure, maybe);
+  const double reg = (double)fast_atan2_deg(sy[i], sx[i]) * kDegToRads, a = (double)r.deg * kDegToRads;
+  out[i] = (uint8_t)(sure | (maybe << 1) | (ord::aligned_fold(reg, a, P.prec, P.prec_hi) << 2) |
+                     (ord::is_aligned_generic(a, reg, P.prec) << 3) | (out_of_range << 4));
+}
+// the exact test alone on given float angles in degrees: bit 0 aligned_fold, bit 1 is_aligned_generic
+__global__ void k_debug_lsd_fold(LineParams P, const float* reg_deg, const float* deg, int n, uint8_t* out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const double reg = (double)reg_deg[i] * kDegToRads, a = (double)deg[i] * kDegToRads;
+  out[i] = (uint8_t)(ord::aligned_fold(reg, a, P.prec, P.prec_hi) | (ord::is_aligned_generic(a, reg, P.prec) << 1));
+}
+}  // namespace
+}  // namespace pl
+extern "C" int pl_debug_lsd_align_dev(PLLine* h, int n, const float* sumdx, const float* sumdy, const int* gx, const int* gy,
+                                      uint8_t* out, void* stream) {
+  PL_ARG(h && n >= 0 && (n == 0 || (sumdx && sumdy && gx && gy && out)));
+  if (n == 0) return PL_OK;
+  k_debug_lsd_align<<<(n + 255) / 256, 256, 0, stream ? (cudaStream_t)stream : (cudaStream_t)h->stream>>>(h->P, h->d_gtab, sumdx, sumdy, gx, gy,
+                                                                                                    n, out);
+  PL_LAUNCH_CHECK();
+  return PL_OK;
+}
+extern "C" int pl_debug_lsd_fold_dev(PLLine* h, int n, const float* reg_deg, const float* deg, uint8_t* out, void* stream) {
+  PL_ARG(h && n >= 0 && (n == 0 || (reg_deg && deg && out)));
+  if (n == 0) return PL_OK;
+  k_debug_lsd_fold<<<(n + 255) / 256, 256, 0, stream ? (cudaStream_t)stream : (cudaStream_t)h->stream>>>(h->P, reg_deg, deg, n, out);
+  PL_LAUNCH_CHECK();
+  return PL_OK;
+}

@@ -104,6 +104,19 @@ __device__ __forceinline__ bool is_aligned_generic(double a, double theta, doubl
 // rounding is < 1e-4 degrees, so with a margin M = 0.05 degrees:  D <= prec - M  implies the exact test says aligned, D >= prec + M
 // implies it says not aligned.  Only candidates inside the 2M band need the exact arctangent (kSure.ca2 / cn2 = cos^2(prec -/+ M)).
 struct Sure { float ca2, cn2; };
+// sure: D <= prec - M, the exact test says aligned; !maybe: D >= prec + M (or the candidate faces away), it says not aligned.
+// (|sum| >= 1 in region_grow: the seed is a unit vector and every added unit vector is within prec < 90 degrees of the sum)
+__device__ __forceinline__ void align_shortcut(float sumdx, float sumdy, float2 cs, Sure sure, bool& sure_al, bool& maybe) {
+  const float n2 = __fmaf_rn(sumdx, sumdx, __fmul_rn(sumdy, sumdy));
+  const float dot = __fmaf_rn(sumdx, cs.x, __fmul_rn(sumdy, cs.y)), d2 = __fmul_rn(dot, dot);
+  sure_al = dot > 0.f && d2 >= __fmul_rn(sure.ca2, n2);
+  maybe = dot > 0.f && d2 > __fmul_rn(sure.cn2, n2);
+}
+// the exact test of the fast path (prec < pi/2): isAligned folded with prec_hi, see region_grow
+__device__ __forceinline__ bool aligned_fold(double reg_angle, double a, double prec, double prec_hi) {
+  const double n1 = fabs(reg_angle - a);
+  return (n1 <= prec) || (n1 >= prec_hi);
+}
 
 // need_n: the caller reads reg_angle_out only for regions of at least this many pixels (min_reg_size in the seed loop, 2 in refine)
 template <bool kFast>
@@ -155,11 +168,8 @@ __device__ __forceinline__ int region_grow(const Ctx& C, unsigned seed, double p
       unsigned A;
       bool exact = !kFast;
       if (kFast) {
-        // (|sum| >= 1 here: the seed is a unit vector and every added unit vector is within prec < 90 degrees of the sum)
-        const float n2 = __fmaf_rn(sumdx, sumdx, __fmul_rn(sumdy, sumdy));
-        const float dot = __fmaf_rn(sumdx, csv.x, __fmul_rn(sumdy, csv.y)), d2 = __fmul_rn(dot, dot);
-        const bool sure_al = dot > 0.f && d2 >= __fmul_rn(sure.ca2, n2);
-        const bool maybe = dot > 0.f && d2 > __fmul_rn(sure.cn2, n2);       // not (surely not aligned)
+        bool sure_al, maybe;
+        align_shortcut(sumdx, sumdy, csv, sure, sure_al, maybe);
         const unsigned MB = __ballot_sync(0xffffffffu, maybe) & live;
         if (MB == 0u) break;
         const unsigned SA = __ballot_sync(0xffffffffu, sure_al);
@@ -171,7 +181,7 @@ __device__ __forceinline__ int region_grow(const Ctx& C, unsigned seed, double p
         if (dirty) { reg_angle = (double)fast_atan2_deg(sumdy, sumdx) * kDegToRads; dirty = false; }
         const double a = (double)__int_as_float(ab) * kDegToRads;
         bool al;
-        if (kFast) { const double n1 = fabs(reg_angle - a); al = (n1 <= prec) || (n1 >= prec_hi); }
+        if (kFast) al = aligned_fold(reg_angle, a, prec, prec_hi);
         else al = is_aligned_generic(a, reg_angle, prec);
         A = __ballot_sync(0xffffffffu, al) & live;
         if (!A) break;
@@ -444,8 +454,7 @@ __global__ void __launch_bounds__(32, 32) k_lsd_grow_ordered(LineParams P, int4*
           const int kq = q + (q >= 4), xx = sx + kq % 3 - 1, yy = sy + kq / 3 - 1;
           if (xx >= 0 && yy >= 0 && xx < P.sw && yy < P.sh) {
             const int4 v = ld_rec(C, yy * P.sw + xx);
-            const double n1 = fabs(a0 - (double)__int_as_float(v.y) * kDegToRads);
-            any |= (v.x == kFree) && ((n1 <= P.prec) || (n1 >= P.prec_hi));
+            any |= (v.x == kFree) && aligned_fold(a0, (double)__int_as_float(v.y) * kDegToRads, P.prec, P.prec_hi);
           }
         }
         single = !any;
